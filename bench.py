@@ -10,6 +10,8 @@ outside the hot path, SURVEY.md §8d).  Metric: megapixels of INPUT per second.
 
   python bench.py [--gpus N --steps K --warmup W]       our engine (one rank per GPU)
   python bench.py --impl reference [...]                 the reference's CPU path
+  python bench.py --dump-outputs DIR [...]               also write the last timed step's results
+                                                         (rank 0) as DIR/<name>.npy, see dump_outputs()
 
 Prints ONE JSON line on rank 0 (contract in the task statement):
   value    : K steps with inputs resident in HBM (device-timed, max over ranks)
@@ -235,6 +237,56 @@ def run_reference(args, rank, world):
     print(json.dumps(line), file=RESULT_OUT, flush=True)
 
 
+# ----------------------------------------------------------------------------- output dump
+DUMP_SEED = 20240601
+DUMP_MOSAIC_PIXELS = 1 << 20          # sampled mosaic pixels (12 MB as float32 RGB)
+DUMP_MAX_DESC_ROWS = 1 << 16          # sampled descriptor rows (32 MB as float32)
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, eng, st, fs, match_total, pairs, params, out_wh):
+    """What one timed step hands its caller, as float32 / float64 .npy files:
+      mosaic_sample    [P, 3] f32  RGB of P canvas pixels, fixed seeded choice (flat index into H x W, sorted)
+      features_count   [n]    f64  descriptors per image
+      features_coord   [N, 2] f64  keypoint coordinates of every image, back to back
+      features_desc    [D, 128] f32  descriptor rows (a fixed seeded sample of rows when N > DUMP_MAX_DESC_ROWS)
+      matches          [M, 3] f64  (pair index, row in image i, row in image j) of every pair's match list
+      match_total      [1]    f64  matches the timed step reported
+    The timed step keeps its match lists on the device and reports only their total, so the lists are
+    matched again from the step's own features after the timed region (deterministic) and must add up
+    to that total."""
+    out_dir.mkdir(parents=True, exist_ok=True)
+    rng = np.random.RandomState(DUMP_SEED)
+    ow, oh = out_wh
+    mosaic = np.empty((oh, ow, 3), np.float32)
+    eng.sync()
+    eng.dev_download(mosaic, st._d_out)
+    flat = mosaic.reshape(-1, 3)
+    pick = np.sort(rng.choice(len(flat), size=min(DUMP_MOSAIC_PIXELS, len(flat)), replace=False))
+    counts, coords, descs = [], [], []
+    for i in range(len(st._shapes)):
+        c, d = fs.download(i)
+        counts.append(len(c))
+        coords.append(c)
+        descs.append(d)
+    desc = np.concatenate(descs)
+    if len(desc) > DUMP_MAX_DESC_ROWS:
+        desc = desc[np.sort(rng.choice(len(desc), size=DUMP_MAX_DESC_ROWS, replace=False))]
+    lists = eng.match_pairs(fs, pairs, params)
+    if sum(len(m) for m in lists) != match_total:
+        raise SystemExit(f"bench.py: dumped match lists hold {sum(len(m) for m in lists)} matches, "
+                         f"the timed step reported {match_total}")
+    matches = np.concatenate([np.column_stack([np.full(len(m), k), m]) for k, m in enumerate(lists)]).astype(np.float64)
+    arrays = {"mosaic_sample": flat[pick], "features_count": np.array(counts, np.float64),
+              "features_coord": np.concatenate(coords).astype(np.float64), "features_desc": desc.astype(np.float32),
+              "matches": matches, "match_total": np.array([match_total], np.float64)}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit(f"bench.py: output dump of {total} bytes exceeds {DUMP_LIMIT_BYTES}")
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", np.ascontiguousarray(a))
+
+
 # ----------------------------------------------------------------------------- our arm
 SHARDED_TIMEOUT_S = 420          # watchdog of the N > 1 sharded legs (collectives: one failed rank would hang the rest)
 
@@ -252,6 +304,8 @@ def main():
                     help="extra BASELINE.json configs measured in the same run at N=1 (comma list of 2mb,3,4,5; "
                          "'all'; 'none').  N>1 adds the sharded config-3 leg instead.")
     ap.add_argument("--sweep-sizes", default="10000,50000,100000,500000")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (mosaic sample, features, match lists) as .npy files")
     args = ap.parse_args()
     # The contract is ONE JSON line on stdout.  Libraries chat on fd 1 (NCCL's version banner, the
     # reference's timers): keep a private handle to the real stdout for the line and point fd 1 at
@@ -264,8 +318,6 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if args.impl == "reference":
-        if args.steps > 5:
-            args.steps = 5          # bounded: each step is the full CPU workload (seconds)
         args.warmup = min(args.warmup, 1)
         run_reference(args, rank, world)
         return
@@ -315,8 +367,10 @@ def main():
             raise SystemExit("bench.py: degenerate workload (no features / matches)")
 
         # ---- value: inputs resident in HBM
-        def step_device():
-            f, _ = st.run_device(pairs, items, geom, args.bands, want_matches=False)
+        def step_device(keep=False):
+            f, total = st.run_device(pairs, items, geom, args.bands, want_matches=False)
+            if keep:
+                return f, total
             f.free()
 
         import gc
@@ -334,14 +388,18 @@ def main():
         l0 = eng.launch_count()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
-        for _ in range(args.steps):
-            step_device()
+        last = None
+        for i in range(args.steps):
+            last = step_device(keep=bool(args.dump_outputs) and rank == 0 and i == args.steps - 1)
         e1.record(stream)
         torch.cuda.synchronize()
         barrier()
         launches = eng.launch_count() - l0
         clocks = sampler.stop() if rank == 0 else None
         exact_rows = eng.match_last_exact_rows()
+        if last is not None:       # after the clock window and the timed step's match statistics are read
+            dump_outputs(Path(args.dump_outputs), eng, st, last[0], last[1], pairs, params, (out_w, out_h))
+            last[0].free()
         ms = e0.elapsed_time(e1)
         t_dev = torch.tensor([ms], device="cuda")
         if world > 1:
@@ -424,7 +482,7 @@ def main():
 
         # headline: the reference's file formats at the boundary (8-bit pixels in, cropped 8-bit
         # mosaic out; conversions and crop on the device).  Beside it one lane, and the Mat32f
-        # boundary.  The GPU box is shared: other tenants' PCIe traffic slows whole legs down for
+        # boundary.  A shared GPU host is noisy: other tenants' PCIe traffic slows whole legs down for
         # seconds at a time (seen: 2.3 -> 5+ ms/job with identical kernel times), so every leg is
         # timed in E2E_TRIALS (9) trials of `steps` jobs, interleaved with the other legs, and the MEDIAN
         # trial is reported (all trials are in the JSON line).
@@ -464,12 +522,12 @@ def main():
             ab = algorithmic_bytes(imgs, items, params, counts)
             peaks = {}
             pk = ROOT / "MEASURED_PEAKS.json"
-            peak_src = "fallback"
+            peak_src = "H100 SXM data sheet (700 W)"
             if pk.exists():
                 peaks = json.loads(pk.read_text())
                 peak_src = "measured"
-            hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-            tf_peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0)))
+            hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+            tf_peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0)))
             tot = sum(v[1] for v in prof.values())
             for name, (cnt, tms) in sorted(prof.items(), key=lambda kv: -kv[1][1]):
                 avg = tms / max(cnt, 1)
@@ -495,9 +553,10 @@ def main():
                 wi = ent.get("warp_instructions_per_launch")
                 if wi:
                     # issue-slot roofline: a kernel cannot finish before its warp instructions have gone through
-                    # the 148 x 4 schedulers (one instruction per scheduler per cycle) at the SM clock seen in this run
-                    sm_hz = float((clocks or {}).get("sm_mhz") or 1965.0) * 1e6
-                    floor_ms = wi / (148 * 4 * sm_hz) * 1e3
+                    # the SMs x 4 schedulers (one instruction per scheduler per cycle) at the SM clock seen in this run
+                    sm_hz = float((clocks or {}).get("sm_mhz") or 1980.0) * 1e6
+                    n_sm = torch.cuda.get_device_properties(local_rank).multi_processor_count
+                    floor_ms = wi / (n_sm * 4 * sm_hz) * 1e3
                     issue = {"warp_instructions": wi, "floor_ms": floor_ms, "frac": floor_ms / t["avg_ms"],
                              "source": tr_files[-1].name}
             roof = {"kernel": top, "bound": t.get("bound"), "achieved": t.get("achieved"), "peak": t.get("peak"),

@@ -1,7 +1,7 @@
 """ctypes binding of libpano_b200.so (include/pano_b200.h).
 
 There is no CPU fallback: if the CUDA library is missing this module raises at
-import, and if no B200 is visible `Engine()` raises PanoError (PANO_ERR_NO_DEVICE).
+import, and if no H100 is visible `Engine()` raises PanoError (PANO_ERR_NO_DEVICE).
 """
 from __future__ import annotations
 
@@ -36,7 +36,7 @@ def _load():
     if not LIB_PATH.exists():
         raise ImportError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). openpano_b200 has no CPU fallback.")
+            "(nvcc, sm_90a). openpano_b200 has no CPU fallback.")
     # PANO_B200_LIB: development override to A/B a differently tuned build of the same library
     lib = C.CDLL(os.environ.get("PANO_B200_LIB", str(LIB_PATH)), mode=os.RTLD_LOCAL)
     P = C.POINTER(PanoParams)

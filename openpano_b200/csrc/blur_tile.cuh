@@ -30,9 +30,9 @@ __device__ __forceinline__ BlurTile find_blur_tile(const int2* __restrict__ span
 // Register-blocked passes for compile-time half-widths C (the reference's defaults give kw = 7,
 // 13 and, in the blender's last level, 19): both passes keep a sliding window in registers so one
 // shared-memory load feeds up to 2C+1 taps, 8 outputs per thread per pass, and work on PAIRS of
-// independent outputs so that the multiplies run packed (Blackwell FMUL2, two products per
-// instruction; the adds stay scalar FADDs — ptxas would fuse a packed add into FFMA2 and change
-// the rounding).  The arithmetic per output is unchanged: tmp = 0; tmp += v[k] * tap[k], k ascending.
+// independent outputs (8-byte shared-memory accesses).  Every product is a separately rounded
+// multiply (__fmul_rn: never contracted into an FMA with the add that follows).  The arithmetic
+// per output is unchanged: tmp = 0; tmp += v[k] * tap[k], k ascending.
 //   column pass: thread = (2 adjacent columns) x (8 rows); the staged tile delivers column pairs
 //                as one 8-byte load; results go to `colbuf2` as ROW pairs: colbuf2[p][x] =
 //                (row 2p, row 2p+1) of column x, row-pair stride `csp` float2 (odd: conflict-free)
@@ -40,15 +40,7 @@ __device__ __forceinline__ BlurTile find_blur_tile(const int2* __restrict__ span
 //   store      : lane <-> column, coalesced writes by the caller
 // `grey` is the staged tile with a halo of R rows / RX columns (RX a multiple of 4, GW floats per
 // row); the column pass covers staged columns [start, start + 2*npair), start = (RX - C) & ~1.
-__device__ __forceinline__ float2 fmul2(float2 a, float t) {
-  unsigned long long ra, rb, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(rb) : "f"(t));
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
-}
+__device__ __forceinline__ float2 fmul2(float2 a, float t) { return make_float2(__fmul_rn(a.x, t), __fmul_rn(a.y, t)); }
 
 #define BLUR_COLBUF_FLOATS(C) (16 * ((((BT_W + 2 * (C) + 2) / 2) * 2) | 1) * 2)   // upper bound for any column parity
 

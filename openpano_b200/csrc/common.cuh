@@ -35,7 +35,7 @@ struct pano_ctx {
   struct CachedBlock { void* p; unsigned long long stamp; };
   std::multimap<size_t, CachedBlock> cache;        // size -> free block
   std::unordered_map<void*, size_t> live;           // blocks handed out -> their true size
-  size_t cached_bytes = 0, cache_limit = (size_t)32 << 30;   // one 64-view multiband job parks ~8 GB; the GPU has 180
+  size_t cached_bytes = 0, cache_limit = (size_t)16 << 30;   // one 64-view multiband job parks ~8 GB; an H100 has 80
   unsigned long long cache_stamp = 0;
   std::string err;
   bool profiling = false;
@@ -46,7 +46,7 @@ struct pano_ctx {
   int last_match_exact_rows = 0;   // rows the last match call had to decide exactly (gathered pass)
   int last_match_nominated_rows = 0;   // columns on demand: rows of the larger sets nominated on request
   int last_match_full_rescans = 0; // of those, rows that needed a scan of every target
-  int num_sms = 148;
+  int num_sms = 132;
   // cudaFuncSetAttribute is per device: remembered per context, never per process
   bool attr_tc = false, attr_match = false;
   int sift_cap = 0;                // per-image list capacity SIFT batches start with (grows on overflow, sticky)
@@ -78,12 +78,12 @@ int  ctx_cuda(pano_ctx* ctx, cudaError_t e, const char* what);
 // Stream-ordered device memory from the CONTEXT'S OWN pool.  Contexts sharing the device's
 // default pool hand each other freed blocks, and the allocator then makes the taking
 // stream wait for the giving stream ("internal dependencies"): concurrent stitch lanes
-// drifted from 2.3 to 5+ ms per job as their arenas started to cross over.
+// slowed down as their arenas started to cross over.
 // On top of the pool sits a per-context cache of freed blocks, matched by size (best fit within
 // 25 %): a stitch job asks for the same ~40 sizes every time, up to a 0.9 GB pyramid arena, and
-// cudaMallocFromPoolAsync was seen to block the host for 0.1 - 1.5 s a few times per second when
-// it had to re-arrange the pool's mappings for such a request — with the allocator's lock held,
-// so every other lane of the process stalled with it (profiles/r02s_e2e_pause_probe.txt).
+// cudaMallocFromPoolAsync can block the host for a long time when it has to re-arrange the
+// pool's mappings for such a request — with the allocator's lock held, so every other lane of
+// the process stalls with it.
 // Everything a context allocates is used on its one stream, so handing a block freed after its
 // last enqueued use to the next request is ordered by the stream itself.  PANO_CACHE_MB bounds
 // the cache (default 8192, 0 = off); pano_trim() gives the cached blocks back to the pool.

@@ -453,8 +453,8 @@ int pano_create(pano_ctx** out, int device, void* cuda_stream) {
   ctx->device = device;
   cudaDeviceProp prop;
   if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) { delete ctx; return ctx_cuda(nullptr, e, "cudaGetDeviceProperties"); }
-  if (prop.major < 10) {
-    int rc = ctx_fail(nullptr, PANO_ERR_NO_DEVICE, "device %d is sm_%d%d; libpano_b200 is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {   // sm_90a code runs on compute capability 9.0 only
+    int rc = ctx_fail(nullptr, PANO_ERR_NO_DEVICE, "device %d is sm_%d%d; libpano_b200 is built for sm_90a only", device, prop.major, prop.minor);
     delete ctx; return rc;
   }
   ctx->num_sms = prop.multiProcessorCount;

@@ -13,7 +13,7 @@
 //
 // Two ways to get those reductions:
 //  * tensor path (default): match_tc.cu nominates (approx best, argmin, approx
-//    second) per row on the tcgen05 tensor cores; here every row gets its exact
+//    second) per row on the tensor cores (wgmma); here every row gets its exact
 //    fp32 best distance, a certified interval for its second-best (the fp16
 //    quantisation bound), and rows whose argmin or accept/reject decision is not
 //    certain within those intervals are re-scanned exactly (k_exact_rows).  The
@@ -611,15 +611,16 @@ static int build_plan(pano_ctx* ctx, pano_featureset* fs, int n_pairs, const int
   }
   if (tcimgs) {
     // Columns on demand halve the first pass but pay a nomination launch chain in each of three
-    // rounds (~20 us a round even when empty): measured, they win from 50 k x 50 k rows in one pair
-    // (153 k block pairs, 1.81 -> 1.60 ms) and lose on 13 pairs of ~2.9 k rows (6.9 k block pairs).
+    // rounds (even when empty): they pay off on large pairs (50 k x 50 k rows = 153 k block pairs)
+    // and not on many small ones (13 pairs of ~2.9 k rows = 6.9 k block pairs).
     pl.lazy = pl.block_pairs >= 32768;
     if (const char* e = getenv("PANO_MATCH_LAZY")) pl.lazy = atoi(e) != 0;
     // a shard nominates its own rows of the smaller sets only; whatever it needs of the larger sets
     // (against ALL rows of the smaller set, matcher.cc:57-61) comes on request
     if (pl.n_shards > 1) pl.lazy = true;
     // Tail balance.  The persistent CTAs walk equal tasks round-robin, so n tasks take
-    // ceil(n / SMs) task times: 782 tasks (100 k rows) on 148 SMs waste 12 % in the last wave.
+    // ceil(n / SMs) task times: a task count just above a multiple of the SM count wastes most of
+    // the last wave.
     // Splitting every task into P column ranges (merged in k_refine) makes the waves P times finer.
     long long n1 = 0, tile_sum = 0;       // first-pass tasks, and their target tiles
     for (int k = 0; k < n_pairs; ++k) {

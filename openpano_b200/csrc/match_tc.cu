@@ -1,9 +1,9 @@
-// match_tc.cu — descriptor distance matrix on the 5th-gen tensor cores.
+// match_tc.cu — descriptor distance matrix on the Hopper tensor cores.
 //
 // The N x 128 . 128 x M contraction of the matcher (feature/matcher.cc:34-47 and
 // :57-61: every query against every target, both directions) is the one GEMM of
-// the hot path.  Here it runs as tcgen05.mma (kind::f16, fp32 accumulate in
-// TMEM) and only NOMINATES: the exact fp32 rule of the reference is then decided
+// the hot path.  Here it runs as wgmma (f16 inputs, fp32 accumulate in registers)
+// and only NOMINATES: the exact fp32 rule of the reference is then decided
 // by match.cu from certified bounds, with an exact re-scan of the few ambiguous
 // rows, so the match pairs stay bit-identical.
 //
@@ -13,29 +13,25 @@
 //     target form: [ -2*s*x     | n_hi, n_lo, 1, 1, 1, 0... ]     n = s^2*|x|^2
 // so that  q . t = s^2 * |xq - xt|^2 + 1   (>= ~1: positive floats order like
 // ints).  s is a power of two making n <= 1024 (s = 1/16 for RootSIFT, |x| = 512).
-// Rows are stored PRE-BLOCKED in the UMMA canonical K-major no-swizzle layout (8x16-byte core
-// matrices, SBO = 128 B): query rows in 128-row blocks (LBO = 2 KiB), target rows in 256-row
-// tiles (LBO = 4 KiB), so one contiguous cp.async.bulk brings a block / tile into shared memory
-// ready for the MMA.
+// Rows are stored PRE-BLOCKED in the canonical K-major no-swizzle layout of wgmma shared-memory
+// operands (8x16-byte core matrices, SBO = 128 B): query rows in 128-row blocks (LBO = 2 KiB),
+// target rows in 256-row tiles (LBO = 4 KiB), so one contiguous cp.async.bulk brings a block / tile
+// into shared memory ready for the MMA.
 //
 // Kernel k_tc_pass, persistent, one CTA per SM walking tasks = (query block of 128 rows) x (a range
 // of target tiles):
-//   warp 0   producer : cp.async.bulk of target tiles (256 rows, 72 KiB) into a 2-stage ring,
-//                       query blocks into two buffers
-//   warp 1   MMA      : 9 tcgen05.mma (M128 N256 K16) per tile into one of two 256-column TMEM
-//                       accumulator stages, tcgen05.commit -> mbarriers (N = 256: the query block
-//                       is read from shared memory once per tile and k-step; two N = 128
-//                       instructions per k-step measured 13 % slower at 100 k x 100 k)
-//   warp 2   TMEM alloc/dealloc (512 columns)
-//   warps 4-11 epilogue: two groups of four warps; group g owns the g-th 128-column half of
-//                       every accumulator stage (its own full/empty barriers), so each SM
-//                       sub-partition holds two epilogue warps and one computes while the
-//                       other waits for its tcgen05.ld.  32 columns at a time; thread = query
-//                       row keeps a running (min, argmin, second-min) with the column packed
-//                       into the low mantissa bits (3.5 ALU instructions per element: one LOP3,
-//                       2.5 VIMNMX / VIMNMX3); on long target sets a chunk whose 32-way minimum
-//                       is not below the row's running second best is skipped (0.5 per element);
-//                       the groups' results are merged through shared memory per task
+//   warpgroup 0    producer : one thread issues cp.async.bulk of target tiles (256 rows, 72 KiB) into
+//                             a 2-stage ring and of query blocks into two buffers (mbarrier transactions)
+//   warpgroups 1-2 consumers: warpgroup c owns query rows [64 c, 64 c + 64) of the block.  Per tile it
+//                             issues 2 x 9 wgmma m64n128k16 (one group per 128-column half, both read
+//                             shared memory directly), and reduces the first half while the second is
+//                             still in flight; while one warpgroup reduces, the other one's MMAs run.
+//                             A thread holds two rows x 32 columns of each half (the wgmma accumulator
+//                             layout) and keeps a running (min, argmin, second-min) per row with the
+//                             column packed into the low mantissa bits (one LOP3 and 1.5 VIMNMX per
+//                             element); on long target sets a half whose minimum is not below the
+//                             thread's running second best is skipped.  The four threads sharing a row
+//                             merge their top-2 through shuffles once per task.
 #include "sift.cuh"
 #include "match_tc.cuh"
 #include <cuda_fp16.h>
@@ -49,8 +45,8 @@
 #define TC_SBO 128u                    // byte stride between 8-row groups
 #define TC_TILE_BLOCKS 2               // target tile = 2 blocks = 256 rows
 #define TC_STAGES 2
-#define TC_THREADS 384
-#define TC_EPI_GROUPS 2
+#define TC_THREADS 384              // warpgroup 0: producer; warpgroups 1, 2: consumers
+#define TC_CONSUMER_WARPS 8
 
 // ------------------------------------------------------------------ prep
 
@@ -163,55 +159,109 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo) {
-  // UMMA::SmemDescriptor (K-major, SWIZZLE_NONE): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48)
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(TC_SBO >> 4) << 32) |
-         (1ull << 46);
+  // wgmma matrix descriptor (K-major, no swizzle): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46)
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(TC_SBO >> 4) << 32);
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// D[64 x 128] (+)= A[64 x 16] . B[128 x 16]^T, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, int accum) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accum));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMA
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------ the GEMM + top-2 kernel
 
 struct __align__(8) TcBarriers {
-  uint64_t full[TC_STAGES], empty[TC_STAGES], acc_full[2][TC_EPI_GROUPS], acc_empty[2][TC_EPI_GROUPS], a_full[2], a_empty[2];
-  uint32_t tmem_base;
-  int merge[2][128][3];   // group 1 -> group 0 hand-over of (best, second, argmin), by task parity
+  uint64_t full[TC_STAGES], empty[TC_STAGES], a_full[2], a_empty[2];
 };
+
+// One half (128 target columns) of a tile in a consumer thread's accumulators: element 4i + e holds
+// row r0 (e < 2) or r0 + 8 (e >= 2), column 128 h + 8 i + 2 quad + (e & 1).  The key packs the column
+// WITHOUT the 2 quad term (the same for every element of the thread) so that it stays an immediate;
+// the term is added back when the key's column is read out.
+template <bool FILTER, int H>
+__device__ __forceinline__ void tc_reduce_half(const float (&d)[64], uint32_t keymask, bool prefilter, const int* g2,
+                                               int* k1, int* k2, const int* thr, int col_base, int t_n, const int* grow,
+                                               int* __restrict__ cand_cnt, int* __restrict__ cand) {
+  if (FILTER) {
+    // branch-free hit masks first: a conditional body inside the unrolled compare blows the loop
+    // up past the instruction cache
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      unsigned hit = 0;
+#pragma unroll
+      for (int j = 0; j < 32; ++j)
+        hit |= ((int)(__float_as_uint(d[4 * (j >> 1) + 2 * r + (j & 1)]) & 0xffffff00u) <= thr[r]) ? (1u << j) : 0u;
+      while (hit) {
+        const int j = __ffs(hit) - 1;
+        hit &= hit - 1;
+        const int col = col_base + H * 128 + 8 * (j >> 1) + (j & 1);
+        if (col < t_n) {
+          const int slot = atomicAdd(&cand_cnt[grow[r]], 1);
+          if (slot < TC_CAND_CAP) cand[(size_t)grow[r] * TC_CAND_CAP + slot] = col;
+        }
+      }
+    }
+  } else {
+    if (prefilter) {
+      // A half none of whose scores is below the thread's running second best cannot change its
+      // top-2 (masking is monotone, ties keep the earlier column); with c columns seen, a row
+      // improves in a half with probability ~2/c, so on long target sets most halves are skipped.
+      int m0 = (int)__float_as_uint(d[0]), m1 = (int)__float_as_uint(d[2]);
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        m0 = min(m0, min((int)__float_as_uint(d[4 * i]), (int)__float_as_uint(d[4 * i + 1])));
+        m1 = min(m1, min((int)__float_as_uint(d[4 * i + 2]), (int)__float_as_uint(d[4 * i + 3])));
+      }
+      if (!__any_sync(0xffffffffu, m0 < g2[0] || m1 < g2[1])) return;
+    }
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        // (v & mask) | column in ONE LOP3: the mask has to sit in a register, because the
+        // instruction takes a single immediate
+        uint32_t ukey;
+        asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(ukey) : "r"(__float_as_uint(d[4 * i + e])), "r"(keymask), "r"((uint32_t)(H * 128 + 8 * i + (e & 1))));
+        const int key = (int)ukey, r = e >> 1;
+        k2[r] = min(k2[r], max(k1[r], key));
+        k1[r] = min(k1[r], key);
+      }
+  }
+}
 
 // FILTER = false: running top-2 per query row (the nomination pass).
 // FILTER = true : second pass over GATHERED rows only; every column whose score is
 //                 within the row's threshold key is appended to that row's candidate
 //                 slots (the exact kernel then decides among a handful of columns).
 //
-// PERSISTENT: a CTA walks tasks blockIdx.x, blockIdx.x + gridDim.x, ...; the three roles run the
-// same task sequence on their own, coupled only through mbarriers whose phases follow two running
-// counters (target tiles and tasks).  Nothing is re-initialised between tasks, so the producer is
-// already fetching the next task's query block (two A buffers) and target tiles while the MMA and
-// the epilogue finish the current one: an image pair of ~2 k descriptors is only ~10 tiles per
-// task, and the per-task prologue used to cost as much as the tiles themselves.
+// PERSISTENT: a CTA walks tasks blockIdx.x, blockIdx.x + gridDim.x, ...; the producer and the two
+// consumer warpgroups run the same task sequence on their own, coupled only through mbarriers whose
+// phases follow two running counters (target tiles and tasks).  Nothing is re-initialised between
+// tasks, so the producer is already fetching the next task's query block (two A buffers) and target
+// tiles while the consumers finish the current one: an image pair of ~2 k descriptors is only ~10
+// tiles per task.
 template <bool FILTER>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_tc_pass(const unsigned char* __restrict__ qbuf, const unsigned char* __restrict__ tbuf,
@@ -220,27 +270,18 @@ k_tc_pass(const unsigned char* __restrict__ qbuf, const unsigned char* __restric
           const int* __restrict__ g_thr, int* __restrict__ cand_cnt, int* __restrict__ cand) {
   extern __shared__ __align__(1024) unsigned char tc_smem[];
   const int task_end = n_tasks_dev ? *n_tasks_dev : n_tasks_host;
-  if ((int)blockIdx.x >= task_end) return;   // uniform per CTA, before any barrier / TMEM use
+  if ((int)blockIdx.x >= task_end) return;   // uniform per CTA, before any barrier use
   unsigned char* sA = tc_smem;                                        // 2 query blocks
   unsigned char* sB = tc_smem + 2 * TC_BLOCK_BYTES;                   // TC_STAGES x 2 blocks
   TcBarriers* bars = (TcBarriers*)(sB + (size_t)TC_STAGES * TC_TILE_BLOCKS * TC_BLOCK_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars->tmem_base)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (threadIdx.x == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(smem_u32(&bars->full[s]), 1); mbar_init(smem_u32(&bars->empty[s]), 1); }
-    for (int s = 0; s < 2; ++s) {
-      for (int g = 0; g < TC_EPI_GROUPS; ++g) { mbar_init(smem_u32(&bars->acc_full[s][g]), 1); mbar_init(smem_u32(&bars->acc_empty[s][g]), 128); }
-      mbar_init(smem_u32(&bars->a_full[s]), 1); mbar_init(smem_u32(&bars->a_empty[s]), 1);
-    }
+    // the consumers release a buffer with one arrival per warp, after that warp's wgmma.wait_group
+    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(smem_u32(&bars->full[s]), 1); mbar_init(smem_u32(&bars->empty[s]), TC_CONSUMER_WARPS); }
+    for (int s = 0; s < 2; ++s) { mbar_init(smem_u32(&bars->a_full[s]), 1); mbar_init(smem_u32(&bars->a_empty[s]), TC_CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars->tmem_base;
 
   if (warp == 0) {
     // ===== producer
@@ -265,152 +306,91 @@ k_tc_pass(const unsigned char* __restrict__ qbuf, const unsigned char* __restric
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one thread)
-    if (lane == 0) {
-      // UMMA::InstrDescriptor: c_format F32 [4,6)=1, a/b F16 = 0, K-major both, N>>3 [17,23), M>>4 [24,29)
-      const uint32_t idesc = (1u << 4) | ((256u >> 3) << 17) | ((128u >> 4) << 24);   // M 128, N 256
-      uint32_t gt = 0, ti = 0;
-      for (int task = blockIdx.x; task < task_end; task += gridDim.x, ++ti) {
-        const TcTask tk = tasks[task];
-        const int ntile = tk.t_blocks / TC_TILE_BLOCKS;
-        const uint32_t asl = ti & 1u;
-        mbar_wait(smem_u32(&bars->a_full[asl]), (ti >> 1) & 1u);
-        const uint32_t a0 = smem_u32(sA + (size_t)asl * TC_BLOCK_BYTES);
-        for (int t = 0; t < ntile; ++t, ++gt) {
-          const uint32_t s = gt % TC_STAGES, as = gt & 1u;
-          mbar_wait(smem_u32(&bars->full[s]), (gt / TC_STAGES) & 1u);
-          const uint32_t b0 = smem_u32(sB + (size_t)s * TC_TILE_BLOCKS * TC_BLOCK_BYTES);
-#pragma unroll
-          for (int half = 0; half < TC_EPI_GROUPS; ++half) mbar_wait(smem_u32(&bars->acc_empty[as][half]), ((gt >> 1) & 1u) ^ 1u);
-          tc_fence_after();
-          // one M128 N256 K16 instruction per k-step covers the whole 256-row target tile: the query
-          // block is read from shared memory once per tile and k-step instead of once per half
-          const uint32_t d = tmem + (uint32_t)(as * 256);
-#pragma unroll
-          for (int k = 0; k < TC_KC / 2; ++k) {
-            const uint64_t ad = make_smem_desc(a0 + k * 2 * TC_LBO, TC_LBO);
-            const uint64_t bd = make_smem_desc(b0 + k * 2 * TC_TLBO, TC_TLBO);
-            umma_f16(d, ad, bd, idesc, k > 0 ? 1u : 0u);
-          }
-#pragma unroll
-          for (int half = 0; half < TC_EPI_GROUPS; ++half) umma_commit(smem_u32(&bars->acc_full[as][half]));   // both column halves are ready
-          umma_commit(smem_u32(&bars->empty[s]));      // smem slot reusable once these MMAs retire
-        }
-        umma_commit(smem_u32(&bars->a_empty[asl]));    // every MMA that reads this query block has retired
-      }
-    }
   } else if (warp >= 4) {
-    // ===== epilogue: thread <-> query row (TMEM lane)
-    const int row = (warp & 3) * 32 + lane;
-    const int grp = (warp - 4) >> 2;           // which 128-column half of every tile
-    const uint32_t lane_addr = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(grp * 128);
+    // ===== consumers: warpgroup wg = query rows [64 wg, 64 wg + 64); thread <-> rows r0, r0 + 8
+    const int wg = (warp - 4) >> 2, quad = lane & 3;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int rows[2] = {r0, r0 + 8};
+    uint32_t keymask;
+    asm volatile("mov.b32 %0, 0xffffff00;" : "=r"(keymask));
+    float acc0[64], acc1[64];
     uint32_t gt = 0, ti = 0;
     for (int task = blockIdx.x; task < task_end; task += gridDim.x, ++ti) {
       const TcTask tk = tasks[task];
       const int ntile = tk.t_blocks / TC_TILE_BLOCKS;
-      int g1 = 0x7f7fff00, g2 = 0x7f7fff00;   // running best / second (value bits, low 8 cleared)
-      int gi = 0x7fffffff;
-      const int grow = tk.q_row0 + row;        // FILTER: index of this gathered row
+      int g1[2] = {0x7f7fff00, 0x7f7fff00}, g2[2] = {0x7f7fff00, 0x7f7fff00};   // running best / second (value bits, low 8 cleared)
+      int gi[2] = {0x7fffffff, 0x7fffffff};
       const int col0 = (FILTER || n_tasks_dev) ? 0 : tk.t_pad;   // first pass: first column of this task's range
-      uint32_t keymask;
-      asm volatile("mov.b32 %0, 0xffffff00;" : "=r"(keymask));
-      const int thr = FILTER ? g_thr[grow] : 0;
-      // long target sets only: on short ones nearly every chunk still improves some row of the warp
+      int grow[2], thr[2];                      // FILTER: index of each row among the gathered rows, its threshold
+#pragma unroll
+      for (int r = 0; r < 2; ++r) { grow[r] = tk.q_row0 + rows[r]; thr[r] = FILTER ? g_thr[grow[r]] : 0; }
+      // long target sets only: on short ones nearly every half still improves some row of the warp
       const bool prefilter = !FILTER && tk.t_blocks >= 128;
+      const uint32_t asl = ti & 1u;
+      mbar_wait(smem_u32(&bars->a_full[asl]), (ti >> 1) & 1u);
+      const uint32_t a0 = smem_u32(sA + (size_t)asl * TC_BLOCK_BYTES) + (uint32_t)(wg * 8) * TC_SBO;
       for (int t = 0; t < ntile; ++t, ++gt) {
-        const uint32_t as = gt & 1u;
-        mbar_wait(smem_u32(&bars->acc_full[as][grp]), (gt >> 1) & 1u);
-        tc_fence_after();
-        int k1 = 0x7fffffff, k2 = 0x7fffffff;
+        const uint32_t s = gt % TC_STAGES;
+        mbar_wait(smem_u32(&bars->full[s]), (gt / TC_STAGES) & 1u);
+        const uint32_t b0 = smem_u32(sB + (size_t)s * TC_TILE_BLOCKS * TC_BLOCK_BYTES);
+        acc_fence(acc0); acc_fence(acc1);
+        wgmma_fence();
 #pragma unroll
-        for (int c0 = 0; c0 < 128; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld32(lane_addr + (uint32_t)(as * 256 + c0), v);
-          tmem_ld_wait();
-          if (FILTER) {
-            // branch-free hit mask first: a conditional body inside the 256-way unrolled compare
-            // blows the loop up past the instruction cache (measured 3x slower per tile)
-            unsigned hit = 0;
+        for (int k = 0; k < TC_KC / 2; ++k)
+          wgmma_m64n128k16(acc0, make_smem_desc(a0 + k * 2 * TC_LBO, TC_LBO), make_smem_desc(b0 + k * 2 * TC_TLBO, TC_TLBO), k);
+        wgmma_commit();
 #pragma unroll
-            for (int j = 0; j < 32; ++j) hit |= ((int)(v[j] & 0xffffff00u) <= thr) ? (1u << j) : 0u;
-            while (hit) {
-              const int j = __ffs(hit) - 1;
-              hit &= hit - 1;
-              const int col = t * 256 + grp * 128 + c0 + j;
-              if (col < tk.t_n) {
-                const int slot = atomicAdd(&cand_cnt[grow], 1);
-                if (slot < TC_CAND_CAP) cand[(size_t)grow * TC_CAND_CAP + slot] = col;
-              }
-            }
-          } else {
-            if (prefilter) {
-              // A chunk none of whose 32 scores is below the row's running second best cannot change
-              // the row's top-2 (masking is monotone, ties keep the earlier column): one 3-input min
-              // per two elements decides that, against 3.5 ALU instructions per element of the full
-              // update.  With c chunks seen, a row improves in a chunk with probability ~2/c, a warp
-              // of 32 rows with ~1 - exp(-64/c): after 16 k columns most chunks are skipped.
-              int m = (int)v[0];
+        for (int k = 0; k < TC_KC / 2; ++k)   // target rows 128-255 of the tile: row groups 16-31
+          wgmma_m64n128k16(acc1, make_smem_desc(a0 + k * 2 * TC_LBO, TC_LBO),
+                           make_smem_desc(b0 + 16 * TC_SBO + k * 2 * TC_TLBO, TC_TLBO), k);
+        wgmma_commit();
+        int k1[2] = {0x7fffffff, 0x7fffffff}, k2[2] = {0x7fffffff, 0x7fffffff};
+        const int col_base = t * 256 + 2 * quad;
+        wgmma_wait<1>();
+        acc_fence(acc0);
+        tc_reduce_half<FILTER, 0>(acc0, keymask, prefilter, g2, k1, k2, thr, col_base, tk.t_n, grow, cand_cnt, cand);
+        wgmma_wait<0>();
+        acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&bars->empty[s]));   // this warp's MMAs have read the stage
+        tc_reduce_half<FILTER, 1>(acc1, keymask, prefilter, g2, k1, k2, thr, col_base, tk.t_n, grow, cand_cnt, cand);
+        if (!FILTER) {
+          // merge the tile's top-2 into the running top-2 (an earlier tile wins a tie: lower column)
 #pragma unroll
-              for (int j = 1; j < 31; j += 2) m = min(m, min((int)v[j], (int)v[j + 1]));
-              m = min(m, (int)v[31]);
-              if (!__any_sync(0xffffffffu, m < g2)) continue;
-            }
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              // (v & mask) | column in ONE LOP3: the mask has to sit in a register, because the
-              // instruction takes a single immediate (the compiler's and-imm / or-imm pair costs two
-              // ALU slots per element of a loop that is ALU-issue bound)
-              uint32_t ukey;
-              asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(ukey) : "r"(v[j]), "r"(keymask), "r"((uint32_t)(c0 + j)));
-              const int key = (int)ukey;
-              k2 = min(k2, max(k1, key));
-              k1 = min(k1, key);
-            }
+          for (int r = 0; r < 2; ++r) {
+            const int v1 = k1[r] & (int)0xffffff00, v2 = k2[r] & (int)0xffffff00;
+            if (v1 < g1[r]) { g2[r] = min(g1[r], v2); g1[r] = v1; gi[r] = col0 + col_base + (k1[r] & 0xff); }
+            else g2[r] = min(g2[r], v1);
           }
         }
-        tc_fence_before();
-        mbar_arrive(smem_u32(&bars->acc_empty[as][grp]));
-        if (!FILTER) {
-          // merge the tile's top-2 into the running top-2
-          const int v1 = k1 & (int)0xffffff00, v2 = k2 & (int)0xffffff00;
-          if (v1 < g1) { g2 = min(g1, v2); g1 = v1; gi = col0 + t * 256 + grp * 128 + (k1 & 0xff); }
-          else g2 = min(g2, v1);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&bars->a_empty[asl]));   // every MMA of this warp that reads the query block is done
+#pragma unroll
+      for (int r = 0; r < 2 && !FILTER; ++r) {
+        // the four threads of a row hold interleaved columns: equal scores keep the lower column
+#pragma unroll
+        for (int off = 1; off < 4; off <<= 1) {
+          const int o1 = __shfl_xor_sync(0xffffffffu, g1[r], off), o2 = __shfl_xor_sync(0xffffffffu, g2[r], off);
+          const int oi = __shfl_xor_sync(0xffffffffu, gi[r], off);
+          if (o1 < g1[r] || (o1 == g1[r] && oi < gi[r])) { g2[r] = min(g1[r], o2); g1[r] = o1; gi[r] = oi; }
+          else g2[r] = min(g2[r], o1);
+        }
+        // device-planned tasks (n_tasks_dev) are GATHERED blocks: q_row0 is the block's first gathered
+        // row, q_n its real rows, and the nomination goes to the gathered row's slot
+        const int qrow = tk.q_row0 + rows[r];
+        if (quad == 0 && (n_tasks_dev ? rows[r] < tk.q_n : qrow < tk.q_n)) {
+          const float s = tc_scale_from_maxnorm(__uint_as_float(*maxnorm_bits));
+          const float inv = 1.f / (s * s);
+          TcTop2 o;
+          o.m1 = (__int_as_float(g1[r]) - 1.f) * inv;
+          o.m2 = g2[r] == 0x7f7fff00 ? FLT_MAX : (__int_as_float(g2[r]) - 1.f) * inv;
+          o.idx = gi[r];
+          o.pad = 0;
+          res[(n_tasks_dev ? 0 : tk.res_off) + qrow] = o;
         }
       }
-      if (!FILTER) {
-        // the two column halves meet here: group 1 hands its running top-2 to group 0.  One named
-        // barrier per task is enough with two slots: group 1 cannot reach task ti+2 before group 0
-        // has arrived at the barrier of task ti+1, i.e. after it read slot ti.
-        int* mg = bars->merge[ti & 1u][row];
-        if (grp == 1) { mg[0] = g1; mg[1] = g2; mg[2] = gi; }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (grp == 1) continue;
-        const int o1 = mg[0], o2 = mg[1], oi = mg[2];
-        // equal scores keep the lower column, as the single-chain scan did
-        if (o1 < g1 || (o1 == g1 && oi < gi)) { g2 = min(g1, o2); g1 = o1; gi = oi; }
-        else g2 = min(g2, o1);
-      }
-      // device-planned tasks (n_tasks_dev) are GATHERED blocks: q_row0 is the block's first gathered
-      // row, q_n its real rows, and the nomination goes to the gathered row's slot
-      const int qrow = tk.q_row0 + row;
-      if (!FILTER && (n_tasks_dev ? row < tk.q_n : qrow < tk.q_n)) {
-        const float s = tc_scale_from_maxnorm(__uint_as_float(*maxnorm_bits));
-        const float inv = 1.f / (s * s);
-        TcTop2 o;
-        o.m1 = (__int_as_float(g1) - 1.f) * inv;
-        o.m2 = g2 == 0x7f7fff00 ? FLT_MAX : (__int_as_float(g2) - 1.f) * inv;
-        o.idx = gi;
-        o.pad = 0;
-        res[(n_tasks_dev ? 0 : tk.res_off) + qrow] = o;
-      }
     }
-  }
-  tc_fence_before();
-  __syncthreads();                 // every role is done with the barriers, smem and TMEM
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
   }
 }
 

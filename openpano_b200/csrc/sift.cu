@@ -1,4 +1,4 @@
-// sift.cu — batched SIFT on sm_100a: working resize, octave grey, fused
+// sift.cu — batched SIFT on sm_90a: working resize, octave grey, fused
 // 6-sigma separable blur + |DoG|, extrema scan + ordered compaction, sub-pixel
 // refinement, orientation assignment and 128-D RootSIFT descriptors.
 //
@@ -1082,7 +1082,7 @@ k_descriptor_v1(const OctMeta* __restrict__ octs, const ImgMeta* __restrict__ im
 
 // ------------------------------------------------------------ K6, quad design
 // Same contract as k_descriptor_v1 (bit-identical output); what changed and why
-// (profiles/r02x_*: the v1 walk ran 47 instructions per cell visit, and a half-warp-per-
+// (the v1 walk paid a ballot-built visit list per cell, and a half-warp-per-
 // keypoint variant with one lane per cell kept only 10 of 32 lanes busy, because a batch of
 // consecutive scan positions is a few window columns and touches 4-6 of the 16 cells):
 //   * FOUR LANES per oriented keypoint, eight keypoints per warp.  Lane (ly, lx) of a quad

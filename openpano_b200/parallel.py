@@ -347,8 +347,8 @@ class DistributedStitcher:
 
         # part 2 (after the blend and C2 are queued): ONE all-gather of [number of matches per dealt task ...,
         # (i, j) ...] padded to that total, through pinned staging both ways.  (Padding to the a-priori bound
-        # min(N_i, N_j) per pair needs no scalar round trip but moved 14 MB at 4 ranks where the lists are 1 MB:
-        # 2.5 of 6.7 ms, profiles/r02ab_run_dist_4gpu_unordered38.json.)
+        # min(N_i, N_j) per pair needs no scalar round trip but moves ~14x the bytes of the real lists on a
+        # 38-image all-pairs job at 4 ranks.)
         def gather_lists():
             stage = self._pinned("send", ntask + 2 * max(tot, 1))
             host = stage.numpy()

@@ -6,7 +6,7 @@
  *                                               reference algorithm (the orc_ C files)
  *   - oracle/_ref/libopenpano_ref.so prefix ref_: the reference's own
  *                                               translation units compiled from
- *                                               /root/reference/src (refshim/)
+ *                                               the reference's src/ (refshim/)
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
  * --impl reference legs may load them.  The product (openpano_b200) never does.
  */

@@ -1,7 +1,7 @@
 /*
  * orc_ba.c — plain-C restatement of the per-point part of the reference's symbolic
  * bundle-adjustment Jacobian.  TEST INFRASTRUCTURE ONLY (see orc_common.h).  Citations
- * relative to /root/reference/src.
+ * relative to the reference's src/.
  *
  * stitch/incremental_bundle_adjuster.cc:306-383 (IncrementalBundleAdjuster::
  * calcJacobianSymbolic): per point match the derivatives of the residual w.r.t. the 6

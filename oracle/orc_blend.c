@@ -1,7 +1,7 @@
 /*
  * orc_blend.c — plain-C restatement of the reference's two blenders.
  * TEST INFRASTRUCTURE ONLY (see orc_common.h).  Citations relative to
- * /root/reference/src.
+ * the reference's src/.
  */
 #include "orc_common.h"
 

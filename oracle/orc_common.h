@@ -5,7 +5,7 @@
  *
  * Parity status: PINNED — every function here is checked bit-for-bit against the
  * reference's own translation units (oracle/_ref/libopenpano_ref.so, built by
- * oracle/Makefile from /root/reference/src) in tests/test_oracle_vs_ref.py, and
+ * oracle/Makefile from the reference's src/) in tests/test_oracle_vs_ref.py, and
  * against the fixtures in tests/golden/ that were generated from that library
  * (tests/golden/make_golden.py).  The one step without a reference-side pin is
  * the 3x3 solve (Eigen absent; see small_linalg.h).

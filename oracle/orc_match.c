@@ -1,7 +1,7 @@
 /*
  * orc_match.c — plain-C restatement of the reference's exact matcher.
  * TEST INFRASTRUCTURE ONLY (see orc_common.h).  Citations relative to
- * /root/reference/src.
+ * the reference's src/.
  */
 #include <float.h>
 #include "orc_common.h"

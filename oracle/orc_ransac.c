@@ -1,6 +1,6 @@
 /*
  * orc_ransac.c — plain-C restatement of the RANSAC inlier scoring of the reference.
- * TEST INFRASTRUCTURE ONLY (see orc_common.h).  Citations relative to /root/reference/src.
+ * TEST INFRASTRUCTURE ONLY (see orc_common.h).  Citations relative to the reference's src/.
  *
  * stitch/transform_estimate.cc:132-148 TransformEstimation::get_inliers and the selection
  * loop of get_transform (:68-85): for every hypothesis (a Homography from image 2 to image 1)

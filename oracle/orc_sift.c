@@ -1,7 +1,7 @@
 /*
  * orc_sift.c — plain-C restatement of the reference's SIFT chain.
  * TEST INFRASTRUCTURE ONLY (see orc_common.h for who may load it and for the
- * parity-pinning status).  Citations are relative to /root/reference/src.
+ * parity-pinning status).  Citations are relative to the reference's src/.
  */
 #include <stdio.h>
 #include "orc_common.h"

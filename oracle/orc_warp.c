@@ -1,7 +1,7 @@
 /*
  * orc_warp.c — plain-C restatement of the reference's cylindrical pre-warp.
  * TEST INFRASTRUCTURE ONLY (see orc_common.h).  Citations relative to
- * /root/reference/src.
+ * the reference's src/.
  */
 #include <float.h>
 #include "orc_common.h"

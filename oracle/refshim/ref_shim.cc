@@ -2,7 +2,7 @@
 // checker API (oracle/oracle_api.h, prefix ref_).  TEST INFRASTRUCTURE ONLY.
 //
 // This file contains no algorithm: every call lands in a translation unit that
-// is compiled, unmodified, from /root/reference/src by oracle/Makefile.  The
+// is compiled, unmodified, from the reference's src/ by oracle/Makefile.  The
 // only stand-ins are lib/matrix.cc (needs Eigen, absent here: see
 // matrix_standin.cc) and a syntactic Eigen/Dense stub so lib/imgproc.cc compiles
 // (its two Eigen functions are off the hot path and are never called).

@@ -7,7 +7,7 @@
 //   B200Stitcher::build  = the three stages chained as Stitcher::build() chains them
 // Results must be bit-identical.  The reference classes come from oracle/_ref/libopenpano_ref.so
 // (the reference's own TUs, parity flags); the engine from openpano_b200/libpano_b200.so.
-// Built by oracle/Makefile (needs /root/reference); run by tests/test_gpu_adaptors.py on a GPU.
+// Built by oracle/Makefile (needs the reference sources); run by tests/test_gpu_adaptors.py on a GPU.
 //   adaptor_test <stack.bin>     stack.bin: int32 n, w, h, then n*h*w*3 float32, then per image
 //                                 int32 x0,y0,x1,y1 + float64 homo_inv[9], then float64 res, min_x, min_y
 #include <cstdio>

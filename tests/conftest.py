@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on a GPU machine)")
 
 
 @pytest.fixture(scope="session")
@@ -28,7 +28,7 @@ def ref():
     prebuilt .so did not travel."""
     from tests.checker import get_checker, have
     if not have("ref"):
-        pytest.skip("oracle/_ref/libopenpano_ref.so not built (needs /root/reference)")
+        pytest.skip("oracle/_ref/libopenpano_ref.so not built (needs the reference sources)")
     return get_checker("ref")
 
 

@@ -1,14 +1,15 @@
 #!/usr/bin/env python
 """Generates tests/golden/*.npz from the REFERENCE's own translation units
-(oracle/_ref/libopenpano_ref.so, built by oracle/Makefile from
-/root/reference/src with -O2 -ffp-contract=off -msse3, single thread).
+(oracle/_ref/libopenpano_ref.so, built by oracle/Makefile from the reference's
+src/ with -O2 -ffp-contract=off -msse3, single thread).
 
 The reference ships no golden vectors for this path (SURVEY.md §4), so these
 fixtures ARE the pin: the plain-C oracle and the CUDA engine are both compared
 against them bit for bit.  Inputs come from openpano_b200.synth (seeded numpy);
 each fixture stores a SHA-256 of its inputs so generator drift is detected.
 
-Run in the build container (needs /root/reference):  python tests/golden/make_golden.py
+Run where the reference tree was available at build time (oracle/_ref built):
+    python tests/golden/make_golden.py [imgio | ba | vs_ref]
 """
 import hashlib
 import sys
@@ -61,6 +62,36 @@ def ba(ref):
     print("ba:", len(pairs), "pairs,", len(pts), "matches")
 
 
+_RATIO_SCRIPT = """
+import json, sys
+sys.path.insert(0, {root!r})
+from tests.checker import get_checker
+from tests import test_oracle_vs_ref as t
+print(json.dumps(t.digests(t.case_match_other_ratios(get_checker('ref'), {ratio!r}))))
+"""
+
+
+def vs_ref(ref):
+    """Digests of the reference's outputs for every case of tests/test_oracle_vs_ref.py, and the
+    per-pair matrices its bundle-adjustment cases start from."""
+    import json
+    import subprocess
+    from tests import test_oracle_vs_ref as t
+    from tests.ba_util import ba_case
+    res = {key: np.array(t.digests(fn(ref, *args))) for key, fn, args in t.golden_cases()}
+    for ratio, _, _ in t.MATCH_RATIOS:       # one process per ratio: the reference freezes it on first use
+        out = subprocess.run([sys.executable, "-c", _RATIO_SCRIPT.format(root=str(ROOT), ratio=ratio)],
+                             capture_output=True, text=True, check=True)
+        res[t.case_key("test_match_other_ratios", ratio)] = np.array(json.loads(out.stdout.strip().splitlines()[-1]))
+    for args in t.BA_CASES:
+        n_cam, per_pair, seed, extra = args
+        cams, pairs, pts = ba_case(n_cam, per_pair, seed, extra_pairs=extra)
+        res[t.ba_mats_key(*args)] = ref.ba_pair_mats(cams, pairs)
+        res[t.case_key("test_ba_jacobian", *args)] = np.array(t.digests(ref.ba_jacobian_ref(cams, pairs, pts)))
+    np.savez_compressed(OUT / t.FIXTURE, **res)
+    print("vs_ref:", len(res), "entries")
+
+
 def main():
     ref = get_checker("ref")
     assert ref.num_threads() == 1
@@ -70,8 +101,12 @@ def main():
     if sys.argv[1:] == ["ba"]:
         ba(ref)
         return
+    if sys.argv[1:] == ["vs_ref"]:
+        vs_ref(ref)
+        return
     imgio(ref)
     ba(ref)
+    vs_ref(ref)
 
     # ---- SIFT chain on one 240x180 view
     img = synth.make_canvas(180, 240, 101)

@@ -40,15 +40,15 @@ def test_binding_covers_the_header():
     assert set(declared_functions()) == set(capi.EXPORTED)
 
 
-def test_library_is_sm100a_with_tensor_core_and_bulk_copy_code():
+def test_library_is_sm90a_with_tensor_core_and_bulk_copy_code():
     out = subprocess.run(["cuobjdump", "-lelf", str(LIB)], capture_output=True, text=True)
     if out.returncode != 0:
         pytest.skip("cuobjdump not available")
-    assert "sm_100a" in out.stdout
+    assert "sm_90a" in out.stdout
     sass = subprocess.run(["cuobjdump", "-sass", str(LIB)], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass          # tcgen05.mma
-    assert "LDTM" in sass             # tcgen05.ld
+    assert "HGMMA" in sass            # wgmma.mma_async
     assert "UBLKCP" in sass           # cp.async.bulk
+    assert "UTMALDG" in sass          # cp.async.bulk.tensor (TMA tile loads)
 
 
 def test_no_cpu_fallback_without_gpu():

@@ -20,7 +20,7 @@ BIN = ROOT / "oracle" / "_ref" / "adaptor_test"
 
 def test_cpp_adaptors_equal_reference_classes(tmp_path):
     if not BIN.exists():
-        pytest.skip("oracle/_ref/adaptor_test not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/adaptor_test not built (needs the reference sources at build time)")
     imgs, org = synth.make_stack(4, 360, 270, 120, 47)
     items, geom = synth.translation_blend_setup(org, 360, 270)
     path = tmp_path / "stack.bin"

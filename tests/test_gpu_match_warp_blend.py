@@ -180,7 +180,7 @@ def test_blend_full_size_properties(engine):
 
 
 def test_match_tensor_path_equals_exact_path(engine, orc, monkeypatch, match_mode):
-    """The tcgen05 nomination + certified exact decisions must give the same pairs
+    """The tensor-core nomination + certified exact decisions must give the same pairs
     as the all-fp32 CUDA-core path and as the oracle, including near-threshold
     ratios (heavy noise) where the fp16 scores cannot decide on their own."""
     rng = np.random.RandomState(77)

@@ -107,8 +107,8 @@ def load_peaks():
     pk = ROOT / "MEASURED_PEAKS.json"
     if pk.exists():
         p = json.loads(pk.read_text())
-        return float(p.get("hbm_gbs", 6650.0)), float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 1590.0))), "measured"
-    return 6650.0, 1590.0, "fallback"
+        return float(p.get("hbm_gbs", 3350.0)), float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 989.0))), "measured"
+    return 3350.0, 989.0, "H100 SXM data sheet (700 W)"
 
 
 # ----------------------------------------------------------------------------- inputs
