@@ -434,7 +434,8 @@ int  pano_sift_trace_run(pano_ctx* ctx, const float* rgb_hwc, int w, int h,
 int  pano_sift_trace_working_size(const pano_sift_trace* t, int* w0, int* h0);
 int  pano_sift_trace_octave_size(const pano_sift_trace* t, int octave, int* w, int* h);
 /* kind: 0 working RGB (3ch, octave ignored), 1 gaussian level i∈[0,nscale),
- * 2 |DoG| level i∈[0,nscale-1), 3 mag level i∈[1,nscale), 4 ort level. */
+ * 2 |DoG| level i∈[0,nscale-1) (formed on the host as fabsf(G(i) - G(i+1)): the
+ * engine keeps no |DoG| planes), 3 mag level i∈[1,nscale), 4 ort level. */
 int  pano_sift_trace_plane(pano_sift_trace* t, int kind, int octave, int level, float* out);
 /* stage: 0 raw extrema (x,y,pyr_id,scale_id valid), 1 refined+edge-tested
  * keypoints, 2 oriented keypoints.  Returns count; copies min(count,cap). */

@@ -938,13 +938,23 @@ int pano_sift_trace_plane(pano_sift_trace* t, int kind, int o, int level, float*
   }
   if (o < 0 || o >= wk->n_oct) return PANO_ERR_INVALID;
   const OctMeta& om = wk->h_oct[o];
-  const float* src = nullptr;
-  if (kind == 1 && level >= 0 && level < wk->n_scale) src = wk->arena + om.gauss_off + (size_t)level * om.plane;
-  if (kind == 2 && level >= 0 && level < wk->n_scale - 1) src = wk->arena + om.dog_off + (size_t)level * om.plane;
-  if (src) {   // planes are pitched on the device, dense for the caller
-    PANO_CUDA(ctx, cudaMemcpy2DAsync(out, (size_t)om.w * sizeof(float), src, (size_t)om.pitch * sizeof(float),
+  // planes are pitched on the device, dense for the caller
+  auto download = [&](float* dst, int lvl) -> int {
+    const float* src = wk->arena + om.gauss_off + (size_t)lvl * om.plane;
+    PANO_CUDA(ctx, cudaMemcpy2DAsync(dst, (size_t)om.w * sizeof(float), src, (size_t)om.pitch * sizeof(float),
                                      (size_t)om.w * sizeof(float), (size_t)om.h, cudaMemcpyDeviceToHost, ctx->stream));
     PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return PANO_OK;
+  };
+  if (kind == 1 && level >= 0 && level < wk->n_scale) return download(out, level);
+  if (kind == 2 && level >= 0 && level < wk->n_scale - 1) {
+    // the engine keeps no |DoG| planes: form fabsf(G(level) - G(level + 1)) as every kernel does
+    const size_t np = (size_t)om.w * om.h;
+    std::vector<float> next(np);
+    int rc = download(out, level);
+    if (rc == PANO_OK) rc = download(next.data(), level + 1);
+    if (rc != PANO_OK) return rc;
+    for (size_t i = 0; i < np; ++i) out[i] = fabsf(out[i] - next[i]);
     return PANO_OK;
   }
   // mag/ort are never materialised by the engine (recomputed inside the

@@ -26,8 +26,7 @@ struct OctMeta {
   int pitch;            // floats per plane row: w rounded up to 32, so rows start on 128-byte lines
                         // (TMA needs 16-byte global strides; warps read / write whole lines)
   float ifx, ify;       // octave resize from the working image (oct > 0)
-  long long gauss_off;  // nscale planes: grey + blurred levels
-  long long dog_off;    // nscale-1 planes
+  long long gauss_off;  // nscale planes: grey + blurred levels (|DoG| is re-formed from them where read)
   long long plane;      // floats per plane = pitch * h
 };
 
@@ -55,6 +54,7 @@ struct SiftWork {
   // keypoint state, all [n_img * cap] unless noted
   int* cand_count = nullptr;      // [n_img] + work counters (see sift.cu)
   uint32_t* cand_keys = nullptr;
+  uint32_t* seam_keys = nullptr;   // [n_img * seam capacity]: tile-perimeter pairs for k_extrema_seams
   uint32_t* sorted_keys = nullptr;
   pano_sspoint* refined = nullptr;  // valid flag in .dir < 0 ? no: see kp_valid
   unsigned char* kp_valid = nullptr;

@@ -56,6 +56,13 @@ def algorithmic_bytes(shapes, items, params, counts, bands):
         "k_rgb8_to_f32": p_in * 15,
         "k_working_resize": min(p_in, 4 * p0) * 12 + p0 * 12,
         "k_octave_grey": p0 * 12 + sp * 4,
+        # kw in {7, 13}: blur + |DoG| + extrema of the tile interiors in one pass; |DoG| is a fused
+        # temporary.  The seam test (k_extrema_seams) re-reads levels around the few tile-perimeter
+        # pixels above the colour threshold, which is not compulsory traffic: it has no bytes of its
+        # own and is counted here.
+        "k_blur_extrema": sp * 4 * (1 + (ns - 1)),           # read grey, write 6 levels
+        # the split pipeline with |DoG| planes through HBM, the traffic k_blur_extrema replaces
+        # (the generic windows run k_blur_dog_generic + k_extrema_scan over every pixel)
         "k_blur_dog": sp * 4 * (1 + 2 * (ns - 1)),            # read grey, write 6 levels + 6 |DoG|
         "k_extrema_scan": sp * 4 * (ns - 1),                  # reads the |DoG| levels once
         "k_rank_sort": n_desc * 8,

@@ -66,7 +66,7 @@ def traffic(path):
     rows = list(csv.reader(out.splitlines()))
     h = rows[0]
     acc = collections.OrderedDict()
-    alias = {"k_blur_dog_fast": "k_blur_dog", "k_tc_pass<0>": "k_tc_top2", "k_tc_pass<1>": "k_tc_filter",
+    alias = {"k_tc_pass<0>": "k_tc_top2", "k_tc_pass<1>": "k_tc_filter",
              "k_mb_blur_tma<6>": "k_mb_blur", "k_mb_blur_tma<9>": "k_mb_blur"}
     for r in rows[2:]:
         name = r[h.index("Kernel Name")].split("(")[0].replace("void ", "").strip()
