@@ -277,6 +277,39 @@ typedef struct pano_ba_pair {
 int pano_ba_jacobian(pano_ctx* ctx, int n_cam, int n_pair, const pano_ba_pair* pairs, const double* pts_to,
                      double* j_rows, double* jtj);
 
+/* A bundle-adjustment session: the per-point work of every LM iteration of
+ * IncrementalBundleAdjuster::optimize (incremental_bundle_adjuster.cc:117-169) on the device —
+ * calcError + ErrorStats::update_stats (:171-220) and get_param_update up to the solve: J, J^T J and
+ * b = J^T * err_vec (:230-238).  The match coordinates, J and the residuals of the last
+ * pano_ba_error call stay on the context's device between calls; an iteration moves the per-pair
+ * matrices up and J^T J, b, avg and max down.  The damping (:240-248) and the solve (:250) stay with
+ * the caller.  Calls on a session are calls on its ctx (same threading rule); the ctx must outlive it. */
+typedef struct pano_ba_session pano_ba_session;
+typedef struct pano_ba_link {
+  int from, to, match_begin, n_match;   /* as in pano_ba_pair */
+} pano_ba_link;
+/* pts: 4 doubles per match, pairs concatenated: p.first.x, p.first.y, p.second.x, p.second.y
+ * (MatchInfo::match; first = `to`, second = `from` in calcError, :187). */
+int  pano_ba_session_create(pano_ctx* ctx, int n_cam, int n_pair, const pano_ba_link* links, const double* pts,
+                            pano_ba_session** out);
+void pano_ba_session_free(pano_ba_session* s);
+/* calcError(state) + update_stats.  hto_to_from: 9 doubles per pair, (c_from.K() * c_from.R) *
+ * (c_to.Rinv() * c_to.K().inverse()) of the state being evaluated (:182-183), row-major.
+ * residuals (optional, 2 per match): from.x - transformed.x, from.y - transformed.y in pair then match
+ * order.  avg: sqrt of the sequential double sum of the FLOAT squares over residuals.size() (NaN without
+ * matches); max: the largest |r|, NaN residuals skipped, 0 if none.  n_pair must be the session's. */
+int  pano_ba_error(pano_ba_session* s, int n_pair, const double* hto_to_from, double* avg, double* max,
+                   double* residuals);
+/* get_param_update (:230-238) up to the damping.  mats: 13*9 doubles per pair, the order of
+ * pano_ba_pair.m, of the state J is taken at.  jtj: (6 n_cam)^2 doubles, UNDAMPED, as
+ * calcJacobianSymbolic leaves it; b: 6 n_cam doubles, J^T times the residuals of the LAST pano_ba_error
+ * call on this session (after a rejected step those belong to the rejected state, as at :140/:152);
+ * an entry is NaN when a residual of a pair without its camera is not finite (0 * inf in the reference's
+ * dense product), and otherwise the reference's sum, inf included.  j_rows (optional) as in
+ * pano_ba_jacobian.  PANO_ERR_INVALID before the first pano_ba_error. */
+int  pano_ba_normal_equations(pano_ba_session* s, int n_pair, const double* mats, double* jtj, double* b,
+                              double* j_rows);
+
 /* ---------------------------------------------------------- cylinder warp
  * Replaces CylinderWarper(h_factor).warp(Mat32f&, vector<Vec2D>&)
  * (stitch/warp.hh:41-66, warp.cc:25-75). */

@@ -111,4 +111,11 @@ class PanoBaPair(C.Structure):
     ]
 
 
+class PanoBaLink(C.Structure):
+    _fields_ = [
+        ("from_", C.c_int), ("to", C.c_int),
+        ("match_begin", C.c_int), ("n_match", C.c_int),
+    ]
+
+
 PROJ_FLAT, PROJ_CYLINDRICAL, PROJ_SPHERICAL = 0, 1, 2

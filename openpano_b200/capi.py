@@ -11,7 +11,7 @@ from pathlib import Path
 
 import numpy as np
 
-from ._abi import (PanoBaPair, PanoBlendGeom, PanoCylJob, PanoBlendImage, PanoMatches, PanoParams, PanoRansacPair, PanoSSPoint,
+from ._abi import (PanoBaLink, PanoBaPair, PanoBlendGeom, PanoCylJob, PanoBlendImage, PanoMatches, PanoParams, PanoRansacPair, PanoSSPoint,
                    default_params)
 
 LIB_PATH = Path(__file__).resolve().parent / "libpano_b200.so"
@@ -79,6 +79,10 @@ def _load():
         "pano_comm_allgather_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
         "pano_ransac_score_pairs": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoRansacPair), _ip, _ip, _vpp, _vpp]),
         "pano_ba_jacobian": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(PanoBaPair), _dp, _dp, _dp]),
+        "pano_ba_session_create": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(PanoBaLink), _dp, _vpp]),
+        "pano_ba_session_free": (None, [C.c_void_p]),
+        "pano_ba_error": (C.c_int, [C.c_void_p, C.c_int, _dp, _dp, _dp, _dp]),
+        "pano_ba_normal_equations": (C.c_int, [C.c_void_p, C.c_int, _dp, _dp, _dp, _dp]),
         "pano_cyl_warp_shape": (C.c_int, [C.c_int, C.c_int, C.c_double, P, _ip, _ip, _dp, _dp]),
         "pano_cyl_warp": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, C.c_double, P, _fp, C.c_int,
                                     C.c_int, _dp, C.c_int]),
@@ -229,6 +233,54 @@ class GpuSiftTrace:
     def close(self):
         if self._h:
             LIB.pano_sift_trace_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class BaSession:
+    """Device-resident state of one bundle adjustment (pano_ba_session): the match coordinates, J and the
+    residuals of the last error() call.  error() is calcError + update_stats; normal_equations() is
+    get_param_update up to the damping, with b = J^T times the residuals of the LAST error() call."""
+
+    def __init__(self, eng, handle, n_cam, n_pair, n_match):
+        self.eng, self._h = eng, handle
+        self.n_cam, self.n_pair, self.n_match = n_cam, n_pair, n_match
+
+    def _mats(self, a, per_pair, what):
+        a = np.ascontiguousarray(a, np.float64)
+        if a.size != self.n_pair * per_pair:
+            raise PanoError(-2, f"ba session: {what} has {a.size} doubles, the session's {self.n_pair} pairs need "
+                                f"{self.n_pair * per_pair}")
+        return a.reshape(-1)
+
+    def error(self, hto, want_residuals=True):
+        """hto: [n_pair, 9] Hto_to_from of the state.  -> (avg, max, residuals [2 n_match] or None)."""
+        h = self._mats(hto, 9, "hto")
+        avg, mx = C.c_double(), C.c_double()
+        res = np.zeros(max(2 * self.n_match, 1), np.float64) if want_residuals else None
+        self.eng._check(LIB.pano_ba_error(self._h, self.n_pair, _d(h) if h.size else None, C.byref(avg), C.byref(mx),
+                                          _d(res) if want_residuals else None))
+        return avg.value, mx.value, (res[:2 * self.n_match] if want_residuals else None)
+
+    def normal_equations(self, mats, want_rows=False):
+        """mats: [n_pair, 13, 9] in pano_ba_pair.m order.  -> (jtj [6n, 6n] undamped, b [6n], j_rows [n_match, 24] or None)."""
+        m = self._mats(mats, 117, "mats")
+        n = 6 * self.n_cam
+        jtj = np.full((n, n), np.nan, np.float64)
+        b = np.full(n, np.nan, np.float64)
+        rows = np.zeros((max(self.n_match, 1), 24), np.float64) if want_rows else None
+        self.eng._check(LIB.pano_ba_normal_equations(self._h, self.n_pair, _d(m) if m.size else None, _d(jtj), _d(b),
+                                                     _d(rows) if want_rows else None))
+        return jtj, b, (rows[:self.n_match] if want_rows else None)
+
+    def close(self):
+        if self._h:
+            LIB.pano_ba_session_free(self._h)
             self._h = None
 
     def __del__(self):
@@ -505,6 +557,22 @@ class Engine:
         jtj = np.full((6 * n_cam, 6 * n_cam), np.nan, np.float64)
         self._check(LIB.pano_ba_jacobian(self._h, n_cam, n, arr, _d(pts_to), _d(rows) if want_rows else None, _d(jtj)))
         return (rows[:begin] if want_rows else None), jtj
+
+    def ba_session(self, n_cam, pairs, pts) -> BaSession:
+        """pairs: list of (from_slot, to_slot, n_match) in match order; pts: [n_match_total, 4] =
+        p.first.x, p.first.y, p.second.x, p.second.y of MatchInfo::match (to, then from)."""
+        n = len(pairs)
+        arr = (PanoBaLink * max(n, 1))()
+        begin = 0
+        for k, (f, t, nm) in enumerate(pairs):
+            arr[k].from_, arr[k].to, arr[k].match_begin, arr[k].n_match = f, t, begin, nm
+            begin += nm
+        pts = np.ascontiguousarray(pts, np.float64).reshape(-1, 4)
+        if len(pts) != begin:
+            raise PanoError(-2, f"ba session: {len(pts)} coordinate rows for {begin} matches")
+        h = C.c_void_p()
+        self._check(LIB.pano_ba_session_create(self._h, n_cam, n, arr, _d(pts) if len(pts) else None, C.byref(h)))
+        return BaSession(self, h, n_cam, n, begin)
 
     # -- cylinder warp
     @staticmethod

@@ -4,6 +4,8 @@
 //   PairWiseMatcher      feature/matcher.hh:40-67  (same constructor shape and match(i, j))
 //   BlenderBase          stitch/blender.hh:14-59
 //   CylinderWarper       stitch/warp.hh:41-66
+//   the LM loop of IncrementalBundleAdjuster::optimize (stitch/incremental_bundle_adjuster.cc:117-169):
+//                        calcError and get_param_update's J / J^T J / b, B200BundleAdjusterStep
 // and forward to the C ABI of libpano_b200.so (include/pano_b200.h).  Header-only; compiles
 // against the reference's headers (-I <reference>/src) with the reference's own flags.
 // tests/adaptor/adaptor_test.cc builds these against the reference tree and checks them
@@ -25,6 +27,8 @@
 #include "stitch/blender.hh"
 #include "stitch/warp.hh"
 #include "stitch/homography.hh"
+#include "stitch/camera.hh"
+#include "stitch/match_info.hh"
 
 namespace pano_b200 {
 
@@ -257,6 +261,71 @@ class B200Stitcher {
  private:
   const Context& c_;
   B200SIFTDetector det_;
+};
+
+// ---- bundle adjustment: the per-point work of one LM iteration of IncrementalBundleAdjuster::optimize
+// (incremental_bundle_adjuster.cc:117-169) on a pano_ba_session.  Constructed where optimize() has
+// called update_index_map(), from match_pairs in order; then, per iteration,
+//   error(cameras)              replaces calcError(state) (:171-197) incl. update_stats (:199-220)
+//   normal_equations(mats, ..)  replaces get_param_update's calcJacobianSymbolic + `J.transpose() * err_vec`
+//                               (:233-238); b uses the residuals of the LAST error() call, as the
+//                               reference's err_stat.residuals do after a rejected step (:140, :152)
+// The damping (:240-248), the solve (:250) and the per-pair 3x3 algebra (the 13 matrices of
+// pano_ba_pair, which need the file-local dRdvi) stay in the caller's TU.
+class B200BundleAdjusterStep {
+ public:
+  struct Pair { int from, to; const pano::MatchInfo* m; };   // slots index_map[pair.from], index_map[pair.to]
+  struct Stats { double avg, max; };
+  B200BundleAdjusterStep(const Context& c, int n_cam, const std::vector<Pair>& pairs) : c_(c), n_cam_(n_cam), pairs_(pairs) {
+    std::vector<pano_ba_link> links(pairs.size() + 1);
+    std::vector<double> pts;
+    int begin = 0;
+    for (size_t p = 0; p < pairs.size(); ++p) {
+      const int n = (int)pairs[p].m->match.size();
+      links[p].from = pairs[p].from; links[p].to = pairs[p].to; links[p].match_begin = begin; links[p].n_match = n;
+      for (const auto& q : pairs[p].m->match) {
+        pts.push_back(q.first.x); pts.push_back(q.first.y); pts.push_back(q.second.x); pts.push_back(q.second.y);
+      }
+      begin += n;
+    }
+    n_res_ = 2 * (size_t)begin;
+    c_.check(pano_ba_session_create(c_.get(), n_cam, (int)pairs.size(), links.data(), pts.empty() ? nullptr : pts.data(), &s_));
+  }
+  ~B200BundleAdjusterStep() { pano_ba_session_free(s_); }
+  B200BundleAdjusterStep(const B200BundleAdjusterStep&) = delete;
+  B200BundleAdjusterStep& operator=(const B200BundleAdjusterStep&) = delete;
+
+  // calcError(state): `cameras` = state.get_cameras() (slot order).  residuals (optional) as ErrorStats::residuals.
+  Stats error(const std::vector<pano::Camera>& cameras, std::vector<double>* residuals = nullptr) {
+    std::vector<double> h(9 * pairs_.size() + 1);
+    for (size_t p = 0; p < pairs_.size(); ++p) {
+      const pano::Camera &c_from = cameras[pairs_[p].from], &c_to = cameras[pairs_[p].to];
+      pano::Homography m = (c_from.K() * c_from.R) * (c_to.Rinv() * c_to.K().inverse());   // :182-183
+      memcpy(&h[9 * p], m.data, sizeof(double) * 9);
+    }
+    Stats st;
+    if (residuals) residuals->resize(n_res_);
+    c_.check(pano_ba_error(s_, (int)pairs_.size(), h.data(), &st.avg, &st.max,
+                           residuals && n_res_ ? residuals->data() : nullptr));
+    return st;
+  }
+  // J^T J (undamped, (6 n_cam)^2 row-major) and b = J^T r at the state the 13 matrices per pair
+  // (pano_ba_pair.m order, 117 doubles each) were evaluated at.  j_rows (optional): pano_ba_jacobian's layout.
+  void normal_equations(const std::vector<double>& mats, std::vector<double>& jtj, std::vector<double>& b,
+                        std::vector<double>* j_rows = nullptr) {
+    const size_t N = 6 * (size_t)n_cam_;
+    jtj.resize(N * N);
+    b.resize(N);
+    if (j_rows) j_rows->resize(12 * n_res_);
+    c_.check(pano_ba_normal_equations(s_, (int)pairs_.size(), mats.data(), jtj.data(), b.data(),
+                                      j_rows && n_res_ ? j_rows->data() : nullptr));
+  }
+ private:
+  const Context& c_;
+  int n_cam_;
+  std::vector<Pair> pairs_;
+  size_t n_res_ = 0;
+  pano_ba_session* s_ = nullptr;
 };
 
 }  // namespace pano_b200
