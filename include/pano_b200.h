@@ -379,6 +379,22 @@ int pano_blend_rows_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
                         int bands, const pano_params* p, float* d_out_rows, int out_w, int out_h,
                         int row0, int row1);
 
+/* ---------------------------------------------------------- little planet
+ * Replaces planet() (main.cc:294-331, the `planet` sub-command) without the file I/O: the
+ * stereographic "little planet" view of a mosaic.  The input is any h×w×3 f32 image (the blenders'
+ * -1 pixels included); h == 1 or w == 1 is valid and gives an image without any colour, as in the
+ * reference.  Output pixel (i, j) is interpolate(mosaic, row, column) (lib/imgproc.cc:135-156) at
+ * row = min(h - (hypot(500 - i, 500 - j) / 500) * h, h - 1), column = theta / (2π) * w; pixels at
+ * distance 0 or >= 500 from the centre, and Color::NO samples, stay -1.  Bit-identical to the
+ * reference: hypot and atan are evaluated once per process on the host with its libm, and each ctx
+ * keeps the resulting 16 MB per-pixel table on its device from its first planet call to pano_destroy. */
+#define PANO_PLANET_SIZE 1000   /* main.cc:297, OUTSIZE */
+/* out_hwc = 1000×1000×3 f32, -1 where nothing maps; host in/out, returns when done. */
+int pano_planet(pano_ctx* ctx, const float* rgb_hwc, int w, int h, float* out_hwc);
+/* Device in/out (e.g. the mosaic pano_blend_dev leaves on the device), asynchronous on the ctx
+ * stream; d_out_hwc holds 1000×1000×3 f32. */
+int pano_planet_dev(pano_ctx* ctx, const float* d_rgb_hwc, int w, int h, float* d_out_hwc);
+
 /* --------------------------------------------------------- multi-GPU
  * One process (or host thread) per GPU, one pano_ctx each (SURVEY.md §8e).  The path shards on
  * independent units — images k mod G for SIFT (stitcherbase.cc:14), the pair list of

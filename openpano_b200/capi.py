@@ -94,6 +94,8 @@ def _load():
                                      C.POINTER(PanoBlendGeom), C.c_int, P, C.c_void_p, C.c_int, C.c_int]),
         "pano_blend_rows_dev": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom),
                                           C.c_int, P, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
+        "pano_planet": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, _fp]),
+        "pano_planet_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
         "pano_featureset_import_dev": (C.c_int, [C.c_void_p, C.c_int, _ip, _vpp, _vpp, _vpp]),
         "pano_featureset_export_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
         "pano_featureset_export_all_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -643,6 +645,22 @@ class Engine:
         arr, g = self._blend_args(ptrs, shapes, items, geom)
         self._check(LIB.pano_blend_dev(self._h, len(ptrs), arr, C.byref(g), bands, C.byref(params),
                                        C.c_void_p(d_out), out_w, out_h))
+
+    # -- little planet (main.cc:294-331)
+    PLANET_SIZE = 1000                 # PANO_PLANET_SIZE, main.cc:297
+
+    def planet(self, img):
+        """img: H×W×3 float32 mosaic (-1 = Color::NO) -> (1000, 1000, 3) float32, -1 where nothing maps."""
+        img = np.ascontiguousarray(img, np.float32)
+        if img.ndim != 3 or img.shape[2] != 3:
+            raise PanoError(-2, f"planet: expected an H×W×3 image, got shape {img.shape}")
+        out = np.empty((self.PLANET_SIZE, self.PLANET_SIZE, 3), np.float32)
+        self._check(LIB.pano_planet(self._h, _f(img), img.shape[1], img.shape[0], _f(out)))
+        return out
+
+    def planet_dev(self, d_src, w, h, d_out):
+        """Device pointers in and out (d_out: 1000×1000×3 f32), asynchronous on the context's stream."""
+        self._check(LIB.pano_planet_dev(self._h, C.c_void_p(d_src or 0), w, h, C.c_void_p(d_out or 0)))
 
     # ---- 8-bit boundary: read_img / crop / write_rgb formats (device pointers)
     def rgb8_to_mat32f_batch_dev(self, d_pix, ws, hs, channels, d_out):

@@ -66,6 +66,8 @@ struct pano_ctx {
   // completion markers: a word in pinned host memory the stream writes sequence numbers to
   volatile unsigned* flag = nullptr;
   unsigned flag_seq = 0;
+  // planet(): per-pixel d / center and theta / 2π (planet.cu), uploaded on the first call, freed by pano_destroy
+  double2* planet_tab = nullptr;
 };
 
 // Every entry point makes its context's device current first: host threads other than the

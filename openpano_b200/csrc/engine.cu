@@ -495,6 +495,7 @@ void pano_destroy(pano_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   ctx_cache_release(ctx, 0);
+  if (ctx->planet_tab) cudaFreeAsync(ctx->planet_tab, ctx->stream);
   cudaStreamSynchronize(ctx->stream);
   prof_drain(ctx);
   for (auto e : ctx->event_pool) cudaEventDestroy(e);

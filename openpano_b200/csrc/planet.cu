@@ -1,0 +1,121 @@
+// planet.cu — the "little planet" (stereographic) view of a mosaic.
+//
+// Replaces planet() (main.cc:294-331, the `planet` sub-command at :352-353) without its file I/O:
+// a PANO_PLANET_SIZE² (1000×1000) image whose pixel (i, j) samples the mosaic at
+//   row    = min(h - (hypot(center - i, center - j) / center) * h, h - 1)
+//   column = theta(i, j) / (2π) * w
+// with one bilinear interpolate (lib/imgproc.cc:135-156).  hypot and atan are the only libm calls,
+// and both depend on (i, j) alone: the host evaluates them once per process with the libm the
+// reference calls and stores d / center and theta / (2π) per pixel (the rule DESIGN.md §3 applies
+// to the warp's tan/cos tables).  Each context uploads that table on its first planet call and keeps
+// it until pano_destroy; the kernel then does only IEEE double arithmetic and the f32 gather.
+#include "common.cuh"
+#include <math.h>
+#include <vector>
+
+namespace {
+
+constexpr int kSize = PANO_PLANET_SIZE, kCenter = PANO_PLANET_SIZE / 2;   // main.cc:297 OUTSIZE, center
+constexpr size_t kPixels = (size_t)kSize * kSize;
+
+// x = d / center (main.cc:302-304), y = theta / (M_PI * 2) (:308-323, left operand of `* w`);
+// x = -1 marks the pixels the loop skips (d >= center || d == 0).
+const std::vector<double2>& planet_table() {
+  static const std::vector<double2> tab = [] {
+    std::vector<double2> t(kPixels);
+    for (int i = 0; i < kSize; ++i)
+      for (int j = 0; j < kSize; ++j) {
+        double2& e = t[(size_t)i * kSize + j];
+        const double d = hypot((double)(kCenter - i), (double)(kCenter - j));
+        if (d >= kCenter || d == 0) { e.x = -1.0; e.y = 0.0; continue; }
+        double theta;
+        if (j == kCenter) {
+          theta = i < kCenter ? M_PI / 2 : 3 * M_PI / 2;
+        } else {
+          theta = atan((double)(kCenter - i) / (kCenter - j));
+          if (theta < 0) theta += M_PI;
+          if ((theta == 0) && (j > kCenter)) theta += M_PI;
+          if (kCenter < i) theta += M_PI;
+        }
+        e.x = d / kCenter;
+        e.y = theta / (M_PI * 2);
+      }
+    return t;
+  }();
+  return tab;
+}
+
+int planet_table_dev(pano_ctx* ctx, const double2** out) {
+  if (!ctx->planet_tab) {
+    const std::vector<double2>& tab = planet_table();
+    void* p = nullptr;
+    PANO_CUDA(ctx, cudaMallocFromPoolAsync(&p, kPixels * sizeof(double2), ctx->pool, ctx->stream));
+    cudaError_t e = cudaMemcpyAsync(p, tab.data(), kPixels * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess) { cudaFreeAsync(p, ctx->stream); return ctx_cuda(ctx, e, "planet table upload"); }
+    ctx->planet_tab = (double2*)p;
+  }
+  *out = ctx->planet_tab;
+  return PANO_OK;
+}
+
+}  // namespace
+
+// one thread per output pixel (main.cc:301-329); every pixel is written, -1 where nothing maps
+__global__ void k_planet(const double2* __restrict__ tab, const float* __restrict__ src, int w, int h,
+                         float* __restrict__ dst) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  const int i = blockIdx.y * blockDim.y + threadIdx.y;
+  if (j >= kSize || i >= kSize) return;
+  const size_t k = (size_t)i * kSize + j;
+  const double2 t = __ldg(tab + k);
+  float o0 = -1.f, o1 = -1.f, o2 = -1.f;
+  if (t.x >= 0) {
+    const double hd = (double)h;
+    double dist = hd - t.x * hd;                 // :306
+    const double theta = t.y * (double)w;        // :323
+    if (hd - 1 < dist) dist = hd - 1;            // :325 update_min
+    float c0, c1, c2;
+    if (interpolate_rgb(src, w, h, (float)dist, (float)theta, &c0, &c1, &c2)) { o0 = c0; o1 = c1; o2 = c2; }
+  }
+  float* p = dst + k * 3;
+  p[0] = o0; p[1] = o1; p[2] = o2;
+}
+
+extern "C" {
+
+int pano_planet_dev(pano_ctx* ctx, const float* d_rgb_hwc, int w, int h, float* d_out_hwc) {
+  ctx_enter(ctx);
+  if (!ctx) return PANO_ERR_INVALID;
+  if (!d_rgb_hwc || !d_out_hwc || w < 1 || h < 1)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "planet: null pointer or empty %dx%d input", w, h);
+  const double2* tab = nullptr;
+  int rc = planet_table_dev(ctx, &tab);
+  if (rc) return rc;
+  dim3 b(32, 8), g(ceil_div(kSize, 32), ceil_div(kSize, 8));
+  PANO_LAUNCH(ctx, "k_planet", k_planet, g, b, 0, tab, d_rgb_hwc, w, h, d_out_hwc);
+  return PANO_OK;
+}
+
+int pano_planet(pano_ctx* ctx, const float* rgb_hwc, int w, int h, float* out_hwc) {
+  ctx_enter(ctx);
+  if (!ctx) return PANO_ERR_INVALID;
+  if (!rgb_hwc || !out_hwc || w < 1 || h < 1)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "planet: null pointer or empty %dx%d input", w, h);
+  const size_t bs = (size_t)w * h * 3 * sizeof(float), bd = kPixels * 3 * sizeof(float);
+  float *d_src = nullptr, *d_dst = nullptr;
+  int rc = 0;
+  if ((rc = ctx_alloc(ctx, (void**)&d_src, bs)) || (rc = ctx_alloc(ctx, (void**)&d_dst, bd))) {
+    ctx_free(ctx, d_src); ctx_free(ctx, d_dst);
+    return rc;
+  }
+  cudaError_t e = cudaMemcpyAsync(d_src, rgb_hwc, bs, cudaMemcpyHostToDevice, ctx->stream);
+  if (e != cudaSuccess) rc = ctx_cuda(ctx, e, "planet upload");
+  if (!rc) rc = pano_planet_dev(ctx, d_src, w, h, d_dst);
+  if (!rc && (e = cudaMemcpyAsync(out_hwc, d_dst, bd, cudaMemcpyDeviceToHost, ctx->stream)) != cudaSuccess)
+    rc = ctx_cuda(ctx, e, "planet download");
+  if (!rc && (e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess) rc = ctx_cuda(ctx, e, "pano_planet");
+  ctx_free(ctx, d_src); ctx_free(ctx, d_dst);
+  return rc;
+}
+
+}  // extern "C"

@@ -4,6 +4,7 @@
 //   PairWiseMatcher      feature/matcher.hh:40-67  (same constructor shape and match(i, j))
 //   BlenderBase          stitch/blender.hh:14-59
 //   CylinderWarper       stitch/warp.hh:41-66
+//   planet()             main.cc:294-331, the little-planet view: b200_planet
 //   the LM loop of IncrementalBundleAdjuster::optimize (stitch/incremental_bundle_adjuster.cc:117-169):
 //                        calcError and get_param_update's J / J^T J / b, B200BundleAdjusterStep
 // and forward to the C ABI of libpano_b200.so (include/pano_b200.h).  Header-only; compiles
@@ -220,6 +221,15 @@ class B200CylinderWarper {
   const Context& c_;
   real_t h_factor_;
 };
+
+// ---- the little-planet view: planet() (main.cc:294-331) without its file I/O, so that its body becomes
+//   write_rgb(IMGFILE(planet), b200_planet(ctx, read_img(fname)));
+inline Mat32f b200_planet(const Context& c, const Mat32f& img) {
+  m_assert(img.channels() == 3);
+  Mat32f out(PANO_PLANET_SIZE, PANO_PLANET_SIZE, 3);
+  c.check(pano_planet(c.get(), img.ptr(), img.width(), img.height(), out.ptr()));
+  return out;
+}
 
 // ---- Stitcher::build()'s hot path (stitcher.cc:32-64) on the engine: calc_feature ->
 // pairwise / linear match -> blend.  The geometry in between (RANSAC, camera estimation,
