@@ -95,6 +95,10 @@ void pano_destroy(pano_ctx* ctx);
  * 1.5 s).  The environment variable PANO_CACHE_MB bounds what a ctx keeps (default 32768, 0 = keep
  * nothing); pano_trim hands everything it keeps back to the pool, e.g. before a long idle period. */
 int  pano_trim(pano_ctx* ctx);
+/* The most device memory the ctx's pool has had in use (cudaMemPoolAttrUsedMemHigh) since creation
+ * or the last reset; reset != 0 restarts the mark at what is in use now.  Blocks the ctx keeps for
+ * reuse count as in use: set PANO_CACHE_MB=0 or call pano_trim first to see what a call needs. */
+int  pano_mem_high_water(pano_ctx* ctx, size_t* bytes, int reset);
 /* Message of the last failure on this ctx ("" if none).  ctx may be NULL for
  * the last pano_create failure. */
 const char* pano_last_error(const pano_ctx* ctx);
@@ -378,6 +382,54 @@ int pano_blend_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pan
 int pano_blend_rows_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g,
                         int bands, const pano_params* p, float* d_out_rows, int out_w, int out_h,
                         int row0, int row1);
+
+/* A blend whose sources arrive in windows: LAZY_READ's memory contract (config.cfg:10-11,
+ * blender.cc:38-64, multiband.cc:27,49) on the device.  The mosaic is bit-identical to pano_blend's
+ * for every partition of the images into windows and every source kind, 8-bit included: an 8-bit
+ * tap is converted exactly as pano_rgb8_to_mat32f_dev converts it.
+ *
+ * Device memory: besides the canvas state a stream never holds more than two windows of sources.
+ * The canvas state, allocated by pano_blend_stream_create, is
+ *   bands == 0: 16 B per canvas pixel (the colour sums and the weight plane);
+ *   bands > 0:  33 B per ROI pixel (two 4-plane f32 level buffers and a mask; ROI rows padded to 32
+ *               pixels) plus 1 B per canvas pixel (the target mask); pano_blend_stream_finish adds the
+ *               12 B per canvas pixel of the output;
+ * plus the per-image table and, for non-flat projections, 8 B per canvas row and column.  Host
+ * sources go through a two-slot device ring, each slot as large as the largest window uploaded
+ * through it; device sources are read in place and take no ring memory.
+ *
+ * Calls on a stream are calls on its ctx (same threading rule); the ctx must outlive it.  A misuse
+ * (null pointers, an unknown kind, channels other than 1 or 3 for 8-bit or 3 for f32 sources, out-of-order,
+ * overlapping or excess adds, finish before the last image or twice) returns PANO_ERR_INVALID, and
+ * every failure is sticky: later adds and finishes return it again.  pano_blend_stream_free is
+ * always valid, and the ctx stays usable. */
+typedef struct pano_blend_stream pano_blend_stream;
+typedef enum pano_src_kind {
+  PANO_SRC_F32_DEV = 0,    /* device, h×w×3 f32 (Mat32f layout) */
+  PANO_SRC_F32_HOST = 1,   /* host, h×w×3 f32 */
+  PANO_SRC_RGB8_DEV = 2,   /* device, h×w×channels u8 (read_img's input, lib/imgio.cc:75-88) */
+  PANO_SRC_RGB8_HOST = 3   /* host, h×w×channels u8 */
+} pano_src_kind;
+/* imgs / g / bands / p / out_w / out_h as for pano_blend; imgs[k].rgb_hwc is ignored and may be NULL.
+ * Builds the projection tables and allocates the canvas state. */
+int  pano_blend_stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g,
+                              int bands, const pano_params* p, int out_w, int out_h, pano_blend_stream** out);
+/* Adds images [first, first + count): first must be the number of images added so far.  srcs[i] is
+ * image first + i in the shape imgs[first + i] gave (w, h; channels for 8-bit kinds, 3 for f32).
+ * Host sources are uploaded on the stream's own copy stream while the previous window's kernels
+ * run.  PAGEABLE host buffers are staged and may be reused as soon as the call returns; PINNED ones
+ * (pano_host_alloc / cudaHostAlloc) are read by an asynchronous copy and must stay untouched until
+ * the add after the next one, or a finish, has returned.  Device sources are read by kernels queued
+ * on the ctx stream: work queued on that stream after this call (the next add, a finish,
+ * pano_dev_upload) may overwrite them; other streams wait for a pano_event recorded after it. */
+int  pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void* const* srcs, int kind,
+                           int channels);
+/* Valid once all n images have been added, once per stream.  _dev: d_out_hwc is a device buffer of
+ * out_h×out_w×3 f32, written asynchronously on the ctx stream; the host form returns when out_hwc
+ * holds the mosaic. */
+int  pano_blend_stream_finish_dev(pano_blend_stream* s, float* d_out_hwc);
+int  pano_blend_stream_finish(pano_blend_stream* s, float* out_hwc);
+void pano_blend_stream_free(pano_blend_stream* s);
 
 /* ---------------------------------------------------------- little planet
  * Replaces planet() (main.cc:294-331, the `planet` sub-command) without the file I/O: the

@@ -94,6 +94,13 @@ def _load():
                                      C.POINTER(PanoBlendGeom), C.c_int, P, C.c_void_p, C.c_int, C.c_int]),
         "pano_blend_rows_dev": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom),
                                           C.c_int, P, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
+        "pano_blend_stream_create": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom),
+                                               C.c_int, P, C.c_int, C.c_int, _vpp]),
+        "pano_blend_stream_add": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _vpp, C.c_int, C.c_int]),
+        "pano_blend_stream_finish_dev": (C.c_int, [C.c_void_p, C.c_void_p]),
+        "pano_blend_stream_finish": (C.c_int, [C.c_void_p, _fp]),
+        "pano_blend_stream_free": (None, [C.c_void_p]),
+        "pano_mem_high_water": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t), C.c_int]),
         "pano_planet": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, _fp]),
         "pano_planet_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
         "pano_featureset_import_dev": (C.c_int, [C.c_void_p, C.c_int, _ip, _vpp, _vpp, _vpp]),
@@ -292,6 +299,81 @@ class BaSession:
             pass
 
 
+# pano_src_kind
+SRC_F32_DEV, SRC_F32_HOST, SRC_RGB8_DEV, SRC_RGB8_HOST = 0, 1, 2, 3
+
+
+class BlendStream:
+    """A pano_blend_stream: the mosaic of pano_blend, fed window by window (LAZY_READ's memory contract).
+    add() takes numpy arrays (host; uint8 H×W / H×W×1 / H×W×3 or float32 H×W×3, the kind from the dtype) or
+    raw pointers with an explicit kind (SRC_*).  Every failure is sticky, as in the C ABI."""
+
+    def __init__(self, eng, handle, shapes, out_w, out_h):
+        self.eng, self._h = eng, handle
+        self.shapes, self.out_w, self.out_h = list(shapes), out_w, out_h
+        self.added = 0
+        self._err = None
+
+    def _fail(self, msg):
+        self._err = PanoError(-2, msg)
+        raise self._err
+
+    def _call(self, rc):
+        if rc != 0:
+            self._err = PanoError(rc, LIB.pano_last_error(self.eng._h).decode())
+            raise self._err
+
+    def add(self, srcs, kind=None, channels=None):
+        """Adds the next len(srcs) images."""
+        if self._err is not None:
+            raise self._err
+        keep = []
+        if kind is None:
+            arrs = list(srcs)
+            dts = {a.dtype for a in arrs}
+            if len(dts) != 1 or dts.pop() not in (np.uint8, np.float32):
+                self._fail("blend stream: sources must all be uint8 or all float32 numpy arrays")
+            u8 = arrs[0].dtype == np.uint8
+            kind = SRC_RGB8_HOST if u8 else SRC_F32_HOST
+            channels = None
+            for k, a in enumerate(arrs):
+                want = self.shapes[self.added + k] if self.added + k < len(self.shapes) else None
+                ch = 1 if a.ndim == 2 else (a.shape[2] if a.ndim == 3 else -1)
+                if want is None or a.shape[:2] != tuple(want) or (ch not in (1, 3) if u8 else ch != 3) or \
+                        (channels is not None and ch != channels):
+                    self._fail(f"blend stream: source {self.added + k} has shape {a.shape}, the stream expects "
+                               f"{want} with {'1 or 3 channels' if u8 else '3 channels'}, the same for the window")
+                channels = ch
+                keep.append(np.ascontiguousarray(a))
+            ptrs = [a.ctypes.data for a in keep]
+        else:
+            ptrs = [int(p or 0) for p in srcs]
+            channels = 3 if channels is None else channels
+        n = len(ptrs)
+        arr = (C.c_void_p * max(n, 1))(*ptrs)
+        self._call(LIB.pano_blend_stream_add(self._h, self.added, n, arr, kind, channels))
+        self.added += n
+
+    def finish(self):
+        out = np.empty((self.out_h, self.out_w, 3), np.float32)
+        self._call(LIB.pano_blend_stream_finish(self._h, _f(out)))
+        return out
+
+    def finish_dev(self, d_out):
+        self._call(LIB.pano_blend_stream_finish_dev(self._h, C.c_void_p(d_out or 0)))
+
+    def close(self):
+        if self._h:
+            LIB.pano_blend_stream_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Engine:
     """One pano_ctx: a CUDA device + stream.  `stream` is a raw cudaStream_t
     (e.g. torch.cuda.current_stream().cuda_stream) or None."""
@@ -336,6 +418,12 @@ class Engine:
 
     def launch_count(self):
         return LIB.pano_launch_count(self._h)
+
+    def mem_high_water(self, reset=False):
+        """Peak bytes in use in this context's device pool since creation or the last reset."""
+        v = C.c_size_t()
+        self._check(LIB.pano_mem_high_water(self._h, C.byref(v), 1 if reset else 0))
+        return v.value
 
     def match_last_exact_rows(self):
         return LIB.pano_match_last_exact_rows(self._h)
@@ -645,6 +733,33 @@ class Engine:
         arr, g = self._blend_args(ptrs, shapes, items, geom)
         self._check(LIB.pano_blend_dev(self._h, len(ptrs), arr, C.byref(g), bands, C.byref(params),
                                        C.c_void_p(d_out), out_w, out_h))
+
+    def blend_stream(self, shapes, items, geom, bands=0, params=None) -> BlendStream:
+        """shapes: (h, w) per image; items / geom as for blend().  Allocates the canvas state."""
+        params = params or default_params()
+        arr, g = self._blend_args([None] * len(items), shapes, items, geom)
+        ow, oh = C.c_int(), C.c_int()
+        self._check(LIB.pano_blend_target_size(len(items), arr, C.byref(ow), C.byref(oh)))
+        h = C.c_void_p()
+        self._check(LIB.pano_blend_stream_create(self._h, len(items), arr, C.byref(g), bands, C.byref(params), ow.value,
+                                                 oh.value, C.byref(h)))
+        return BlendStream(self, h, shapes, ow.value, oh.value)
+
+    def blend_lazy(self, imgs, items, geom, bands=0, params=None, window=1):
+        """blend() with the sources added `window` images at a time (an int, or a list of window sizes):
+        numpy uint8 (read_img's input: H×W, H×W×1 or H×W×3) or float32 H×W×3 images."""
+        sizes = window if isinstance(window, (list, tuple)) else None
+        s = self.blend_stream([im.shape[:2] for im in imgs], items, geom, bands, params)
+        try:
+            k = 0
+            for q in (sizes if sizes is not None else iter(lambda: window, None)):
+                if k >= len(imgs):
+                    break
+                s.add(imgs[k:k + q])
+                k += q
+            return s.finish()
+        finally:
+            s.close()
 
     # -- little planet (main.cc:294-331)
     PLANET_SIZE = 1000                 # PANO_PLANET_SIZE, main.cc:297

@@ -14,9 +14,13 @@
 #include <string.h>
 #include <vector>
 #include <algorithm>
+#include <climits>
 
 struct BlendImg {
-  const float* rgb;       // device
+  union {
+    const float* rgb;           // device, h×w×3 f32 (SrcF32)
+    const unsigned char* pix;   // device, h×w×channels u8 (SrcRgb8)
+  };
   int w, h;
   int x0, y0, x1, y1;
   double hi[9];
@@ -27,7 +31,14 @@ struct BlendImg {
   long long plane;        // floats per plane (pitch * rh)
   long long mask_off;     // first byte of the validity mask (same pitch)
   int rw, rh, pitch;
+  int channels;           // SrcRgb8 only: 1 or 3
 };
+
+template <class Src> __device__ __forceinline__ Src blend_src(const BlendImg& im, const float* lut);
+template <> __device__ __forceinline__ SrcF32 blend_src<SrcF32>(const BlendImg& im, const float*) { return SrcF32{im.rgb}; }
+template <> __device__ __forceinline__ SrcRgb8 blend_src<SrcRgb8>(const BlendImg& im, const float* lut) {
+  return SrcRgb8{im.pix, lut, im.channels};
+}
 
 struct BlendGeom {
   int projection;
@@ -89,20 +100,15 @@ __device__ __forceinline__ void build_tile_list(const BlendImg* __restrict__ img
 
 // ============================================================ linear blend
 // blender.cc:24-96.  lazy != 0 selects the LAZY_READ branch (exclusive max
-// bounds, accumulate then divide); otherwise the per-pixel branch.
-__global__ void k_linear_blend(const BlendImg* __restrict__ imgs, int n, BlendGeom g, int lazy, int ordered,
-                               float* __restrict__ out, int tw, int row0, int row1) {
-  // rows [row0, row1) of the canvas; `out` starts at row0 (a strip of a row-sharded mosaic, or the whole)
-  __shared__ TileList tl;
-  {
-    const int tj0 = blockIdx.x * blockDim.x, ti0 = row0 + blockIdx.y * blockDim.y;
-    build_tile_list(imgs, n, tj0, ti0, tj0 + blockDim.x - 1, ti0 + blockDim.y - 1, &tl);
-  }
-  int j = blockIdx.x * blockDim.x + threadIdx.x;
-  int i = row0 + blockIdx.y * blockDim.y + threadIdx.y;
-  if (j >= tw || i >= row1) return;
+// bounds, accumulate then divide); otherwise the per-pixel branch.  Both add c·w and w
+// of every covering image in image order, starting from 0.
+
+// Adds the contributions of imgs[0, n) (tile list tl) at canvas pixel (i, j) to the sums.
+template <class Src>
+__device__ __forceinline__ void linear_add_px(const BlendImg* __restrict__ imgs, int n, const TileList& tl,
+                                              const BlendGeom& g, int lazy, int ordered, const float* lut, int i, int j,
+                                              float& s0, float& s1, float& s2, float& wsum) {
   const int nl = tl.n < 0 ? n : tl.n;
-  float s0 = 0.f, s1 = 0.f, s2 = 0.f, wsum = 0.f;
   for (int q = 0; q < nl; ++q) {
     const BlendImg& im = imgs[tl.n < 0 ? q : (int)tl.idx[q]];
     bool in = lazy ? (i >= im.y0 && i < im.y1 && j >= im.x0 && j < im.x1)
@@ -113,14 +119,17 @@ __global__ void k_linear_blend(const BlendImg* __restrict__ imgs, int n, BlendGe
     if (x < 0 || x >= im.w || y < 0 || y >= im.h) continue;       // map_coor -> NaN
     float r = (float)y, c = (float)x;
     float c0, c1, c2;
-    if (!interpolate_rgb(im.rgb, im.w, im.h, r, c, &c0, &c1, &c2)) continue;
+    if (!interpolate_rgb(blend_src<Src>(im, lut), im.w, im.h, r, c, &c0, &c1, &c2)) continue;
     if (c0 < 0) continue;
     float w = (float)(0.5 - fabs((double)(c / (float)im.w) - 0.5));
     if (!ordered) w = (float)((double)w * (0.5 - fabs((double)(r / (float)im.h) - 0.5)));
     s0 += c0 * w; s1 += c1 * w; s2 += c2 * w;
     wsum += w;
   }
-  float* p = out + ((size_t)(i - row0) * tw + j) * 3;
+}
+
+// The final step of both branches: blender.cc:66-76 (lazy) and :91-92, -1 where nothing was added.
+__device__ __forceinline__ void linear_resolve_px(int lazy, float s0, float s1, float s2, float wsum, float* p) {
   if (lazy) {
     if (wsum != 0.f) { p[0] = s0 / wsum; p[1] = s1 / wsum; p[2] = s2 / wsum; }
     else { p[0] = -1.f; p[1] = -1.f; p[2] = -1.f; }
@@ -132,10 +141,65 @@ __global__ void k_linear_blend(const BlendImg* __restrict__ imgs, int n, BlendGe
   }
 }
 
+__global__ void k_linear_blend(const BlendImg* __restrict__ imgs, int n, BlendGeom g, int lazy, int ordered,
+                               float* __restrict__ out, int tw, int row0, int row1) {
+  // rows [row0, row1) of the canvas; `out` starts at row0 (a strip of a row-sharded mosaic, or the whole)
+  __shared__ TileList tl;
+  {
+    const int tj0 = blockIdx.x * blockDim.x, ti0 = row0 + blockIdx.y * blockDim.y;
+    build_tile_list(imgs, n, tj0, ti0, tj0 + blockDim.x - 1, ti0 + blockDim.y - 1, &tl);
+  }
+  int j = blockIdx.x * blockDim.x + threadIdx.x;
+  int i = row0 + blockIdx.y * blockDim.y + threadIdx.y;
+  if (j >= tw || i >= row1) return;
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f, wsum = 0.f;
+  linear_add_px<SrcF32>(imgs, n, tl, g, lazy, ordered, nullptr, i, j, s0, s1, s2, wsum);
+  linear_resolve_px(lazy, s0, s1, s2, wsum, out + ((size_t)(i - row0) * tw + j) * 3);
+}
+
+// One window of a blend stream: adds imgs[0, n) into the persistent sums (sum: tw×th×3, wsum:
+// tw×th, both zero at the start), one thread per pixel of the window's bounding rectangle
+// [rx0, rx1) × [ry0, ry1).  Windows run in image order, so every pixel sees the float additions
+// of k_linear_blend in the same order.
+template <class Src>
+__global__ void k_linear_accumulate(const BlendImg* __restrict__ imgs, int n, BlendGeom g, int lazy, int ordered,
+                                    float* __restrict__ sum, float* __restrict__ wsum, int tw, int rx0, int ry0, int rx1,
+                                    int ry1) {
+  __shared__ TileList tl;
+  __shared__ float lut[Src::kLut ? 256 : 1];
+  if constexpr (Src::kLut) build_rgb8_lut(lut, threadIdx.y * blockDim.x + threadIdx.x);   // ordered by the list's barrier
+  const int tj0 = rx0 + blockIdx.x * blockDim.x, ti0 = ry0 + blockIdx.y * blockDim.y;
+  build_tile_list(imgs, n, tj0, ti0, tj0 + blockDim.x - 1, ti0 + blockDim.y - 1, &tl);
+  const int j = tj0 + threadIdx.x, i = ti0 + threadIdx.y;
+  if (tl.n == 0 || j >= rx1 || i >= ry1) return;
+  const size_t t = (size_t)i * tw + j;
+  float* p = sum + t * 3;
+  float s0 = p[0], s1 = p[1], s2 = p[2], ws = wsum[t];
+  linear_add_px<Src>(imgs, n, tl, g, lazy, ordered, lut, i, j, s0, s1, s2, ws);
+  p[0] = s0; p[1] = s1; p[2] = s2;
+  wsum[t] = ws;
+}
+
+// The stream's last step: k_linear_blend's tail on the sums.  out may be `sum` itself.
+__global__ void k_linear_resolve(const float* sum, const float* __restrict__ wsum, float* out, size_t n_px, int lazy) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_px) return;
+  const float* p = sum + t * 3;
+  linear_resolve_px(lazy, p[0], p[1], p[2], wsum[t], out + t * 3);
+}
+
 // ============================================================ multiband
 // multiband.cc:19-57 create_first_level
+// The first level of an image depends on that image only: a blend stream runs this once per
+// window over the window's entries.
+template <class Src>
 __global__ void k_mb_first_level(const BlendImg* __restrict__ imgs, BlendGeom g, float* __restrict__ cur,
                                  unsigned char* __restrict__ mask) {
+  __shared__ float lut[Src::kLut ? 256 : 1];
+  if constexpr (Src::kLut) {
+    build_rgb8_lut(lut, threadIdx.y * blockDim.x + threadIdx.x);
+    __syncthreads();
+  }
   const BlendImg& im = imgs[blockIdx.z];
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   int i = blockIdx.y * blockDim.y + threadIdx.y;
@@ -143,7 +207,7 @@ __global__ void k_mb_first_level(const BlendImg* __restrict__ imgs, BlendGeom g,
   double x, y;
   coor_func(im, g, j + im.x0, i + im.y0, &x, &y);
   float c0, c1, c2;
-  bool ok = interpolate_rgb(im.rgb, im.w, im.h, (float)y, (float)x, &c0, &c1, &c2);
+  bool ok = interpolate_rgb(blend_src<Src>(im, lut), im.w, im.h, (float)y, (float)x, &c0, &c1, &c2);
   if (ok && fminf(c0, fminf(c1, c2)) < 0) ok = false;
   const size_t o = (size_t)i * im.pitch + j;
   float* p = cur + im.roi_off + o;
@@ -372,6 +436,7 @@ __global__ void k_fill(float* __restrict__ p, size_t n, float v) {
 
 // ------------------------------------------------------------------ host driver
 
+// Everything a blend derives from its arguments on the host, before any device work.
 struct BlendJob {
   std::vector<BlendImg> imgs;
   BlendGeom g;
@@ -379,6 +444,27 @@ struct BlendJob {
   long long roi_floats = 0;   // floats of one level buffer (4 planes per image)
   long long mask_bytes = 0;
   int max_rw = 0, max_rh = 0;
+  std::vector<BlurTaps> level_taps;
+  int halo = 0;               // summed half-widths of the level blurs
+  bool strip = false;
+  int clip0 = INT_MIN, clip1 = INT_MAX;
+  std::vector<double> tab;    // sin / cos per canvas column, tan per row (non-flat projections)
+  size_t ncol = 0, nrow = 0;
+};
+
+// The device state of one blend: image table, projection tables and, for multiband, the ROI level
+// buffers, masks, target mask and blur tables.
+struct BlendDev {
+  BlendImg* d_imgs = nullptr;
+  double* d_tab = nullptr;
+  float *d_cur = nullptr, *d_next = nullptr;
+  unsigned char *d_mask = nullptr, *d_tmask = nullptr;
+  MbPlane* d_planes = nullptr;
+  int2* d_span = nullptr;
+  TmaDesc* d_maps = nullptr;
+  std::vector<int> centers;   // distinct TMA blur half-widths
+  int n_planes = 0, n_tiles = 0;
+  int wrow0 = 0, wrow1 = 0;   // rows the weight map is needed on
 };
 
 #define BL_LAUNCH(ctx, name, kernel, grid, block, smem, ...)                        \
@@ -388,7 +474,7 @@ struct BlendJob {
     kernel<<<(grid), (block), (smem), (ctx)->stream>>>(__VA_ARGS__);                \
     if ((ctx)->profiling) ctx_prof_end((ctx));                                      \
     cudaError_t _e = cudaGetLastError();                                            \
-    if (_e != cudaSuccess) { rc = ctx_cuda((ctx), _e, name); goto done; }           \
+    if (_e != cudaSuccess) return ctx_cuda((ctx), _e, name);                        \
   } while (0)
 
 template <int C>
@@ -402,19 +488,14 @@ static cudaError_t launch_mb_blur_tma(pano_ctx* ctx, int grid, const MbPlane* pl
   return cudaGetLastError();
 }
 
-static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
-                        const pano_params* p, float* d_out, int ow, int oh, int row0, int row1) {
-  if (!ctx || n <= 0 || !imgs || !g || !p || !d_out || bands < 0) return PANO_ERR_INVALID;
-  if (row0 < 0 || row1 > oh || row0 > row1)
-    return ctx_fail(ctx, PANO_ERR_INVALID, "blend: rows [%d, %d) outside the %d-row canvas", row0, row1, oh);
-  if (row0 == row1) return PANO_OK;
+// Validates the images (need_src: every rgb_hwc must be set) and builds the job of rows [row0, row1).
+static int blend_plan(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
+                      const pano_params* p, int ow, int oh, int row0, int row1, bool need_src, BlendJob* job) {
   // Multiband on a row strip: a band at level l of pixel p depends on level 0 inside a
   // radius of the summed half-widths of the blurs up to l, so the strip is computed from
   // each image's ROI clipped to [row0 - H, row1 + H) with H = that sum over all blurred
   // levels.  The replicate rule at a clipped edge differs from the true neighbourhood only
   // within H rows of it, i.e. outside the strip; true ROI edges are kept as they are.
-  std::vector<BlurTaps> level_taps;
-  int halo = 0;
   for (int level = 0; level + 1 < bands; ++level) {   // multiband.cc:145-151
     float sigma = (float)(sqrt(level * 2 + 1.0) * 4);
     BlurTaps bt;
@@ -422,173 +503,348 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
     int kw = host_gauss_kernel(sigma, p->gauss_window_factor, bt.taps, 63);
     if (kw < 0) return ctx_fail(ctx, PANO_ERR_INVALID, "blend: gaussian window %d too wide", -kw);
     bt.center = kw / 2;
-    halo += bt.center;
-    level_taps.push_back(bt);
+    job->halo += bt.center;
+    job->level_taps.push_back(bt);
   }
-  const bool strip = bands > 0 && (row0 != 0 || row1 != oh);
-  const int clip0 = (strip && row0 > 0) ? std::max(0, row0 - halo) : INT_MIN;          // first ROI row kept
-  const int clip1 = (strip && row1 < oh) ? row1 + halo - 1 : INT_MAX;                  // last ROI row kept
-  BlendJob job;
-  job.imgs.reserve(n);
+  job->strip = bands > 0 && (row0 != 0 || row1 != oh);
+  job->clip0 = (job->strip && row0 > 0) ? std::max(0, row0 - job->halo) : INT_MIN;    // first ROI row kept
+  job->clip1 = (job->strip && row1 < oh) ? row1 + job->halo - 1 : INT_MAX;            // last ROI row kept
+  job->imgs.reserve(n);
   for (int k = 0; k < n; ++k) {
     const pano_blend_image& s = imgs[k];
-    if (!s.rgb_hwc || s.w < 2 || s.h < 2 || s.x1 < s.x0 || s.y1 < s.y0 || s.x0 < 0 || s.y0 < 0)
+    if ((need_src && !s.rgb_hwc) || s.w < 2 || s.h < 2 || s.x1 < s.x0 || s.y1 < s.y0 || s.x0 < 0 || s.y0 < 0)
       return ctx_fail(ctx, PANO_ERR_INVALID, "blend: image %d has an invalid shape or range", k);
-    job.tw = std::max(job.tw, s.x1); job.th = std::max(job.th, s.y1);
+    job->tw = std::max(job->tw, s.x1); job->th = std::max(job->th, s.y1);
     BlendImg d;
+    memset(&d, 0, sizeof(d));
     d.rgb = s.rgb_hwc; d.w = s.w; d.h = s.h;
     d.x0 = s.x0; d.x1 = s.x1;
-    d.y0 = std::max(s.y0, clip0); d.y1 = std::min(s.y1, clip1);
+    d.y0 = std::max(s.y0, job->clip0); d.y1 = std::min(s.y1, job->clip1);
     if (d.y0 > d.y1) continue;                         // no row of this image reaches the strip
     memcpy(d.hi, s.homo_inv, sizeof(d.hi));
     d.rw = d.x1 - d.x0 + 1; d.rh = d.y1 - d.y0 + 1;
     d.pitch = (int)align_up((size_t)d.rw, 32);
     d.plane = (long long)d.pitch * d.rh;
-    d.roi_off = job.roi_floats;
-    d.mask_off = job.mask_bytes;
-    job.roi_floats += 4 * d.plane;
-    job.mask_bytes += d.plane;
-    job.max_rw = std::max(job.max_rw, d.rw); job.max_rh = std::max(job.max_rh, d.rh);
-    job.imgs.push_back(d);
+    d.roi_off = job->roi_floats;
+    d.mask_off = job->mask_bytes;
+    d.channels = 3;
+    job->roi_floats += 4 * d.plane;
+    job->mask_bytes += d.plane;
+    job->max_rw = std::max(job->max_rw, d.rw); job->max_rh = std::max(job->max_rh, d.rh);
+    job->imgs.push_back(d);
   }
-  if (job.tw != ow || job.th != oh || ow <= 0 || oh <= 0)
-    return ctx_fail(ctx, PANO_ERR_INVALID, "blend: output is %dx%d but target_size is %dx%d", ow, oh, job.tw, job.th);
-  const int tw = job.tw, th = job.th;
-  n = (int)job.imgs.size();                            // images that reach the strip (all of them for a full canvas)
-  if (n == 0) {
-    size_t nfl = (size_t)tw * (row1 - row0) * 3;
+  if (job->tw != ow || job->th != oh || ow <= 0 || oh <= 0)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "blend: output is %dx%d but target_size is %dx%d", ow, oh, job->tw, job->th);
+  if (job->imgs.empty()) return PANO_OK;
+  // ROIs reach one pixel past the canvas (inclusive max): tables cover [0, tw] / [0, th]
+  job->ncol = (size_t)job->tw + 2; job->nrow = (size_t)job->th + 2;
+  if (g->projection != PANO_PROJ_FLAT) {
+    job->tab.resize(2 * job->ncol + job->nrow);
+    for (size_t j = 0; j < job->ncol; ++j) {
+      double cx = (double)j * g->res_x + g->proj_min_x;
+      job->tab[j] = sin(cx); job->tab[job->ncol + j] = cos(cx);
+    }
+    for (size_t i = 0; i < job->nrow; ++i) {
+      double cy = (double)i * g->res_y + g->proj_min_y;
+      job->tab[2 * job->ncol + i] = tan(cy);
+    }
+  }
+  job->g.projection = g->projection; job->g.res_x = g->res_x; job->g.res_y = g->res_y;
+  job->g.min_x = g->proj_min_x; job->g.min_y = g->proj_min_y;
+  return PANO_OK;
+}
+
+static void blend_dev_free(pano_ctx* ctx, BlendDev* d) {
+  ctx_free(ctx, d->d_imgs); ctx_free(ctx, d->d_tab); ctx_free(ctx, d->d_cur); ctx_free(ctx, d->d_next);
+  ctx_free(ctx, d->d_mask); ctx_free(ctx, d->d_tmask); ctx_free(ctx, d->d_planes); ctx_free(ctx, d->d_span);
+  ctx_free(ctx, d->d_maps);
+  *d = BlendDev();
+}
+
+// Allocates and uploads the device state of `job` (rows [row0, row1)); on failure the caller frees *d.
+static int blend_dev_setup(pano_ctx* ctx, BlendJob* job, int bands, int row0, int row1, BlendDev* d) {
+  const int n = (int)job->imgs.size(), tw = job->tw, th = job->th;
+  int rc = 0;
+  if ((rc = ctx_alloc(ctx, (void**)&d->d_imgs, n * sizeof(BlendImg)))) return rc;
+  if ((rc = ctx_alloc(ctx, (void**)&d->d_tab, std::max<size_t>(job->tab.size(), 1) * sizeof(double)))) return rc;
+  {
+    void* dsts[2] = {d->d_imgs, d->d_tab};
+    const void* srcs[2] = {job->imgs.data(), job->tab.data()};
+    size_t sizes[2] = {n * sizeof(BlendImg), job->tab.size() * sizeof(double)};
+    if ((rc = ctx_put_many(ctx, 2, dsts, srcs, sizes))) return rc;
+  }
+  job->g.col_sin = d->d_tab; job->g.col_cos = d->d_tab + job->ncol; job->g.row_tan = d->d_tab + 2 * job->ncol;
+  if (bands == 0) return PANO_OK;
+  const size_t roi = (size_t)job->roi_floats;
+  if ((rc = ctx_alloc(ctx, (void**)&d->d_cur, roi * sizeof(float)))) return rc;
+  if ((rc = ctx_alloc(ctx, (void**)&d->d_next, roi * sizeof(float)))) return rc;
+  if ((rc = ctx_alloc(ctx, (void**)&d->d_mask, (size_t)job->mask_bytes))) return rc;
+  const size_t strip_px = (size_t)tw * (row1 - row0);
+  // the weight map is needed wherever a clipped ROI has pixels on the canvas
+  d->wrow0 = std::max(0, std::max(row0 - job->halo, job->clip0));
+  d->wrow1 = std::min(th, job->strip ? row1 + job->halo : th);
+  if ((rc = ctx_alloc(ctx, (void**)&d->d_tmask, strip_px))) return rc;
+  // plane table of the blur launches: (image, channel) -> offset, size; tiles of 64x32
+  d->n_planes = 4 * n;
+  std::vector<MbPlane> planes(d->n_planes);
+  std::vector<int2> span(d->n_planes);
+  for (int k = 0; k < n; ++k)
+    for (int ch = 0; ch < 4; ++ch) {
+      const BlendImg& im = job->imgs[k];
+      planes[4 * k + ch] = MbPlane{im.roi_off + ch * im.plane, im.rw, im.rh, im.pitch, 0};
+      span[4 * k + ch] = make_int2(d->n_tiles, ceil_div(im.rw, BT_W));
+      d->n_tiles += ceil_div(im.rw, BT_W) * ceil_div(im.rh, BT_H);
+    }
+  if (bands > 1) {
+    if ((rc = ctx_alloc(ctx, (void**)&d->d_planes, d->n_planes * sizeof(MbPlane)))) return rc;
+    if ((rc = ctx_alloc(ctx, (void**)&d->d_span, d->n_planes * sizeof(int2)))) return rc;
+    if ((rc = ctx_put(ctx, d->d_planes, planes.data(), d->n_planes * sizeof(MbPlane)))) return rc;
+    if ((rc = ctx_put(ctx, d->d_span, span.data(), d->n_planes * sizeof(int2)))) return rc;
+  }
+  // TMA descriptors: one per (plane, level buffer, distinct window half-width)
+  for (auto& bt : job->level_taps)
+    if ((bt.center == 6 || bt.center == 9) && std::find(d->centers.begin(), d->centers.end(), bt.center) == d->centers.end())
+      d->centers.push_back(bt.center);
+  if (!d->centers.empty()) {
+    std::vector<TmaDesc> maps((size_t)d->centers.size() * 2 * d->n_planes);
+    for (size_t ci = 0; ci < d->centers.size(); ++ci)
+      for (int buf = 0; buf < 2; ++buf)
+        for (int q = 0; q < d->n_planes; ++q) {
+          const MbPlane& pl = planes[q];
+          const int C = d->centers[ci];
+          unsigned long long dims[2] = {(unsigned long long)pl.w, (unsigned long long)pl.h};
+          unsigned long long strides[1] = {(unsigned long long)pl.pitch * sizeof(float)};
+          unsigned box[2] = {(unsigned)(BT_W + 2 * ((C + 3) & ~3)), (unsigned)(BT_H + 2 * C)};
+          if ((rc = ctx_tma_encode(ctx, &maps[(ci * 2 + buf) * d->n_planes + q], (buf ? d->d_next : d->d_cur) + pl.off, 2,
+                                   dims, strides, box)))
+            return rc;
+        }
+    if ((rc = ctx_alloc(ctx, (void**)&d->d_maps, maps.size() * sizeof(TmaDesc)))) return rc;
+    if ((rc = ctx_put(ctx, d->d_maps, maps.data(), maps.size() * sizeof(TmaDesc)))) return rc;
+  }
+  return PANO_OK;
+}
+
+// multiband.cc:59-151 after create_first_level: the weight map, then per level blur + accumulate
+// into rows [row0, row1) of d_out.  Every image's first level must be in d_cur.
+static int mb_levels(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands, float* d_out, int row0, int row1) {
+  const int n = (int)job.imgs.size(), tw = job.tw;
+  const dim3 b(32, 8);
+  dim3 gw(ceil_div(tw, 32), ceil_div(d->wrow1 - d->wrow0, 8)), gs(ceil_div(tw, 32), ceil_div(row1 - row0, 8));
+  BL_LAUNCH(ctx, "k_mb_weight_argmax", k_mb_weight_argmax, gw, b, 0, d->d_imgs, n, d->d_cur, tw, d->wrow0, d->wrow1);
+  float *cur = d->d_cur, *next = d->d_next;
+  int buf = 0;     // which level buffer `cur` currently is (0: the first allocation)
+  for (int level = 0; level < bands; ++level) {
+    int is_last = level == bands - 1;
+    if (!is_last) {
+      const BlurTaps& bt = job.level_taps[level];
+      const int c = bt.center;
+      cudaError_t e = cudaSuccess;
+      ctx->launches++;
+      if (ctx->profiling) ctx_prof_begin(ctx, "k_mb_blur");
+      auto ci = std::find(d->centers.begin(), d->centers.end(), c);
+      if (ci != d->centers.end()) {
+        const TmaDesc* maps = d->d_maps + ((size_t)(ci - d->centers.begin()) * 2 + buf) * d->n_planes;
+        const int grid = std::min(d->n_tiles, ctx->num_sms * 4);
+        e = c == 6 ? launch_mb_blur_tma<6>(ctx, grid, d->d_planes, d->d_span, d->n_planes, d->n_tiles, maps, next, bt)
+                   : launch_mb_blur_tma<9>(ctx, grid, d->d_planes, d->d_span, d->n_planes, d->n_tiles, maps, next, bt);
+      } else {
+        const size_t smem = sizeof(float) * ((size_t)(MB_TH + 2 * c) * (MB_TW + 2 * c) + (size_t)MB_TH * (MB_TW + 2 * c));
+        if (smem > 200 * 1024) {
+          if (ctx->profiling) ctx_prof_end(ctx);
+          return ctx_fail(ctx, PANO_ERR_INVALID, "blend: gaussian window %d too wide", 2 * c + 1);
+        }
+        e = cudaFuncSetAttribute(k_mb_blur_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e == cudaSuccess) {
+          k_mb_blur_generic<<<d->n_tiles, 256, smem, ctx->stream>>>(d->d_planes, d->d_span, d->n_planes, cur, next, bt);
+          e = cudaGetLastError();
+        }
+      }
+      if (ctx->profiling) ctx_prof_end(ctx);
+      if (e != cudaSuccess) return ctx_cuda(ctx, e, "k_mb_blur");
+    }
+    BL_LAUNCH(ctx, "k_mb_accumulate", k_mb_accumulate, gs, b, 0, d->d_imgs, n, cur, next, d->d_mask, level == 0 ? 1 : 0,
+              is_last, d_out, d->d_tmask, tw, row0, row1);
+    if (!is_last) { std::swap(cur, next); buf ^= 1; }
+  }
+  return PANO_OK;
+}
+
+static int blend_run(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands, const pano_params* p, float* d_out,
+                     int row0, int row1) {
+  const int n = (int)job.imgs.size(), tw = job.tw;
+  const dim3 b(32, 8);
+  if (bands == 0) {
+    dim3 gs(ceil_div(tw, 32), ceil_div(row1 - row0, 8));
+    BL_LAUNCH(ctx, "k_linear_blend", k_linear_blend, gs, b, 0, d->d_imgs, n, job.g, p->lazy_read, p->ordered_input, d_out,
+              tw, row0, row1);
+    return PANO_OK;
+  }
+  dim3 gr(ceil_div(job.max_rw, 32), ceil_div(job.max_rh, 8), n);
+  BL_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<SrcF32>, gr, b, 0, d->d_imgs, job.g, d->d_cur, d->d_mask);
+  return mb_levels(ctx, job, d, bands, d_out, row0, row1);
+}
+
+static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
+                        const pano_params* p, float* d_out, int ow, int oh, int row0, int row1) {
+  if (!ctx || n <= 0 || !imgs || !g || !p || !d_out || bands < 0) return PANO_ERR_INVALID;
+  if (row0 < 0 || row1 > oh || row0 > row1)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "blend: rows [%d, %d) outside the %d-row canvas", row0, row1, oh);
+  if (row0 == row1) return PANO_OK;
+  BlendJob job;
+  int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, row0, row1, true, &job);
+  if (rc) return rc;
+  if (job.imgs.empty()) {                              // no image reaches the strip
+    size_t nfl = (size_t)job.tw * (row1 - row0) * 3;
     PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((nfl + 255) / 256), 256, 0, d_out, nfl, -1.f);
     return PANO_OK;
   }
-  // ROIs reach one pixel past the canvas (inclusive max): tables cover [0, tw] / [0, th]
-  std::vector<double> tab;
-  size_t ncol = (size_t)tw + 2, nrow = (size_t)th + 2;
-  if (g->projection != PANO_PROJ_FLAT) {
-    tab.resize(2 * ncol + nrow);
-    for (size_t j = 0; j < ncol; ++j) {
-      double cx = (double)j * g->res_x + g->proj_min_x;
-      tab[j] = sin(cx); tab[ncol + j] = cos(cx);
-    }
-    for (size_t i = 0; i < nrow; ++i) {
-      double cy = (double)i * g->res_y + g->proj_min_y;
-      tab[2 * ncol + i] = tan(cy);
-    }
-  }
-  int rc = 0;
-  BlendImg* d_imgs = nullptr;
-  double* d_tab = nullptr;
-  float *d_cur = nullptr, *d_next = nullptr;
-  unsigned char *d_mask = nullptr, *d_tmask = nullptr;
-  MbPlane* d_planes = nullptr;
-  int2* d_span = nullptr;
-  TmaDesc* d_maps = nullptr;
-  cudaError_t e = cudaSuccess;
-  if ((rc = ctx_alloc(ctx, (void**)&d_imgs, n * sizeof(BlendImg)))) goto done;
-  if ((rc = ctx_alloc(ctx, (void**)&d_tab, std::max<size_t>(tab.size(), 1) * sizeof(double)))) goto done;
-  {
-    void* dsts[2] = {d_imgs, d_tab};
-    const void* srcs[2] = {job.imgs.data(), tab.data()};
-    size_t sizes[2] = {n * sizeof(BlendImg), tab.size() * sizeof(double)};
-    if ((rc = ctx_put_many(ctx, 2, dsts, srcs, sizes))) goto done;
-  }
-  job.g.projection = g->projection; job.g.res_x = g->res_x; job.g.res_y = g->res_y;
-  job.g.min_x = g->proj_min_x; job.g.min_y = g->proj_min_y;
-  job.g.col_sin = d_tab; job.g.col_cos = d_tab + ncol; job.g.row_tan = d_tab + 2 * ncol;
-  {
-    dim3 b(32, 8);
-    if (bands == 0) {
-      dim3 gs(ceil_div(tw, 32), ceil_div(row1 - row0, 8));
-      BL_LAUNCH(ctx, "k_linear_blend", k_linear_blend, gs, b, 0, d_imgs, n, job.g, p->lazy_read, p->ordered_input, d_out, tw,
-                row0, row1);
-    } else {
-      const size_t roi = (size_t)job.roi_floats;
-      if ((rc = ctx_alloc(ctx, (void**)&d_cur, roi * sizeof(float)))) goto done;
-      if ((rc = ctx_alloc(ctx, (void**)&d_next, roi * sizeof(float)))) goto done;
-      if ((rc = ctx_alloc(ctx, (void**)&d_mask, (size_t)job.mask_bytes))) goto done;
-      const size_t strip_px = (size_t)tw * (row1 - row0);
-      // the weight map is needed wherever a clipped ROI has pixels on the canvas
-      const int wrow0 = std::max(0, std::max(row0 - halo, clip0)), wrow1 = std::min(th, strip ? row1 + halo : th);
-      if ((rc = ctx_alloc(ctx, (void**)&d_tmask, strip_px))) goto done;
-      // plane table of the blur launches: (image, channel) -> offset, size; tiles of 64x32
-      const int n_planes = 4 * n;
-      std::vector<MbPlane> planes(n_planes);
-      std::vector<int2> span(n_planes);
-      int n_tiles = 0;
-      for (int k = 0; k < n; ++k)
-        for (int ch = 0; ch < 4; ++ch) {
-          const BlendImg& im = job.imgs[k];
-          planes[4 * k + ch] = MbPlane{im.roi_off + ch * im.plane, im.rw, im.rh, im.pitch, 0};
-          span[4 * k + ch] = make_int2(n_tiles, ceil_div(im.rw, BT_W));
-          n_tiles += ceil_div(im.rw, BT_W) * ceil_div(im.rh, BT_H);
-        }
-      if (bands > 1) {
-        if ((rc = ctx_alloc(ctx, (void**)&d_planes, n_planes * sizeof(MbPlane)))) goto done;
-        if ((rc = ctx_alloc(ctx, (void**)&d_span, n_planes * sizeof(int2)))) goto done;
-        if ((rc = ctx_put(ctx, d_planes, planes.data(), n_planes * sizeof(MbPlane)))) goto done;
-        if ((rc = ctx_put(ctx, d_span, span.data(), n_planes * sizeof(int2)))) goto done;
-      }
-      // TMA descriptors: one per (plane, level buffer, distinct window half-width)
-      std::vector<int> centers;
-      for (auto& bt : level_taps)
-        if ((bt.center == 6 || bt.center == 9) && std::find(centers.begin(), centers.end(), bt.center) == centers.end())
-          centers.push_back(bt.center);
-      if (!centers.empty()) {
-        std::vector<TmaDesc> maps((size_t)centers.size() * 2 * n_planes);
-        for (size_t ci = 0; ci < centers.size(); ++ci)
-          for (int buf = 0; buf < 2; ++buf)
-            for (int q = 0; q < n_planes; ++q) {
-              const MbPlane& pl = planes[q];
-              const int C = centers[ci];
-              unsigned long long dims[2] = {(unsigned long long)pl.w, (unsigned long long)pl.h};
-              unsigned long long strides[1] = {(unsigned long long)pl.pitch * sizeof(float)};
-              unsigned box[2] = {(unsigned)(BT_W + 2 * ((C + 3) & ~3)), (unsigned)(BT_H + 2 * C)};
-              if ((rc = ctx_tma_encode(ctx, &maps[(ci * 2 + buf) * n_planes + q], (buf ? d_next : d_cur) + pl.off, 2, dims,
-                                       strides, box)))
-                goto done;
-            }
-        if ((rc = ctx_alloc(ctx, (void**)&d_maps, maps.size() * sizeof(TmaDesc)))) goto done;
-        if ((rc = ctx_put(ctx, d_maps, maps.data(), maps.size() * sizeof(TmaDesc)))) goto done;
-      }
-      dim3 gr(ceil_div(job.max_rw, 32), ceil_div(job.max_rh, 8), n);
-      dim3 gw(ceil_div(tw, 32), ceil_div(wrow1 - wrow0, 8)), gs(ceil_div(tw, 32), ceil_div(row1 - row0, 8));
-      BL_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level, gr, b, 0, d_imgs, job.g, d_cur, d_mask);
-      BL_LAUNCH(ctx, "k_mb_weight_argmax", k_mb_weight_argmax, gw, b, 0, d_imgs, n, d_cur, tw, wrow0, wrow1);
-      int buf = 0;     // which level buffer `d_cur` currently is (0: the first allocation)
-      for (int level = 0; level < bands; ++level) {
-        int is_last = level == bands - 1;
-        if (!is_last) {
-          const BlurTaps& bt = level_taps[level];
-          const int c = bt.center;
-          ctx->launches++;
-          if (ctx->profiling) ctx_prof_begin(ctx, "k_mb_blur");
-          auto ci = std::find(centers.begin(), centers.end(), c);
-          if (ci != centers.end()) {
-            const TmaDesc* maps = d_maps + ((size_t)(ci - centers.begin()) * 2 + buf) * n_planes;
-            const int grid = std::min(n_tiles, ctx->num_sms * 4);
-            e = c == 6 ? launch_mb_blur_tma<6>(ctx, grid, d_planes, d_span, n_planes, n_tiles, maps, d_next, bt)
-                       : launch_mb_blur_tma<9>(ctx, grid, d_planes, d_span, n_planes, n_tiles, maps, d_next, bt);
-          } else {
-            const size_t smem = sizeof(float) * ((size_t)(MB_TH + 2 * c) * (MB_TW + 2 * c) + (size_t)MB_TH * (MB_TW + 2 * c));
-            if (smem > 200 * 1024) { rc = ctx_fail(ctx, PANO_ERR_INVALID, "blend: gaussian window %d too wide", 2 * c + 1); goto done; }
-            e = cudaFuncSetAttribute(k_mb_blur_generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e == cudaSuccess) {
-              k_mb_blur_generic<<<n_tiles, 256, smem, ctx->stream>>>(d_planes, d_span, n_planes, d_cur, d_next, bt);
-              e = cudaGetLastError();
-            }
-          }
-          if (ctx->profiling) ctx_prof_end(ctx);
-          if (e != cudaSuccess) { rc = ctx_cuda(ctx, e, "k_mb_blur"); goto done; }
-        }
-        BL_LAUNCH(ctx, "k_mb_accumulate", k_mb_accumulate, gs, b, 0, d_imgs, n, d_cur, d_next, d_mask, level == 0 ? 1 : 0, is_last,
-                  d_out, d_tmask, tw, row0, row1);
-        if (!is_last) { std::swap(d_cur, d_next); buf ^= 1; }
-      }
-    }
-  }
-done:
-  ctx_free(ctx, d_imgs); ctx_free(ctx, d_tab); ctx_free(ctx, d_cur); ctx_free(ctx, d_next);
-  ctx_free(ctx, d_mask); ctx_free(ctx, d_tmask); ctx_free(ctx, d_planes); ctx_free(ctx, d_span); ctx_free(ctx, d_maps);
+  BlendDev dev;
+  rc = blend_dev_setup(ctx, &job, bands, row0, row1, &dev);
+  if (!rc) rc = blend_run(ctx, job, &dev, bands, p, d_out, row0, row1);
+  blend_dev_free(ctx, &dev);
   return rc;
+}
+
+// ------------------------------------------------------------------ blend stream
+// LAZY_READ's memory contract (blender.cc:38-64, multiband.cc:27,49): sources arrive window by
+// window and are dropped after their window.  State: the canvas (linear: sums + weight plane;
+// multiband: BlendDev's level buffers and masks) plus at most two windows of host sources in a
+// two-slot device ring.  Window k's upload runs on the stream's copy stream into slot k & 1 while
+// window k-1's kernels run on the context's stream; events order the slot's reuse.
+struct pano_blend_stream {
+  pano_ctx* ctx = nullptr;
+  int n = 0, bands = 0, lazy = 0, ordered = 0;
+  BlendJob job;
+  BlendDev dev;
+  float* d_sum = nullptr;      // linear: tw×th×3 Σ c·w
+  float* d_wsum = nullptr;     // linear: tw×th Σ w
+  int added = 0, windows = 0, err = 0;
+  bool finished = false;
+  cudaStream_t copy = nullptr;
+  cudaEvent_t ev_copied[2] = {nullptr, nullptr};   // slot's upload done (copy stream)
+  cudaEvent_t ev_done[2] = {nullptr, nullptr};     // slot's last reader done (context stream)
+  unsigned char* slot[2] = {nullptr, nullptr};
+  size_t slot_cap[2] = {0, 0};
+  unsigned char* stage[2] = {nullptr, nullptr};    // pinned staging of pageable sources
+  size_t stage_cap[2] = {0, 0};
+};
+
+static void blend_stream_release(pano_blend_stream* s) {
+  pano_ctx* ctx = s->ctx;
+  if (s->copy) cudaStreamSynchronize(s->copy);
+  for (int b = 0; b < 2; ++b) {
+    ctx_free(ctx, s->slot[b]);
+    if (s->stage[b]) cudaFreeHost(s->stage[b]);
+    if (s->ev_copied[b]) cudaEventDestroy(s->ev_copied[b]);
+    if (s->ev_done[b]) cudaEventDestroy(s->ev_done[b]);
+  }
+  if (s->copy) cudaStreamDestroy(s->copy);
+  ctx_free(ctx, s->d_sum); ctx_free(ctx, s->d_wsum);
+  blend_dev_free(ctx, &s->dev);
+  delete s;
+}
+
+// every failure is sticky: the canvas state is undefined after it
+static int stream_fail(pano_blend_stream* s, int rc) { s->err = rc; return rc; }
+#define STREAM_MISUSE(s, ...) stream_fail((s), ctx_fail((s)->ctx, PANO_ERR_INVALID, __VA_ARGS__))
+#define STREAM_CUDA(s, call)                                               \
+  do {                                                                     \
+    cudaError_t _e = (call);                                               \
+    if (_e != cudaSuccess) return stream_fail((s), ctx_cuda((s)->ctx, _e, #call)); \
+  } while (0)
+
+// Uploads host window `win` (count images from srcs) into ring slot windows & 1; points win[] at it.
+static int stream_upload(pano_blend_stream* s, int first, int count, const void* const* srcs, bool u8, int channels,
+                         BlendImg* win, int* slot_out) {
+  pano_ctx* ctx = s->ctx;
+  const int b = s->windows & 1;
+  std::vector<size_t> bytes(count), off(count);
+  size_t total = 0;
+  bool all_pinned = true;
+  for (int k = 0; k < count; ++k) {
+    const BlendImg& im = s->job.imgs[first + k];
+    bytes[k] = (size_t)im.w * im.h * (u8 ? channels : 3 * sizeof(float));
+    off[k] = total;
+    total += align_up(bytes[k], 256);
+    all_pinned = all_pinned && host_is_pinned(srcs[k]);
+  }
+  // slot b and its staging were last used by window - 2: its upload must be over before the host
+  // refills the staging buffer (an event never recorded counts as complete)
+  STREAM_CUDA(s, cudaEventSynchronize(s->ev_copied[b]));
+  if (s->slot_cap[b] < total) {
+    ctx_free(ctx, s->slot[b]);
+    s->slot[b] = nullptr; s->slot_cap[b] = 0;
+    int rc = ctx_alloc(ctx, (void**)&s->slot[b], total);
+    if (rc) return stream_fail(s, rc);
+    s->slot_cap[b] = total;
+    STREAM_CUDA(s, cudaEventRecord(s->ev_done[b], ctx->stream));   // the block is ours from here on the context stream
+  }
+  if (!all_pinned && s->stage_cap[b] < total) {
+    if (s->stage[b]) cudaFreeHost(s->stage[b]);
+    s->stage[b] = nullptr; s->stage_cap[b] = 0;
+    STREAM_CUDA(s, cudaMallocHost((void**)&s->stage[b], total));
+    s->stage_cap[b] = total;
+  }
+  // the copy must not overwrite the slot before window - 2's kernels have read it
+  STREAM_CUDA(s, cudaStreamWaitEvent(s->copy, s->ev_done[b], 0));
+  for (int k = 0; k < count; ++k) {
+    const void* src = srcs[k];
+    if (!host_is_pinned(src)) {               // pageable: staged, the caller may reuse it on return
+      memcpy(s->stage[b] + off[k], src, bytes[k]);
+      src = s->stage[b] + off[k];
+    }
+    STREAM_CUDA(s, cudaMemcpyAsync(s->slot[b] + off[k], src, bytes[k], cudaMemcpyHostToDevice, s->copy));
+    win[k].pix = s->slot[b] + off[k];
+  }
+  STREAM_CUDA(s, cudaEventRecord(s->ev_copied[b], s->copy));
+  STREAM_CUDA(s, cudaStreamWaitEvent(ctx->stream, s->ev_copied[b], 0));
+  *slot_out = b;
+  return PANO_OK;
+}
+
+template <class Src>
+static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const BlendImg* win, int count) {
+  pano_ctx* ctx = s->ctx;
+  const BlendJob& job = s->job;
+  const dim3 b(32, 8);
+  if (s->bands == 0) {
+    // bounding rectangle of the window on the canvas (inclusive ranges: a superset of both range rules)
+    int x0 = INT_MAX, y0 = INT_MAX, x1 = 0, y1 = 0;
+    for (int k = 0; k < count; ++k) {
+      x0 = std::min(x0, win[k].x0); y0 = std::min(y0, win[k].y0);
+      x1 = std::max(x1, win[k].x1 + 1); y1 = std::max(y1, win[k].y1 + 1);
+    }
+    x1 = std::min(x1, job.tw); y1 = std::min(y1, job.th);
+    if (x0 >= x1 || y0 >= y1) return PANO_OK;
+    dim3 g(ceil_div(x1 - x0, 32), ceil_div(y1 - y0, 8));
+    BL_LAUNCH(ctx, "k_linear_accumulate", k_linear_accumulate<Src>, g, b, 0, d_win, count, job.g, s->lazy, s->ordered,
+              s->d_sum, s->d_wsum, job.tw, x0, y0, x1, y1);
+  } else {
+    int rw = 0, rh = 0;
+    for (int k = 0; k < count; ++k) { rw = std::max(rw, win[k].rw); rh = std::max(rh, win[k].rh); }
+    dim3 g(ceil_div(rw, 32), ceil_div(rh, 8), count);
+    BL_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<Src>, g, b, 0, d_win, job.g, s->dev.d_cur, s->dev.d_mask);
+  }
+  return PANO_OK;
+}
+
+static int stream_resolve(pano_blend_stream* s, float* d_out) {
+  pano_ctx* ctx = s->ctx;
+  if (s->bands > 0) return mb_levels(ctx, s->job, &s->dev, s->bands, d_out, 0, s->job.th);
+  const size_t npx = (size_t)s->job.tw * s->job.th;
+  PANO_LAUNCH(ctx, "k_linear_resolve", k_linear_resolve, (unsigned)((npx + 255) / 256), 256, 0, s->d_sum, s->d_wsum,
+              d_out, npx, s->lazy);
+  return PANO_OK;
+}
+
+static int stream_finish_check(pano_blend_stream* s, const void* out) {
+  if (s->err) return s->err;
+  if (!out) return STREAM_MISUSE(s, "blend stream: null output");
+  if (s->finished) return STREAM_MISUSE(s, "blend stream: already finished");
+  if (s->added != s->n) return STREAM_MISUSE(s, "blend stream: finish after %d of %d images", s->added, s->n);
+  s->finished = true;
+  return PANO_OK;
 }
 
 extern "C" {
@@ -611,6 +867,108 @@ int pano_blend_rows_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
                         const pano_params* p, float* d_out_rows, int ow, int oh, int row0, int row1) {
   ctx_enter(ctx);
   return blend_device(ctx, n, imgs, g, bands, p, d_out_rows, ow, oh, row0, row1);
+}
+
+int pano_blend_stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
+                             const pano_params* p, int ow, int oh, pano_blend_stream** out) {
+  ctx_enter(ctx);
+  if (!ctx || !out) return PANO_ERR_INVALID;
+  *out = nullptr;
+  if (n <= 0 || !imgs || !g || !p || bands < 0) return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: bad argument");
+  pano_blend_stream* s = new pano_blend_stream;
+  s->ctx = ctx; s->n = n; s->bands = bands; s->lazy = p->lazy_read; s->ordered = p->ordered_input;
+  int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, 0, oh, false, &s->job);
+  if (!rc) rc = blend_dev_setup(ctx, &s->job, bands, 0, oh, &s->dev);
+  const size_t npx = (size_t)ow * oh;
+  if (!rc && bands == 0) {
+    rc = ctx_alloc(ctx, (void**)&s->d_sum, npx * 3 * sizeof(float));
+    if (!rc) rc = ctx_alloc(ctx, (void**)&s->d_wsum, npx * sizeof(float));
+    if (!rc) {
+      k_fill<<<(unsigned)((npx * 3 + 255) / 256), 256, 0, ctx->stream>>>(s->d_sum, npx * 3, 0.f);
+      k_fill<<<(unsigned)((npx + 255) / 256), 256, 0, ctx->stream>>>(s->d_wsum, npx, 0.f);
+      ctx->launches += 2;
+      cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) rc = ctx_cuda(ctx, e, "k_fill");
+    }
+  }
+  cudaError_t e = cudaSuccess;
+  if (!rc) e = cudaStreamCreateWithFlags(&s->copy, cudaStreamNonBlocking);
+  for (int b = 0; b < 2 && !rc && e == cudaSuccess; ++b) {
+    e = cudaEventCreateWithFlags(&s->ev_copied[b], cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_done[b], cudaEventDisableTiming);
+  }
+  if (!rc && e != cudaSuccess) rc = ctx_cuda(ctx, e, "blend stream: copy stream / events");
+  if (rc) { blend_stream_release(s); return rc; }
+  *out = s;
+  return PANO_OK;
+}
+
+int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void* const* srcs, int kind, int channels) {
+  if (!s) return PANO_ERR_INVALID;
+  pano_ctx* ctx = s->ctx;
+  ctx_enter(ctx);
+  if (s->err) return s->err;
+  if (s->finished) return STREAM_MISUSE(s, "blend stream: add after finish");
+  if (first != s->added || count <= 0 || count > s->n - first)
+    return STREAM_MISUSE(s, "blend stream: images [%d, %d) added, %d of %d so far", first, first + count, s->added, s->n);
+  if (!srcs) return STREAM_MISUSE(s, "blend stream: null source list");
+  for (int k = 0; k < count; ++k)
+    if (!srcs[k]) return STREAM_MISUSE(s, "blend stream: image %d has no source", first + k);
+  const bool u8 = kind == PANO_SRC_RGB8_DEV || kind == PANO_SRC_RGB8_HOST;
+  const bool host = kind == PANO_SRC_F32_HOST || kind == PANO_SRC_RGB8_HOST;
+  if (!u8 && kind != PANO_SRC_F32_DEV && kind != PANO_SRC_F32_HOST) return STREAM_MISUSE(s, "blend stream: unknown source kind %d", kind);
+  if (u8 ? (channels != 1 && channels != 3) : channels != 3)
+    return STREAM_MISUSE(s, "blend stream: %d channels for source kind %d", channels, kind);
+  std::vector<BlendImg> win(s->job.imgs.begin() + first, s->job.imgs.begin() + first + count);
+  for (int k = 0; k < count; ++k) {
+    win[k].pix = (const unsigned char*)srcs[k];
+    win[k].channels = u8 ? channels : 3;
+  }
+  int slot = -1, rc = 0;
+  if (host && (rc = stream_upload(s, first, count, srcs, u8, channels, win.data(), &slot))) return rc;
+  BlendImg* d_win = s->dev.d_imgs + first;
+  if ((rc = ctx_put(ctx, d_win, win.data(), count * sizeof(BlendImg)))) return stream_fail(s, rc);
+  rc = u8 ? stream_launch<SrcRgb8>(s, d_win, win.data(), count) : stream_launch<SrcF32>(s, d_win, win.data(), count);
+  if (rc) return stream_fail(s, rc);
+  if (slot >= 0) {
+    STREAM_CUDA(s, cudaEventRecord(s->ev_done[slot], ctx->stream));
+    ++s->windows;
+  }
+  s->added += count;
+  return PANO_OK;
+}
+
+int pano_blend_stream_finish_dev(pano_blend_stream* s, float* d_out) {
+  if (!s) return PANO_ERR_INVALID;
+  ctx_enter(s->ctx);
+  int rc = stream_finish_check(s, d_out);
+  if (!rc) rc = stream_resolve(s, d_out);
+  return rc ? stream_fail(s, rc) : PANO_OK;
+}
+
+int pano_blend_stream_finish(pano_blend_stream* s, float* out) {
+  if (!s) return PANO_ERR_INVALID;
+  pano_ctx* ctx = s->ctx;
+  ctx_enter(ctx);
+  int rc = stream_finish_check(s, out);
+  if (rc) return stream_fail(s, rc);
+  const size_t ob = (size_t)s->job.tw * s->job.th * 3 * sizeof(float);
+  float* d_out = s->d_sum;     // linear: resolved in place
+  if (s->bands > 0) rc = ctx_alloc(ctx, (void**)&d_out, ob);
+  if (!rc) rc = stream_resolve(s, d_out);
+  if (!rc) {
+    cudaError_t e = cudaMemcpyAsync(out, d_out, ob, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) rc = ctx_cuda(ctx, e, "blend stream download");
+  }
+  if (s->bands > 0) ctx_free(ctx, d_out);
+  return rc ? stream_fail(s, rc) : PANO_OK;
+}
+
+void pano_blend_stream_free(pano_blend_stream* s) {
+  if (!s) return;
+  ctx_enter(s->ctx);
+  blend_stream_release(s);
 }
 
 int pano_blend(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,

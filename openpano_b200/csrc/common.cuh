@@ -94,6 +94,7 @@ void ctx_cache_release(pano_ctx* ctx, size_t keep_bytes);
 void ctx_free(pano_ctx* ctx, void* p);
 void* ctx_pinned(pano_ctx* ctx, size_t bytes);   // staging buffer A (inputs)
 void* ctx_pinned2(pano_ctx* ctx, size_t bytes);  // staging buffer B (results)
+extern "C" bool host_is_pinned(const void* p);   // page-locked (cudaHostAlloc / pano_host_alloc) host memory
 // Small host<->device moves that stay OFF the copy engines: a big image upload or
 // mosaic download queued on another stream of the same device would otherwise
 // delay every tiny metadata copy queued behind it on the same engine, and with it
@@ -304,22 +305,63 @@ __device__ __forceinline__ void mag_ort_at(const float* __restrict__ img, int w,
   *ort = (float)((double)fast_atan(dy, dx) + PANO_PI);
 }
 
+// Sources of the interpolate_rgb gather.  Each fetches the two horizontally adjacent pixels
+// (fr, fc), (fr, fc + 1) and the two below them as 12 floats: q[0..5] row fr, q[6..11] row fr + 1.
+// A Mat32f, h×w×3 f32 (Color::NO = negative samples):
+struct SrcF32 {
+  const float* img;
+  static constexpr bool kMayBeNo = true, kLut = false;
+  __device__ __forceinline__ void fetch(int w, int fr, int fc, float* q) const {
+    const float* p00 = img + ((size_t)fr * w + fc) * 3;
+    const float* p10 = p00 + (size_t)w * 3;
+    // all twelve samples first (the four positions are in range), tests afterwards: the
+    // loads overlap instead of each Color::NO test waiting on its own load
+#pragma unroll
+    for (int k = 0; k < 6; ++k) { q[k] = __ldg(p00 + k); q[6 + k] = __ldg(p10 + k); }
+  }
+};
+// 8-bit pixels as read_img converts them (lib/imgio.cc:75-88, k_rgb8_to_f32): channels == 3 ->
+// lut[v] = (float)((double)v / 255.0), a 256-entry table in shared memory (build_rgb8_lut);
+// channels == 1 -> the grey value replicated to r, g, b WITHOUT the division.  The taps are the
+// f32 values read_img would have stored, bit for bit, and never Color::NO.
+struct SrcRgb8 {
+  const unsigned char* pix;
+  const float* lut;
+  int channels;
+  static constexpr bool kMayBeNo = false, kLut = true;
+  __device__ __forceinline__ void fetch(int w, int fr, int fc, float* q) const {
+    if (channels == 1) {
+      const unsigned char* p00 = pix + (size_t)fr * w + fc;
+      const float a = (float)__ldg(p00), b = (float)__ldg(p00 + 1);
+      const float c = (float)__ldg(p00 + w), d = (float)__ldg(p00 + w + 1);
+      q[0] = q[1] = q[2] = a; q[3] = q[4] = q[5] = b;
+      q[6] = q[7] = q[8] = c; q[9] = q[10] = q[11] = d;
+    } else {
+      const unsigned char* p00 = pix + ((size_t)fr * w + fc) * 3;
+      const unsigned char* p10 = p00 + (size_t)w * 3;
+#pragma unroll
+      for (int k = 0; k < 6; ++k) { q[k] = lut[__ldg(p00 + k)]; q[6 + k] = lut[__ldg(p10 + k)]; }
+    }
+  }
+};
+// every thread of a block of at least 256 writes one entry; the caller synchronises
+__device__ __forceinline__ void build_rgb8_lut(float* lut, int tid) {
+  if (tid < 256) lut[tid] = (float)((double)tid / 255.0);
+}
+
 // lib/imgproc.cc:135-156 interpolate; returns false for Color::NO
-__device__ __forceinline__ bool interpolate_rgb(const float* __restrict__ img, int w, int h, float r,
-                                                float c, float* o0, float* o1, float* o2) {
+template <class Src>
+__device__ __forceinline__ bool interpolate_rgb(const Src& src, int w, int h, float r, float c, float* o0, float* o1,
+                                                float* o2) {
   int fr = (int)floorf(r), fc = (int)floorf(c);
   if (fr < 0 || fc < 0 || fc + 1 >= w || fr + 1 >= h) return false;
   r -= (float)fr;
   c -= (float)fc;
-  const float* p00 = img + ((size_t)fr * w + fc) * 3;
-  const float* p10 = p00 + (size_t)w * 3;
-  // all twelve samples first (the four positions are in range), tests afterwards: the
-  // loads overlap instead of each Color::NO test waiting on its own load
-  const float q00 = __ldg(p00), q01 = __ldg(p00 + 1), q02 = __ldg(p00 + 2);
-  const float q03 = __ldg(p00 + 3), q04 = __ldg(p00 + 4), q05 = __ldg(p00 + 5);
-  const float q10 = __ldg(p10), q11 = __ldg(p10 + 1), q12 = __ldg(p10 + 2);
-  const float q13 = __ldg(p10 + 3), q14 = __ldg(p10 + 4), q15 = __ldg(p10 + 5);
-  if (q00 < 0 || q10 < 0 || q13 < 0 || q03 < 0) return false;
+  float q[12];
+  src.fetch(w, fr, fc, q);
+  const float q00 = q[0], q01 = q[1], q02 = q[2], q03 = q[3], q04 = q[4], q05 = q[5];
+  const float q10 = q[6], q11 = q[7], q12 = q[8], q13 = q[9], q14 = q[10], q15 = q[11];
+  if (Src::kMayBeNo && (q00 < 0 || q10 < 0 || q13 < 0 || q03 < 0)) return false;
   float w00 = (1 - r) * (1 - c), w10 = r * (1 - c), w11 = r * c, w01 = (1 - r) * c;
   float a0 = 0.f + q00 * w00, a1 = 0.f + q01 * w00, a2 = 0.f + q02 * w00;
   a0 += q10 * w10; a1 += q11 * w10; a2 += q12 * w10;
@@ -327,6 +369,10 @@ __device__ __forceinline__ bool interpolate_rgb(const float* __restrict__ img, i
   a0 += q03 * w01; a1 += q04 * w01; a2 += q05 * w01;
   *o0 = a0; *o1 = a1; *o2 = a2;
   return true;
+}
+__device__ __forceinline__ bool interpolate_rgb(const float* __restrict__ img, int w, int h, float r, float c,
+                                                float* o0, float* o1, float* o2) {
+  return interpolate_rgb(SrcF32{img}, w, h, r, c, o0, o1, o2);
 }
 
 #endif  // __CUDACC__

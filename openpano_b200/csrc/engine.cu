@@ -491,6 +491,19 @@ int pano_trim(pano_ctx* ctx) {
   return PANO_OK;
 }
 
+int pano_mem_high_water(pano_ctx* ctx, size_t* bytes, int reset) {
+  if (!ctx || !bytes) return PANO_ERR_INVALID;
+  ctx_enter(ctx);
+  unsigned long long v = 0;   // cuuint64_t
+  PANO_CUDA(ctx, cudaMemPoolGetAttribute(ctx->pool, cudaMemPoolAttrUsedMemHigh, &v));
+  *bytes = (size_t)v;
+  if (reset) {
+    unsigned long long zero = 0;   // the mark restarts at what is in use now
+    PANO_CUDA(ctx, cudaMemPoolSetAttribute(ctx->pool, cudaMemPoolAttrUsedMemHigh, &zero));
+  }
+  return PANO_OK;
+}
+
 void pano_destroy(pano_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
@@ -665,7 +678,7 @@ int pano_sift_detect_batch_dev(pano_ctx* ctx, int n, const float* const* d_rgb, 
   return PANO_OK;
 }
 
-static bool host_is_pinned(const void* p) {
+bool host_is_pinned(const void* p) {
   cudaPointerAttributes a;
   if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
   return a.type == cudaMemoryTypeHost;

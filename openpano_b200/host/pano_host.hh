@@ -12,6 +12,7 @@
 // tests/adaptor/adaptor_test.cc builds these against the reference tree and checks them
 // against the reference classes they replace, bit for bit.
 #pragma once
+#include <algorithm>
 #include <cstring>
 #include <functional>
 #include <memory>
@@ -198,6 +199,60 @@ class B200Blender : public pano::BlenderBase {
   int bands_;
   pano_blend_geom g_;
   std::vector<pano_blend_image> imgs_;
+};
+
+// ---- blend with LAZY_READ's memory contract (blender.cc:38-64, multiband.cc:27,49): run() loads the images
+// `window` at a time, hands them to a pano_blend_stream and releases them before the next window, so at most one
+// window of Mat32f is resident on the host and two on the device.  The output is B200Blender's, bit for bit.
+// The stream needs every image's shape up front: each ImageRef must have been loaded once before run() (as
+// calc_feature() does; ImageRef::release keeps the shape).
+class B200LazyBlender : public pano::BlenderBase {
+ public:
+  B200LazyBlender(const Context& c, int bands, int projection, Vec2D resolution, Vec2D proj_min, int window = 1)
+      : c_(c), bands_(bands), window_(window < 1 ? 1 : window) {
+    g_.projection = projection; g_.res_x = resolution.x; g_.res_y = resolution.y;
+    g_.proj_min_x = proj_min.x; g_.proj_min_y = proj_min.y;
+  }
+  void add_image(const Coor& upper_left, const Coor& bottom_right, pano::ImageRef& img, const pano::Homography& homo_inv) {
+    pano_blend_image b;
+    b.rgb_hwc = nullptr; b.w = img.width(); b.h = img.height();
+    b.x0 = upper_left.x; b.y0 = upper_left.y; b.x1 = bottom_right.x; b.y1 = bottom_right.y;
+    memcpy(b.homo_inv, homo_inv.data, sizeof(double) * 9);
+    imgs_.push_back(b);
+    refs_.push_back(&img);
+  }
+  void add_image(const Coor&, const Coor&, pano::ImageRef&, std::function<Vec2D(Coor)>) override {
+    error_exit("B200LazyBlender: pass the homography (add_image(ul, br, img, homo_inv)), a closure cannot cross the C ABI");
+  }
+  Mat32f run() override {
+    const int n = (int)imgs_.size();
+    int ow = 0, oh = 0;
+    c_.check(pano_blend_target_size(n, imgs_.data(), &ow, &oh));
+    pano_params p = snapshot_params();
+    pano_blend_stream* s = nullptr;
+    c_.check(pano_blend_stream_create(c_.get(), n, imgs_.data(), &g_, bands_, &p, ow, oh, &s));
+    for (int k0 = 0; k0 < n; k0 += window_) {
+      const int k1 = std::min(n, k0 + window_);
+      std::vector<const void*> src;
+      for (int k = k0; k < k1; ++k) {
+        refs_[k]->load();
+        src.push_back(refs_[k]->img->ptr());
+      }
+      // Mat32f storage is pageable: the stream stages it before returning
+      c_.check(pano_blend_stream_add(s, k0, k1 - k0, src.data(), PANO_SRC_F32_HOST, 3));
+      for (int k = k0; k < k1; ++k) refs_[k]->release();
+    }
+    Mat32f out(oh, ow, 3);
+    c_.check(pano_blend_stream_finish(s, out.ptr()));
+    pano_blend_stream_free(s);
+    return out;
+  }
+ private:
+  const Context& c_;
+  int bands_, window_;
+  pano_blend_geom g_;
+  std::vector<pano_blend_image> imgs_;
+  std::vector<pano::ImageRef*> refs_;
 };
 
 // ---- cylinder warp: CylinderWarper(h_factor).warp(mat, kpts) (warp.hh:41-66)
