@@ -164,6 +164,20 @@ int pano_sift_detect_batch_dev(pano_ctx* ctx, int n, const float* const* d_rgb_h
 /* Single-image convenience = detect_feature(const Mat32f&). */
 int pano_sift_detect(pano_ctx* ctx, const float* rgb_hwc, int w, int h,
                      const pano_params* p, pano_featureset** out);
+/* SIFT straight from decoded 8-bit pixels, read_img's input (lib/imgio.cc:72-88): n pointers to
+ * h×w×channels[i] interleaved u8, channels 1 or 3 per image.  The featureset equals
+ * pano_sift_detect_batch's on read_img's f32 images of the same pixels (channels == 3:
+ * (float)((double)v / 255.0); channels == 1: the grey value replicated, not divided), and no f32
+ * copy of an image is made: the working-size resize reads the 8-bit taps.
+ * _rgb8: host memory, pageable or pinned, with pano_sift_detect_batch's rules (3 B/px cross PCIe).
+ * _rgb8_dev: device memory, valid until the first count query / download / match on the featureset.
+ * Null pointers, n <= 0, channels other than 1 or 3 or an image under 2×2 return PANO_ERR_INVALID. */
+int pano_sift_detect_batch_rgb8(pano_ctx* ctx, int n, const unsigned char* const* pix, const int* w,
+                                const int* h, const int* channels, const pano_params* p,
+                                pano_featureset** out);
+int pano_sift_detect_batch_rgb8_dev(pano_ctx* ctx, int n, const unsigned char* const* d_pix, const int* w,
+                                    const int* h, const int* channels, const pano_params* p,
+                                    pano_featureset** out);
 
 /* Builds a featureset from host descriptors = PairWiseMatcher ctor
  * (feature/matcher.hh:40-46; matcher.cc:73-88 without the kd-forest).
@@ -371,6 +385,14 @@ int pano_blend(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_bl
 /* Device-resident variant: imgs[k].rgb_hwc and d_out_hwc are device pointers. */
 int pano_blend_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g,
                    int bands, const pano_params* p, float* d_out_hwc, int out_w, int out_h);
+/* pano_blend_dev from device 8-bit sources: d_pix[k] is h×w×channels[k] interleaved u8 (channels 1 or
+ * 3), imgs[k].rgb_hwc is ignored and may be NULL.  The mosaic is pano_blend_dev's on read_img's f32
+ * images of the same pixels, bit for bit: every tap is converted as pano_rgb8_to_mat32f_dev converts
+ * it, and no f32 copy of a source is made.  Null pointers, n <= 0, other channel counts or an image
+ * under 2×2 return PANO_ERR_INVALID. */
+int pano_blend_rgb8_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const unsigned char* const* d_pix,
+                        const int* channels, const pano_blend_geom* g, int bands, const pano_params* p,
+                        float* d_out_hwc, int out_w, int out_h);
 
 /* Rows [row0, row1) of the same mosaic into d_out_rows ((row1-row0)×out_w×3 f32): the
  * strip partition of the canvas across GPUs (every output pixel of

@@ -57,6 +57,8 @@ def _load():
         "pano_sift_detect_batch": (C.c_int, [C.c_void_p, C.c_int, _vpp, _ip, _ip, P, _vpp]),
         "pano_sift_detect_batch_dev": (C.c_int, [C.c_void_p, C.c_int, _vpp, _ip, _ip, P, _vpp]),
         "pano_sift_detect": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, P, _vpp]),
+        "pano_sift_detect_batch_rgb8": (C.c_int, [C.c_void_p, C.c_int, _vpp, _ip, _ip, _ip, P, _vpp]),
+        "pano_sift_detect_batch_rgb8_dev": (C.c_int, [C.c_void_p, C.c_int, _vpp, _ip, _ip, _ip, P, _vpp]),
         "pano_featureset_upload": (C.c_int, [C.c_void_p, C.c_int, _ip, _vpp, _vpp, _vpp]),
         "pano_featureset_num_images": (C.c_int, [C.c_void_p]),
         "pano_featureset_count": (C.c_int, [C.c_void_p, C.c_int]),
@@ -92,6 +94,8 @@ def _load():
                                  C.c_int, P, _fp, C.c_int, C.c_int]),
         "pano_blend_dev": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage),
                                      C.POINTER(PanoBlendGeom), C.c_int, P, C.c_void_p, C.c_int, C.c_int]),
+        "pano_blend_rgb8_dev": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), _vpp, _ip,
+                                          C.POINTER(PanoBlendGeom), C.c_int, P, C.c_void_p, C.c_int, C.c_int]),
         "pano_blend_rows_dev": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom),
                                           C.c_int, P, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
         "pano_blend_stream_create": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom),
@@ -528,6 +532,31 @@ class Engine:
         self._check(fn(self._h, n, cp, cw, ch, C.byref(params), C.byref(out)))
         return FeatureSet(self, out)
 
+    def sift_detect_batch_rgb8(self, pix, params=None) -> FeatureSet:
+        """SIFT straight from decoded 8-bit pixels (numpy uint8 H×W, H×W×1 or H×W×3, read_img's input):
+        the features of sift_detect_batch on read_img's f32 images, without those images."""
+        pix = [np.ascontiguousarray(x, np.uint8) for x in pix]
+        for x in pix:
+            if not (x.ndim == 2 or (x.ndim == 3 and x.shape[2] in (1, 3))):
+                raise PanoError(-2, f"sift rgb8: expected H×W or H×W×{{1,3}} uint8, got shape {x.shape}")
+        return self.sift_detect_batch_rgb8_ptr([x.ctypes.data for x in pix], [x.shape[1] for x in pix],
+                                               [x.shape[0] for x in pix], [1 if x.ndim == 2 else x.shape[2] for x in pix],
+                                               params)
+
+    def sift_detect_batch_rgb8_ptr(self, ptrs, ws, hs, channels, params=None, device=False) -> FeatureSet:
+        """Raw-pointer variant: h×w×channels u8 images in host memory (pageable or pinned) or, with device=True,
+        in device memory (valid until the first count query / download / match of the featureset)."""
+        params = params or default_params()
+        n = len(ptrs)
+        cp = (C.c_void_p * max(n, 1))(*ptrs)
+        cw = (C.c_int * max(n, 1))(*ws)
+        chh = (C.c_int * max(n, 1))(*hs)
+        cc = (C.c_int * max(n, 1))(*channels)
+        out = C.c_void_p()
+        fn = LIB.pano_sift_detect_batch_rgb8_dev if device else LIB.pano_sift_detect_batch_rgb8
+        self._check(fn(self._h, n, cp, cw, chh, cc, C.byref(params), C.byref(out)))
+        return FeatureSet(self, out)
+
     def sift_detect(self, img, params=None):
         fs = self.sift_detect_batch([img], params)
         try:
@@ -733,6 +762,17 @@ class Engine:
         arr, g = self._blend_args(ptrs, shapes, items, geom)
         self._check(LIB.pano_blend_dev(self._h, len(ptrs), arr, C.byref(g), bands, C.byref(params),
                                        C.c_void_p(d_out), out_w, out_h))
+
+    def blend_rgb8_dev(self, d_pix, channels, shapes, items, geom, d_out, out_w, out_h, bands=0, params=None):
+        """blend_dev from device h×w×channels u8 sources (channels 1 or 3 per image): the mosaic of blend_dev on
+        read_img's f32 images of the same pixels."""
+        params = params or default_params()
+        n = len(d_pix)
+        arr, g = self._blend_args([None] * n, shapes, items, geom)
+        src = (C.c_void_p * max(n, 1))(*d_pix)
+        ch = (C.c_int * max(n, 1))(*channels)
+        self._check(LIB.pano_blend_rgb8_dev(self._h, n, arr, src, ch, C.byref(g), bands, C.byref(params),
+                                            C.c_void_p(d_out), out_w, out_h))
 
     def blend_stream(self, shapes, items, geom, bands=0, params=None) -> BlendStream:
         """shapes: (h, w) per image; items / geom as for blend().  Allocates the canvas state."""

@@ -141,10 +141,13 @@ __device__ __forceinline__ void linear_resolve_px(int lazy, float s0, float s1, 
   }
 }
 
+template <class Src>
 __global__ void k_linear_blend(const BlendImg* __restrict__ imgs, int n, BlendGeom g, int lazy, int ordered,
                                float* __restrict__ out, int tw, int row0, int row1) {
   // rows [row0, row1) of the canvas; `out` starts at row0 (a strip of a row-sharded mosaic, or the whole)
   __shared__ TileList tl;
+  __shared__ float lut[Src::kLut ? 256 : 1];
+  if constexpr (Src::kLut) build_rgb8_lut(lut, threadIdx.y * blockDim.x + threadIdx.x);   // ordered by the list's barrier
   {
     const int tj0 = blockIdx.x * blockDim.x, ti0 = row0 + blockIdx.y * blockDim.y;
     build_tile_list(imgs, n, tj0, ti0, tj0 + blockDim.x - 1, ti0 + blockDim.y - 1, &tl);
@@ -153,7 +156,7 @@ __global__ void k_linear_blend(const BlendImg* __restrict__ imgs, int n, BlendGe
   int i = row0 + blockIdx.y * blockDim.y + threadIdx.y;
   if (j >= tw || i >= row1) return;
   float s0 = 0.f, s1 = 0.f, s2 = 0.f, wsum = 0.f;
-  linear_add_px<SrcF32>(imgs, n, tl, g, lazy, ordered, nullptr, i, j, s0, s1, s2, wsum);
+  linear_add_px<Src>(imgs, n, tl, g, lazy, ordered, lut, i, j, s0, s1, s2, wsum);
   linear_resolve_px(lazy, s0, s1, s2, wsum, out + ((size_t)(i - row0) * tw + j) * 3);
 }
 
@@ -489,8 +492,10 @@ static cudaError_t launch_mb_blur_tma(pano_ctx* ctx, int grid, const MbPlane* pl
 }
 
 // Validates the images (need_src: every rgb_hwc must be set) and builds the job of rows [row0, row1).
+// pix / channels (8-bit sources, else null): the images' pixels instead of rgb_hwc.
 static int blend_plan(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
-                      const pano_params* p, int ow, int oh, int row0, int row1, bool need_src, BlendJob* job) {
+                      const pano_params* p, int ow, int oh, int row0, int row1, bool need_src, BlendJob* job,
+                      const unsigned char* const* pix = nullptr, const int* channels = nullptr) {
   // Multiband on a row strip: a band at level l of pixel p depends on level 0 inside a
   // radius of the summed half-widths of the blurs up to l, so the strip is computed from
   // each image's ROI clipped to [row0 - H, row1 + H) with H = that sum over all blurred
@@ -514,10 +519,13 @@ static int blend_plan(pano_ctx* ctx, int n, const pano_blend_image* imgs, const 
     const pano_blend_image& s = imgs[k];
     if ((need_src && !s.rgb_hwc) || s.w < 2 || s.h < 2 || s.x1 < s.x0 || s.y1 < s.y0 || s.x0 < 0 || s.y0 < 0)
       return ctx_fail(ctx, PANO_ERR_INVALID, "blend: image %d has an invalid shape or range", k);
+    if (pix && (!pix[k] || (channels[k] != 1 && channels[k] != 3)))
+      return ctx_fail(ctx, PANO_ERR_INVALID, "blend: image %d has no pixels or %d channels (1 or 3)", k, channels[k]);
     job->tw = std::max(job->tw, s.x1); job->th = std::max(job->th, s.y1);
     BlendImg d;
     memset(&d, 0, sizeof(d));
     d.rgb = s.rgb_hwc; d.w = s.w; d.h = s.h;
+    if (pix) d.pix = pix[k];
     d.x0 = s.x0; d.x1 = s.x1;
     d.y0 = std::max(s.y0, job->clip0); d.y1 = std::min(s.y1, job->clip1);
     if (d.y0 > d.y1) continue;                         // no row of this image reaches the strip
@@ -527,7 +535,7 @@ static int blend_plan(pano_ctx* ctx, int n, const pano_blend_image* imgs, const 
     d.plane = (long long)d.pitch * d.rh;
     d.roi_off = job->roi_floats;
     d.mask_off = job->mask_bytes;
-    d.channels = 3;
+    d.channels = pix ? channels[k] : 3;
     job->roi_floats += 4 * d.plane;
     job->mask_bytes += d.plane;
     job->max_rw = std::max(job->max_rw, d.rw); job->max_rh = std::max(job->max_rh, d.rh);
@@ -670,29 +678,32 @@ static int mb_levels(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands,
   return PANO_OK;
 }
 
+template <class Src>
 static int blend_run(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands, const pano_params* p, float* d_out,
                      int row0, int row1) {
   const int n = (int)job.imgs.size(), tw = job.tw;
-  const dim3 b(32, 8);
+  const dim3 b(32, 8);   // 256 threads: the 8-bit kernels' conversion table
   if (bands == 0) {
     dim3 gs(ceil_div(tw, 32), ceil_div(row1 - row0, 8));
-    BL_LAUNCH(ctx, "k_linear_blend", k_linear_blend, gs, b, 0, d->d_imgs, n, job.g, p->lazy_read, p->ordered_input, d_out,
-              tw, row0, row1);
+    BL_LAUNCH(ctx, Src::kLut ? "k_linear_blend_rgb8" : "k_linear_blend", k_linear_blend<Src>, gs, b, 0, d->d_imgs, n,
+              job.g, p->lazy_read, p->ordered_input, d_out, tw, row0, row1);
     return PANO_OK;
   }
   dim3 gr(ceil_div(job.max_rw, 32), ceil_div(job.max_rh, 8), n);
-  BL_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<SrcF32>, gr, b, 0, d->d_imgs, job.g, d->d_cur, d->d_mask);
+  BL_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<Src>, gr, b, 0, d->d_imgs, job.g, d->d_cur, d->d_mask);
   return mb_levels(ctx, job, d, bands, d_out, row0, row1);
 }
 
+// pix / channels: 8-bit device sources (pano_blend_rgb8_dev), else null and imgs[k].rgb_hwc are the sources
 static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
-                        const pano_params* p, float* d_out, int ow, int oh, int row0, int row1) {
+                        const pano_params* p, float* d_out, int ow, int oh, int row0, int row1,
+                        const unsigned char* const* pix = nullptr, const int* channels = nullptr) {
   if (!ctx || n <= 0 || !imgs || !g || !p || !d_out || bands < 0) return PANO_ERR_INVALID;
   if (row0 < 0 || row1 > oh || row0 > row1)
     return ctx_fail(ctx, PANO_ERR_INVALID, "blend: rows [%d, %d) outside the %d-row canvas", row0, row1, oh);
   if (row0 == row1) return PANO_OK;
   BlendJob job;
-  int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, row0, row1, true, &job);
+  int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, row0, row1, !pix, &job, pix, channels);
   if (rc) return rc;
   if (job.imgs.empty()) {                              // no image reaches the strip
     size_t nfl = (size_t)job.tw * (row1 - row0) * 3;
@@ -701,7 +712,8 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
   }
   BlendDev dev;
   rc = blend_dev_setup(ctx, &job, bands, row0, row1, &dev);
-  if (!rc) rc = blend_run(ctx, job, &dev, bands, p, d_out, row0, row1);
+  if (!rc) rc = pix ? blend_run<SrcRgb8>(ctx, job, &dev, bands, p, d_out, row0, row1)
+                    : blend_run<SrcF32>(ctx, job, &dev, bands, p, d_out, row0, row1);
   blend_dev_free(ctx, &dev);
   return rc;
 }
@@ -861,6 +873,15 @@ int pano_blend_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pan
                    const pano_params* p, float* d_out, int ow, int oh) {
   ctx_enter(ctx);
   return blend_device(ctx, n, imgs, g, bands, p, d_out, ow, oh, 0, oh);
+}
+
+int pano_blend_rgb8_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const unsigned char* const* d_pix,
+                        const int* channels, const pano_blend_geom* g, int bands, const pano_params* p, float* d_out,
+                        int ow, int oh) {
+  ctx_enter(ctx);
+  if (!ctx) return PANO_ERR_INVALID;
+  if (!d_pix || !channels) return ctx_fail(ctx, PANO_ERR_INVALID, "blend rgb8: null source list");
+  return blend_device(ctx, n, imgs, g, bands, p, d_out, ow, oh, 0, oh, d_pix, channels);
 }
 
 int pano_blend_rows_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,

@@ -658,24 +658,31 @@ static void featureset_release(pano_featureset* fs) {
   delete fs;
 }
 
+// channels == nullptr: h×w×3 f32 device images; otherwise h×w×channels[i] u8 device images
+static int sift_detect_dev(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w,
+                           const int* h, const pano_params* p, pano_featureset** out) {
+  pano_featureset* fs = new pano_featureset;
+  fs->ctx = ctx;
+  // kept for the capacity retry of featureset_sync_counts
+  fs->src.assign(d_src, d_src + n); fs->src_w.assign(w, w + n); fs->src_h.assign(h, h + n); fs->src_params = *p;
+  if (channels) fs->src_channels.assign(channels, channels + n);
+  if (ctx->sift_cap <= 0) {
+    const char* e = getenv("PANO_SIFT_CAP");            // test hook: start small to exercise the growth path
+    ctx->sift_cap = e ? std::max(256, atoi(e)) : SIFT_CAP_DEFAULT;
+  }
+  int rc = sift_run_batch(ctx, n, d_src, channels, w, h, p, fs, nullptr, ctx->sift_cap);
+  if (rc != 0) { featureset_release(fs); return rc; }
+  *out = fs;
+  return PANO_OK;
+}
+
 int pano_sift_detect_batch_dev(pano_ctx* ctx, int n, const float* const* d_rgb, const int* w, const int* h,
                                const pano_params* p, pano_featureset** out) {
   ctx_enter(ctx);
   if (!ctx || !out) return PANO_ERR_INVALID;
   *out = nullptr;
   if (n <= 0 || !d_rgb || !w || !h || !p) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: bad argument");
-  pano_featureset* fs = new pano_featureset;
-  fs->ctx = ctx;
-  // kept for the capacity retry of featureset_sync_counts
-  fs->src.assign(d_rgb, d_rgb + n); fs->src_w.assign(w, w + n); fs->src_h.assign(h, h + n); fs->src_params = *p;
-  if (ctx->sift_cap <= 0) {
-    const char* e = getenv("PANO_SIFT_CAP");            // test hook: start small to exercise the growth path
-    ctx->sift_cap = e ? std::max(256, atoi(e)) : SIFT_CAP_DEFAULT;
-  }
-  int rc = sift_run_batch(ctx, n, d_rgb, w, h, p, fs, nullptr, ctx->sift_cap);
-  if (rc != 0) { featureset_release(fs); return rc; }
-  *out = fs;
-  return PANO_OK;
+  return sift_detect_dev(ctx, n, (const void* const*)d_rgb, nullptr, w, h, p, out);
 }
 
 bool host_is_pinned(const void* p) {
@@ -685,36 +692,50 @@ bool host_is_pinned(const void* p) {
 }
 
 // Uploads host images through one pinned staging buffer (async H2D on the ctx
-// stream), then runs the device path.
-static int upload_images(pano_ctx* ctx, int n, const float* const* rgb, const int* w, const int* h,
-                         std::vector<float*>& d_imgs, float** d_block) {
+// stream), then runs the device path.  channels == nullptr: h×w×3 f32 images; otherwise
+// h×w×channels[i] u8 images.  Every image starts on a 256-byte boundary of *d_block.
+static int upload_images(pano_ctx* ctx, int n, const void* const* src, const int* channels, const int* w, const int* h,
+                         std::vector<const void*>& d_imgs, unsigned char** d_block) {
   size_t total = 0;
-  std::vector<size_t> offs(n);
+  std::vector<size_t> offs(n), bytes(n);
   for (int i = 0; i < n; ++i) {
-    if (!rgb[i] || w[i] <= 0 || h[i] <= 0) return ctx_fail(ctx, PANO_ERR_INVALID, "image %d: null or empty", i);
+    if (!src[i] || w[i] <= 0 || h[i] <= 0) return ctx_fail(ctx, PANO_ERR_INVALID, "image %d: null or empty", i);
     offs[i] = total;
-    total += align_up((size_t)w[i] * h[i] * 3, 64);
+    bytes[i] = (size_t)w[i] * h[i] * (channels ? (size_t)channels[i] : 3 * sizeof(float));
+    total += align_up(bytes[i], 256);
   }
-  int rc = ctx_alloc(ctx, (void**)d_block, total * sizeof(float));
+  int rc = ctx_alloc(ctx, (void**)d_block, total);
   if (rc) return rc;
   // the staging buffer may still feed an earlier async copy
   PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   bool all_pinned = true;
-  for (int i = 0; i < n; ++i) all_pinned = all_pinned && host_is_pinned(rgb[i]);
-  float* st = all_pinned ? (float*)ctx_pinned(ctx, 64) : (float*)ctx_pinned(ctx, total * sizeof(float));
-  if (!st) return ctx_fail(ctx, PANO_ERR_CUDA, "pinned staging allocation of %zu bytes failed", total * sizeof(float));
+  for (int i = 0; i < n; ++i) all_pinned = all_pinned && host_is_pinned(src[i]);
+  unsigned char* st = all_pinned ? (unsigned char*)ctx_pinned(ctx, 64) : (unsigned char*)ctx_pinned(ctx, total);
+  if (!st) return ctx_fail(ctx, PANO_ERR_CUDA, "pinned staging allocation of %zu bytes failed", total);
   d_imgs.resize(n);
   for (int i = 0; i < n; ++i) {
-    size_t bytes = (size_t)w[i] * h[i] * 3 * sizeof(float);
-    const float* src = rgb[i];
-    if (!host_is_pinned(rgb[i])) {  // pageable caller memory: stage it
-      memcpy(st + offs[i], rgb[i], bytes);
-      src = st + offs[i];
+    const void* s = src[i];
+    if (!host_is_pinned(src[i])) {  // pageable caller memory: stage it
+      memcpy(st + offs[i], src[i], bytes[i]);
+      s = st + offs[i];
     }
-    PANO_CUDA(ctx, cudaMemcpyAsync(*d_block + offs[i], src, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    PANO_CUDA(ctx, cudaMemcpyAsync(*d_block + offs[i], s, bytes[i], cudaMemcpyHostToDevice, ctx->stream));
     d_imgs[i] = *d_block + offs[i];
   }
   return PANO_OK;
+}
+
+// The host entry points: upload, then the device path; the uploaded block lives until the counts are
+// known (a capacity retry reads it again).
+static int sift_detect_host(pano_ctx* ctx, int n, const void* const* src, const int* channels, const int* w,
+                            const int* h, const pano_params* p, pano_featureset** out) {
+  std::vector<const void*> d_imgs;
+  unsigned char* d_block = nullptr;
+  int rc = upload_images(ctx, n, src, channels, w, h, d_imgs, &d_block);
+  if (!rc) rc = sift_detect_dev(ctx, n, d_imgs.data(), channels, w, h, p, out);
+  if (rc) { ctx_free(ctx, d_block); return rc; }
+  (*out)->owned_block = d_block;
+  return rc;
 }
 
 int pano_sift_detect_batch(pano_ctx* ctx, int n, const float* const* rgb, const int* w, const int* h,
@@ -722,14 +743,40 @@ int pano_sift_detect_batch(pano_ctx* ctx, int n, const float* const* rgb, const 
   ctx_enter(ctx);
   if (!ctx || !out || n <= 0 || !rgb || !w || !h || !p) return PANO_ERR_INVALID;
   *out = nullptr;
-  std::vector<float*> d_imgs;
-  float* d_block = nullptr;
-  int rc = upload_images(ctx, n, rgb, w, h, d_imgs, &d_block);
-  if (rc) { ctx_free(ctx, d_block); return rc; }
-  rc = pano_sift_detect_batch_dev(ctx, n, d_imgs.data(), w, h, p, out);
-  if (rc) { ctx_free(ctx, d_block); return rc; }
-  (*out)->owned_block = d_block;       // released once the counts are known (a capacity retry reads it again)
-  return rc;
+  return sift_detect_host(ctx, n, (const void* const*)rgb, nullptr, w, h, p, out);
+}
+
+// Checks of the 8-bit entry points: the f32 ones take any pointer, these reject what they cannot read.
+static int rgb8_args_ok(pano_ctx* ctx, int n, const unsigned char* const* pix, const int* w, const int* h,
+                        const int* channels, const pano_params* p) {
+  if (n <= 0 || !pix || !w || !h || !channels || !p) return ctx_fail(ctx, PANO_ERR_INVALID, "sift rgb8: bad argument");
+  for (int i = 0; i < n; ++i) {
+    if (!pix[i]) return ctx_fail(ctx, PANO_ERR_INVALID, "sift rgb8: image %d is null", i);
+    if (channels[i] != 1 && channels[i] != 3)
+      return ctx_fail(ctx, PANO_ERR_INVALID, "sift rgb8: image %d has %d channels (1 or 3)", i, channels[i]);
+    if (w[i] < 2 || h[i] < 2) return ctx_fail(ctx, PANO_ERR_INVALID, "sift rgb8: image %d is %dx%d (at least 2x2)", i, w[i], h[i]);
+  }
+  return PANO_OK;
+}
+
+int pano_sift_detect_batch_rgb8_dev(pano_ctx* ctx, int n, const unsigned char* const* d_pix, const int* w, const int* h,
+                                    const int* channels, const pano_params* p, pano_featureset** out) {
+  ctx_enter(ctx);
+  if (!ctx || !out) return PANO_ERR_INVALID;
+  *out = nullptr;
+  int rc = rgb8_args_ok(ctx, n, d_pix, w, h, channels, p);
+  if (rc) return rc;
+  return sift_detect_dev(ctx, n, (const void* const*)d_pix, channels, w, h, p, out);
+}
+
+int pano_sift_detect_batch_rgb8(pano_ctx* ctx, int n, const unsigned char* const* pix, const int* w, const int* h,
+                                const int* channels, const pano_params* p, pano_featureset** out) {
+  ctx_enter(ctx);
+  if (!ctx || !out) return PANO_ERR_INVALID;
+  *out = nullptr;
+  int rc = rgb8_args_ok(ctx, n, pix, w, h, channels, p);
+  if (rc) return rc;
+  return sift_detect_host(ctx, n, (const void* const*)pix, channels, w, h, p, out);
 }
 
 int pano_sift_detect(pano_ctx* ctx, const float* rgb, int w, int h, const pano_params* p, pano_featureset** out) {
@@ -896,23 +943,24 @@ struct pano_sift_trace {
   pano_ctx* ctx;
   SiftWork* wk;
   pano_featureset* fs;
-  float* d_img;
+  void* d_img;
 };
 
 int pano_sift_trace_run(pano_ctx* ctx, const float* rgb, int w, int h, const pano_params* p, pano_sift_trace** out) {
   ctx_enter(ctx);
   if (!ctx || !rgb || !p || !out) return PANO_ERR_INVALID;
   *out = nullptr;
-  std::vector<float*> d_imgs;
-  float* d_block = nullptr;
-  int rc = upload_images(ctx, 1, &rgb, &w, &h, d_imgs, &d_block);
+  std::vector<const void*> d_imgs;
+  unsigned char* d_block = nullptr;
+  const void* src = rgb;
+  int rc = upload_images(ctx, 1, &src, nullptr, &w, &h, d_imgs, &d_block);
   if (rc) { ctx_free(ctx, d_block); return rc; }
   pano_featureset* fs = new pano_featureset;
   fs->ctx = ctx;
   SiftWork* wk = nullptr;
   // the trace keeps the work buffers of ONE run, so it grows the lists itself
   for (int cap = SIFT_CAP_DEFAULT;; cap *= 2) {
-    rc = sift_run_batch(ctx, 1, d_imgs.data(), &w, &h, p, fs, &wk, cap);
+    rc = sift_run_batch(ctx, 1, d_imgs.data(), nullptr, &w, &h, p, fs, &wk, cap);
     if (rc) { featureset_release(fs); ctx_free(ctx, d_block); return rc; }
     rc = featureset_sync_counts(fs);
     if (rc == PANO_ERR_CAPACITY && cap < SIFT_CAP_MAX) {

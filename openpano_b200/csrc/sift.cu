@@ -27,8 +27,17 @@ __device__ __forceinline__ void bilinear_coef(int d, float inv, int src_n, int* 
 
 // The octave-0 grey plane (lib/imgproc.cc:237-249 rgb2grey of the working image) is written
 // here from the same three values, so the working image is not read back for it.
+// kRgb8: the sources are 8-bit pixels, and every tap is the f32 value read_img would have stored
+// (SrcRgb8's rule, common.cuh): the bilinear sample of those taps is the sample of read_img's image.
+// The block must have at least 256 threads (build_rgb8_lut).
+template <bool kRgb8>
 __global__ void k_working_resize(const ImgMeta* __restrict__ imgs, const OctMeta* __restrict__ octs, int n_oct,
                                  float* __restrict__ arena) {
+  __shared__ float lut[kRgb8 ? 256 : 1];
+  if constexpr (kRgb8) {
+    build_rgb8_lut(lut, threadIdx.y * blockDim.x + threadIdx.x);
+    __syncthreads();
+  }
   const ImgMeta im = imgs[blockIdx.z];
   int c = blockIdx.x * blockDim.x + threadIdx.x;
   int r = blockIdx.y * blockDim.y + threadIdx.y;
@@ -37,15 +46,34 @@ __global__ void k_working_resize(const ImgMeta* __restrict__ imgs, const OctMeta
   bilinear_coef(r, im.ifx, im.in_h, &sx, &rx);
   bilinear_coef(c, im.ify, im.in_w, &sy, &ry);
   float irx = 1.0f - rx, iry = 1.0f - ry;
-  const float* p0 = im.src + ((size_t)sx * im.in_w + sy) * 3;
-  const float* p1 = p0 + (size_t)im.in_w * 3;
   float* dst = arena + im.work_off + ((size_t)r * im.w0 + c) * 3;
   float v[3];
+  if constexpr (!kRgb8) {
+    const float* p0 = im.src + ((size_t)sx * im.in_w + sy) * 3;
+    const float* p1 = p0 + (size_t)im.in_w * 3;
 #pragma unroll
-  for (int ch = 0; ch < 3; ++ch) {
-    float p00 = __ldg(p0 + ch), p01 = __ldg(p0 + 3 + ch), p10 = __ldg(p1 + ch), p11 = __ldg(p1 + 3 + ch);
-    v[ch] = rx * (p11 * ry + p10 * iry) + irx * (p01 * ry + p00 * iry);
-    dst[ch] = v[ch];
+    for (int ch = 0; ch < 3; ++ch) {
+      float p00 = __ldg(p0 + ch), p01 = __ldg(p0 + 3 + ch), p10 = __ldg(p1 + ch), p11 = __ldg(p1 + 3 + ch);
+      v[ch] = rx * (p11 * ry + p10 * iry) + irx * (p01 * ry + p00 * iry);
+      dst[ch] = v[ch];
+    }
+  } else if (im.channels == 1) {
+    // read_img replicates the grey value to r, g, b: one sample serves all three channels
+    const unsigned char* p0 = im.pix + (size_t)sx * im.in_w + sy;
+    const unsigned char* p1 = p0 + im.in_w;
+    const float p00 = (float)__ldg(p0), p01 = (float)__ldg(p0 + 1), p10 = (float)__ldg(p1), p11 = (float)__ldg(p1 + 1);
+    const float s = rx * (p11 * ry + p10 * iry) + irx * (p01 * ry + p00 * iry);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) { v[ch] = s; dst[ch] = s; }
+  } else {
+    const unsigned char* p0 = im.pix + ((size_t)sx * im.in_w + sy) * 3;
+    const unsigned char* p1 = p0 + (size_t)im.in_w * 3;
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      float p00 = lut[__ldg(p0 + ch)], p01 = lut[__ldg(p0 + 3 + ch)], p10 = lut[__ldg(p1 + ch)], p11 = lut[__ldg(p1 + 3 + ch)];
+      v[ch] = rx * (p11 * ry + p10 * iry) + irx * (p01 * ry + p00 * iry);
+      dst[ch] = v[ch];
+    }
   }
   const OctMeta& om = octs[blockIdx.z * n_oct];
   arena[om.gauss_off + (size_t)r * om.pitch + c] = (v[0] + v[1] + v[2]) / 3.f;
@@ -1446,7 +1474,7 @@ int ctx_tma_encode(pano_ctx* ctx, TmaDesc* out, void* base, int rank, const unsi
   return PANO_OK;
 }
 
-int sift_run_batch(pano_ctx* ctx, int n, const float* const* d_src, const int* w, const int* h,
+int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w, const int* h,
                    const pano_params* p, pano_featureset* fs, SiftWork** keep, int cap) {
   if (n <= 0 || !d_src || !w || !h || !p || !fs) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: bad argument");
   if (n > SIFT_MAX_IMG) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: %d images in one batch (limit %d): split the batch", n, SIFT_MAX_IMG);
@@ -1475,8 +1503,13 @@ int sift_run_batch(pano_ctx* ctx, int n, const float* const* d_src, const int* w
   std::vector<int2> tilespan((size_t)n * n_oct);
   for (int i = 0; i < n; ++i) {
     if (w[i] < 2 || h[i] < 2) { delete wk; return ctx_fail(ctx, PANO_ERR_INVALID, "sift: image too small"); }
+    if (channels && (channels[i] != 1 && channels[i] != 3)) {
+      delete wk; return ctx_fail(ctx, PANO_ERR_INVALID, "sift: image %d has %d channels (1 or 3)", i, channels[i]);
+    }
     ImgMeta& im = wk->h_img[i];
-    im.src = d_src[i]; im.in_w = w[i]; im.in_h = h[i];
+    if (channels) { im.pix = (const unsigned char*)d_src[i]; im.channels = channels[i]; }
+    else { im.src = (const float*)d_src[i]; im.channels = 3; }
+    im.in_w = w[i]; im.in_h = h[i];
     // feature/feature.cc:33-34
     float ratio = p->sift_working_size * 2.0f / (w[i] + h[i]);
     im.h0 = (int)(h[i] * ratio); im.w0 = (int)(w[i] * ratio);
@@ -1591,8 +1624,11 @@ int sift_run_batch(pano_ctx* ctx, int n, const float* const* d_src, const int* w
   } while (0)
 
   {
-    dim3 b(32, 8), g(ceil_div(max_w0, 32), ceil_div(max_h0, 8), n);
-    SIFT_LAUNCH("k_working_resize", k_working_resize, g, b, 0, wk->d_img, wk->d_oct, n_oct, wk->arena);
+    dim3 b(32, 8), g(ceil_div(max_w0, 32), ceil_div(max_h0, 8), n);   // 256 threads: k_working_resize<true>'s table
+    if (channels)
+      SIFT_LAUNCH("k_working_resize_rgb8", k_working_resize<true>, g, b, 0, wk->d_img, wk->d_oct, n_oct, wk->arena);
+    else
+      SIFT_LAUNCH("k_working_resize", k_working_resize<false>, g, b, 0, wk->d_img, wk->d_oct, n_oct, wk->arena);
     if (n_oct > 1) {   // octave 0's grey came with the working image
       int max_w1 = 0, max_h1 = 0;
       for (int i = 0; i < n; ++i) {
@@ -1719,8 +1755,10 @@ int featureset_sync_counts(pano_featureset* fs) {
     ctx_free(ctx, fs->d_desc); ctx_free(ctx, fs->d_coor); ctx_free(ctx, fs->d_count);
     fs->d_desc = nullptr; fs->d_coor = nullptr; fs->d_real = nullptr; fs->d_count = nullptr;
     ctx->sift_cap = cap;
-    const std::vector<const float*> src = fs->src;
-    int rc = sift_run_batch(ctx, n, src.data(), fs->src_w.data(), fs->src_h.data(), &fs->src_params, fs, nullptr, cap);
+    const std::vector<const void*> src = fs->src;
+    const std::vector<int> channels = fs->src_channels;
+    int rc = sift_run_batch(ctx, n, src.data(), channels.empty() ? nullptr : channels.data(), fs->src_w.data(),
+                            fs->src_h.data(), &fs->src_params, fs, nullptr, cap);
     if (rc) return fs->error = rc;
   }
   if (fs->owned_block) { ctx_free(ctx, fs->owned_block); fs->owned_block = nullptr; }

@@ -13,11 +13,15 @@
 #define SIFT_MAX_PEAKS 18        // a peak needs two lower neighbours: <= 36/2
 
 struct ImgMeta {
-  const float* src;   // input RGB (device)
+  union {
+    const float* src;           // input, h×w×3 f32 (device)
+    const unsigned char* pix;   // input, h×w×channels u8 (device), read as SrcRgb8 reads it
+  };
   int in_w, in_h;
   int w0, h0;         // working size
   float ifx, ify;     // 1/fx (rows), 1/fy (cols) of the working resize
   long long work_off; // working RGB offset in the arena (floats)
+  int channels;       // u8 sources only: 1 or 3
 };
 
 struct OctMeta {
@@ -87,13 +91,15 @@ struct pano_featureset {
   // What a capacity overflow needs to run the batch again with larger lists (SIFT sets only):
   // the sources must stay valid until the counts have been read once (pano_b200.h).
   int cap = 0;                          // per-image row capacity of d_desc / d_coor (0: not a SIFT set)
-  std::vector<const float*> src;        // device images
+  std::vector<const void*> src;         // device images
+  std::vector<int> src_channels;        // u8 sources: channels per image; empty: f32 sources
   std::vector<int> src_w, src_h;
   pano_params src_params;
-  float* owned_block = nullptr;         // staged upload of pano_sift_detect_batch, freed after the count sync
+  void* owned_block = nullptr;          // staged upload of the host entry points, freed after the count sync
 };
 
-int sift_run_batch(pano_ctx* ctx, int n, const float* const* d_src, const int* w, const int* h,
+// d_src: h×w×3 f32 device images when channels is null, else h×w×channels[i] u8 device images
+int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w, const int* h,
                    const pano_params* p, pano_featureset* fs, SiftWork** keep, int cap);
 void sift_work_free(pano_ctx* ctx, SiftWork* wk);
 int featureset_sync_counts(pano_featureset* fs);

@@ -92,6 +92,25 @@ class B200SIFTDetector : public pano::FeatureDetector {
     pano_params p = snapshot_params();
     pano_featureset* fs = nullptr;
     c_.check(pano_sift_detect_batch(c_.get(), n, ptr.data(), w.data(), h.data(), &p, &fs));
+    return unpack_batch(fs, n, keep);
+  }
+  // detect_batch for callers that decode the files themselves: pix[k] is h[k]×w[k]×channels[k] interleaved
+  // 8-bit pixels in host memory (channels 1 or 3, what read_img converts, lib/imgio.cc:72-88).  Returns what
+  // detect_batch returns on read_img's Mat32f of the same pixels, without building those images.
+  std::vector<std::vector<pano::Descriptor>> detect_batch_rgb8(const std::vector<const unsigned char*>& pix,
+                                                               const std::vector<int>& w, const std::vector<int>& h,
+                                                               const std::vector<int>& channels,
+                                                               pano_featureset** keep = nullptr) const {
+    const int n = (int)pix.size();
+    if ((int)w.size() != n || (int)h.size() != n || (int)channels.size() != n)
+      error_exit("B200SIFTDetector::detect_batch_rgb8: pix, w, h and channels differ in length");
+    pano_params p = snapshot_params();
+    pano_featureset* fs = nullptr;
+    c_.check(pano_sift_detect_batch_rgb8(c_.get(), n, pix.data(), w.data(), h.data(), channels.data(), &p, &fs));
+    return unpack_batch(fs, n, keep);
+  }
+ private:
+  std::vector<std::vector<pano::Descriptor>> unpack_batch(pano_featureset* fs, int n, pano_featureset** keep) const {
     std::vector<std::vector<pano::Descriptor>> feats(n);
     for (int k = 0; k < n; ++k) {
       feats[k] = unpack(fs, k, /*real=*/false);
@@ -100,7 +119,6 @@ class B200SIFTDetector : public pano::FeatureDetector {
     if (keep) *keep = fs; else pano_featureset_free(fs);
     return feats;
   }
- private:
   std::vector<pano::Descriptor> unpack(pano_featureset* fs, int k, bool real) const {
     const int m = pano_featureset_count(fs, k);
     if (m < 0) error_exit(pano_last_error(c_.get()));

@@ -22,14 +22,22 @@ T = time.perf_counter
 
 
 def timed_run(k, out_ptr):
-    s = ps.slots[k]; sh = s["shapes"]; p = [s["imgs"] + o for o in s["offs"]]
+    s = ps.slots[k]; sh = s["shapes"]
     ws, hs = [q[1] for q in sh], [q[0] for q in sh]
     t0 = T(); ps.cmp.event_wait(s["ev_up"])
     if rgb8:
-        ps.cmp.rgb8_to_mat32f_batch_dev([s["pix"] + o for o in s["pix_offs"]], ws, hs, [3] * len(sh), p)
-    fs = ps.cmp.sift_detect_batch_ptr(p, ws, hs, params, device=True); t1 = T()
+        p = [s["pix"] + o for o in s["pix_offs"]]
+        fs = ps.cmp.sift_detect_batch_rgb8_ptr(p, ws, hs, [3] * len(sh), params, device=True)
+    else:
+        p = [s["imgs"] + o for o in s["offs"]]
+        fs = ps.cmp.sift_detect_batch_ptr(p, ws, hs, params, device=True)
+    t1 = T()
     m = ps.cmp.match_pairs(fs, pairs, params); t2 = T()
-    ps.cmp.event_wait(s["ev_dn"]); ps.cmp.blend_dev(p, sh, items, geom, s["out"], ow, oh, 0, params)
+    ps.cmp.event_wait(s["ev_dn"])
+    if rgb8:
+        ps.cmp.blend_rgb8_dev(p, [3] * len(sh), sh, items, geom, s["out"], ow, oh, 0, params)
+    else:
+        ps.cmp.blend_dev(p, sh, items, geom, s["out"], ow, oh, 0, params)
     if rgb8:
         ps.cmp.crop_rect_dev(s["out"], ow, oh, s["out8"])
         ps.cmp.mat32f_to_rgb8_dev(s["out"], ow, oh, s["out8"], s["out8"] + ps.RGB8_HEADER)

@@ -72,10 +72,10 @@ def wrap(obj, name, lane, label, before=None, after=None):
 
 for q, ps in enumerate(lanes.lanes):
     s_up, s_cmp, s_dn = (torch.cuda.ExternalStream(e.stream) for e in (ps.up, ps.cmp, ps.dn))
-    wrap(ps.cmp, "rgb8_to_mat32f_batch_dev", q, "cmp.rgb8_to_f32", before=("c0 compute starts", s_cmp))
-    wrap(ps.cmp, "sift_detect_batch_ptr", q, "cmp.sift", after=("c1 sift enqueued", s_cmp))
+    wrap(ps.cmp, "sift_detect_batch_rgb8_ptr", q, "cmp.sift", before=("c0 compute starts", s_cmp),
+         after=("c1 sift enqueued", s_cmp))
     wrap(ps.cmp, "match_pairs", q, "cmp.match_pairs", after=("c2 match lists on host", s_cmp))
-    wrap(ps.cmp, "blend_dev", q, "cmp.blend")
+    wrap(ps.cmp, "blend_rgb8_dev", q, "cmp.blend")
     wrap(ps.cmp, "event_record", q, "cmp.event_record", before=("c3 blend+convert enqueued", s_cmp))
     wrap(ps.dn, "dev_download_async", q, "dn.download_async", after=("d1 download enqueued", s_dn))
     wrap(ps.cmp, "event_wait", q, "cmp.event_wait")
