@@ -20,7 +20,7 @@ struct ImgMeta {
   int in_w, in_h;
   int w0, h0;         // working size
   float ifx, ify;     // 1/fx (rows), 1/fy (cols) of the working resize
-  long long work_off; // working RGB offset in the arena (floats)
+  long long work_off; // working RGB offset in the arena (floats); a trace's arena only holds it
   int channels;       // u8 sources only: 1 or 3
 };
 

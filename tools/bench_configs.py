@@ -54,8 +54,10 @@ def algorithmic_bytes(shapes, items, params, counts, bands):
     tw, th = max(it[2] for it in items), max(it[3] for it in items)
     return {
         "k_rgb8_to_f32": p_in * 15,
-        "k_working_resize": min(p_in, 4 * p0) * 12 + p0 * 12,
-        "k_octave_grey": p0 * 12 + sp * 4,
+        # the source's bilinear taps (at most 4 per working pixel) in, every octave's grey plane out; the
+        # working RGB image is a shared-memory tile.  8-bit sources: 3 B per tap pixel (1 for grey ones)
+        "k_pyramid_grey": min(p_in, 4 * p0) * 12 + sp * 4,
+        "k_pyramid_grey_rgb8": min(p_in, 4 * p0) * 3 + sp * 4,
         # kw in {7, 13}: blur + |DoG| + extrema of the tile interiors in one pass; |DoG| is a fused
         # temporary.  The seam test (k_extrema_seams) re-reads levels around the few tile-perimeter
         # pixels above the colour threshold, which is not compulsory traffic: it has no bytes of its
