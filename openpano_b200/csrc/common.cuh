@@ -26,6 +26,8 @@ struct ProfEvent {
   cudaEvent_t start, stop;
 };
 
+struct SiftPlan;   // sift.cuh
+
 struct pano_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
@@ -50,6 +52,11 @@ struct pano_ctx {
   // cudaFuncSetAttribute is per device: remembered per context, never per process
   bool attr_tc = false, attr_match = false;
   int sift_cap = 0;                // per-image list capacity SIFT batches start with (grows on overflow, sticky)
+  // The last SIFT batch's shape-dependent setup (sift.cu), one entry; its device bytes count against
+  // cache_limit, so PANO_CACHE_MB=0 keeps none.  pano_trim, pano_destroy and ctx_alloc's
+  // out-of-memory retry release it.
+  SiftPlan* sift_plan = nullptr;
+  size_t sift_plan_bytes = 0;
   void* tma_encode = nullptr;      // cuTensorMapEncodeTiled, resolved through the runtime (no -lcuda)
   // pinned host staging (grown on demand)
   void* pinned = nullptr;
@@ -92,6 +99,7 @@ int  ctx_cuda(pano_ctx* ctx, cudaError_t e, const char* what);
 int  ctx_alloc(pano_ctx* ctx, void** p, size_t bytes);
 void ctx_cache_release(pano_ctx* ctx, size_t keep_bytes);
 void ctx_free(pano_ctx* ctx, void* p);
+void ctx_sift_plan_release(pano_ctx* ctx);   // frees the kept SIFT plan's blocks (into the cache)
 void* ctx_pinned(pano_ctx* ctx, size_t bytes);   // staging buffer A (inputs)
 void* ctx_pinned2(pano_ctx* ctx, size_t bytes);  // staging buffer B (results)
 extern "C" bool host_is_pinned(const void* p);   // page-locked (cudaHostAlloc / pano_host_alloc) host memory

@@ -52,8 +52,9 @@ int ctx_alloc(pano_ctx* ctx, void** p, size_t bytes) {
     }
   }
   cudaError_t e = ctx->pool ? cudaMallocFromPoolAsync(p, bytes, ctx->pool, ctx->stream) : cudaMallocAsync(p, bytes, ctx->stream);
-  if (e != cudaSuccess && ctx->cached_bytes) {      // out of memory with blocks parked here: give them back, retry
+  if (e != cudaSuccess && (ctx->cached_bytes || ctx->sift_plan)) {   // out of memory with blocks parked here: give them back, retry
     cudaGetLastError();
+    ctx_sift_plan_release(ctx);
     ctx_cache_release(ctx, 0);
     e = ctx->pool ? cudaMallocFromPoolAsync(p, bytes, ctx->pool, ctx->stream) : cudaMallocAsync(p, bytes, ctx->stream);
   }
@@ -84,7 +85,15 @@ void ctx_free(pano_ctx* ctx, void* p) {
   if (!ctx->cache_limit || size > ctx->cache_limit) { cudaFreeAsync(p, ctx->stream); return; }
   ctx->cache.emplace(size, pano_ctx::CachedBlock{p, ++ctx->cache_stamp});
   ctx->cached_bytes += size;
-  if (ctx->cached_bytes > ctx->cache_limit) ctx_cache_release(ctx, ctx->cache_limit);
+  if (ctx->cached_bytes + ctx->sift_plan_bytes > ctx->cache_limit)   // the kept SIFT plan shares the budget
+    ctx_cache_release(ctx, ctx->cache_limit - std::min(ctx->sift_plan_bytes, ctx->cache_limit));
+}
+
+void ctx_sift_plan_release(pano_ctx* ctx) {
+  SiftPlan* plan = ctx->sift_plan;
+  ctx->sift_plan = nullptr;
+  ctx->sift_plan_bytes = 0;
+  sift_plan_free(ctx, plan);
 }
 
 static void* grow_pinned(void** buf, size_t* cap, size_t bytes) {
@@ -487,6 +496,7 @@ int pano_create(pano_ctx** out, int device, void* cuda_stream) {
 int pano_trim(pano_ctx* ctx) {
   if (!ctx) return PANO_ERR_INVALID;
   ctx_enter(ctx);
+  ctx_sift_plan_release(ctx);
   ctx_cache_release(ctx, 0);
   return PANO_OK;
 }
@@ -507,6 +517,7 @@ int pano_mem_high_water(pano_ctx* ctx, size_t* bytes, int reset) {
 void pano_destroy(pano_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
+  ctx_sift_plan_release(ctx);
   ctx_cache_release(ctx, 0);
   if (ctx->planet_tab) cudaFreeAsync(ctx->planet_tab, ctx->stream);
   cudaStreamSynchronize(ctx->stream);

@@ -70,6 +70,20 @@ struct SiftWork {
   float* desc_dir = nullptr;        // [n_img * cap]
 };
 
+// What a batch's shape alone decides, kept by the context (pano_ctx::sift_plan) for the next batch of the
+// same shape: the work buffers with their arena, the uploaded OctMeta / tile spans / TMA maps (valid
+// because the arena stays put), the Gaussian table and the launch sizes.  A repeat batch only uploads its
+// ImgMeta (the source pointers) and resets the counters.
+struct SiftPlan {
+  std::vector<int> key;           // see sift_plan_key: n, cap, every (w, h, source kind), pano_params
+  SiftWork* wk = nullptr;
+  size_t bytes = 0;               // device bytes held (counted against the context's cache_limit)
+  GaussTable gt;
+  bool fast = true;
+  size_t seam_cap = 0;
+  int max_w0 = 0, max_h0 = 0;
+};
+
 struct pano_featureset {
   pano_ctx* ctx = nullptr;
   int n_images = 0;
@@ -102,4 +116,5 @@ struct pano_featureset {
 int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w, const int* h,
                    const pano_params* p, pano_featureset* fs, SiftWork** keep, int cap);
 void sift_work_free(pano_ctx* ctx, SiftWork* wk);
+void sift_plan_free(pano_ctx* ctx, SiftPlan* plan);
 int featureset_sync_counts(pano_featureset* fs);

@@ -27,8 +27,7 @@ class Stitcher:
     def __init__(self, engine: Engine, params=None, overlap_blend: bool = True):
         """overlap_blend: the composite depends on the images and the caller's geometry only, not
         on the features (the geometry in between is host code), so it runs on a second context /
-        stream of the same device next to SIFT + matching: its bandwidth-bound kernels fill the
-        gaps of the issue-bound descriptor kernel.  Ordered with events; results are unchanged."""
+        stream of the same device, ordered with events (see run_device); results are unchanged."""
         self.eng = engine
         self.params = params or default_params()
         self._aux = None
@@ -97,14 +96,17 @@ class Stitcher:
         (featureset, matches-or-total)."""
         shapes = self._shapes
         ptrs = self.image_ptrs()
+        fs = self.eng.sift_detect_batch_ptr(ptrs, [s[1] for s in shapes], [s[0] for s in shapes], self.params,
+                                            device=True)
         if self._overlap:
+            # The composite waits for SIFT's last kernel.  Queued ahead of SIFT, its grid filled every SM and
+            # SIFT's kernels waited behind it; waiting for the images only, it slowed SIFT by more than it
+            # saved.  Behind SIFT it runs while the host reads the feature counts and plans the matcher.
             aux = self._aux_engine()
-            self.eng.event_record(self._ev_in)          # images (and the previous reader of d_out) are done on the main stream
+            self.eng.event_record(self._ev_in)
             aux.event_wait(self._ev_in)
             aux.blend_dev(ptrs, shapes, items, geom, self._d_out, self._out_shape[0], self._out_shape[1], bands, self.params)
             aux.event_record(self._ev_blend)
-        fs = self.eng.sift_detect_batch_ptr(ptrs, [s[1] for s in shapes], [s[0] for s in shapes], self.params,
-                                            device=True)
         if want_matches:
             m = self.eng.match_pairs(fs, pairs, self.params)
         else:
