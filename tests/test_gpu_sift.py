@@ -99,28 +99,6 @@ def test_sift_wide_descriptor_windows(engine, orc, hist_scale, ori_radius):
     assert_same("desc", d, do)
 
 
-def test_first_design_kernels_agree(engine, monkeypatch):
-    """The first designs of the orientation / descriptor kernels (warp per keypoint), kept behind
-    PANO_ORI_V1 / PANO_DESC_V1 as in-engine cross-checks, produce the same bits as the shipped quad kernels."""
-    imgs, _ = synth.make_stack(3, 480, 360, 160, 51)
-    monkeypatch.delenv("PANO_ORI_V1", raising=False)
-    monkeypatch.delenv("PANO_DESC_V1", raising=False)
-    fs = engine.sift_detect_batch(imgs)
-    want = [fs.download(i) for i in range(3)]
-    fs.free()
-    monkeypatch.setenv("PANO_ORI_V1", "1")
-    monkeypatch.setenv("PANO_DESC_V1", "1")
-    fs = engine.sift_detect_batch(imgs)
-    got = [fs.download(i) for i in range(3)]
-    fs.free()
-    monkeypatch.delenv("PANO_ORI_V1", raising=False)
-    monkeypatch.delenv("PANO_DESC_V1", raising=False)
-    for i in range(3):
-        assert len(want[i][1]) > 200
-        assert_same(f"coor[{i}]", got[i][0], want[i][0])
-        assert_same(f"desc[{i}]", got[i][1], want[i][1])
-
-
 def test_sift_flat_image_has_no_features(engine, orc):
     img = np.full((200, 300, 3), 0.5, np.float32)
     c, d = engine.sift_detect(img)

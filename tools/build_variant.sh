@@ -1,6 +1,6 @@
 #!/bin/bash
 # Builds a variant of the library with extra -D flags on one translation unit:
-#   tools/build_variant.sh <name> <file.cu> "-DDESC_HCAP=128 -DDESC_CTAS_PER_SM=5"
+#   tools/build_variant.sh <name> <file.cu> "-DDESC_MIN_CTAS=5"
 # -> openpano_b200/_variants/<name>.so (git-ignored); use with
 #   PANO_B200_LIB=openpano_b200/_variants/<name>.so python tools/ab_value.py
 set -e
