@@ -11,8 +11,20 @@
 // of K = 144 (128 + one extra 16-wide k-step):
 //     query  form: [ s*x        | 1, 1, n_hi, n_lo, 1, 0... ]
 //     target form: [ -2*s*x     | n_hi, n_lo, 1, 1, 1, 0... ]     n = s^2*|x|^2
-// so that  q . t = s^2 * |xq - xt|^2 + 1   (>= ~1: positive floats order like
-// ints).  s is a power of two making n <= 1024 (s = 1/16 for RootSIFT, |x| = 512).
+// so that  q . t ~ s^2 * |xq - xt|^2 + 1.  s is a power of two making n <= 1024 (s = 1/16 for RootSIFT,
+// |x| = 512).  The score is NOT always positive: with f = fp16(s*x), q . t = s^2 |fq - ft|^2 + 1
+// + (nq - |fq|^2) + (nt - |ft|^2), and each bracket reaches -n/1024, so a row against a near-duplicate of
+// itself scores down to 1 - n/512 (-1 at n = 1024; ~-0.98 for rows whose components all sit just above
+// fp16 midpoints).  Negative scores order backwards as signed-int keys, so among two such targets the
+// top-2 may nominate the worse as best, with m2 < m1.  The decision stays exact because every
+// approximate distance lies within tc_eps of the exact one, and m + tc_eps > 0 for every reachable m:
+// refine_row then finds the argmin uncertain, keeps lower bounds of 0 and positive upper bounds, and the
+// row is re-scanned exactly.  Until then its bounds also serve as a column's bounds in k_match_decide,
+// where sec_hi = m2 + eps can lie below min_{kk != k} d(j, kk) when k is the column behind m2.  That
+// bound can only reject row k (its lower bound c_lo is 0), and every row k it rejects is one the
+// reference rejects too; the filter threshold m2 + 2.5 eps still covers every column that can be the
+// exact best or second best (|m1 - m2| stays below eps / 2).  tests/test_match_bound.py checks these
+// facts on the operands of k_tc_prep; tests/test_gpu_match_warp_blend.py runs such rows on the device.
 // Rows are stored PRE-BLOCKED in the canonical K-major no-swizzle layout of wgmma shared-memory
 // operands (8x16-byte core matrices, SBO = 128 B): query rows in 128-row blocks (LBO = 2 KiB),
 // target rows in 256-row tiles (LBO = 4 KiB), so one contiguous cp.async.bulk brings a block / tile

@@ -98,13 +98,16 @@ def test_match_empty(engine, match_mode):
     assert len(engine.match_bruteforce(a, np.zeros((0, 128), np.float32))) == 0
 
 
-@pytest.mark.parametrize("w,h,hf", [(600, 400, 1.0), (300, 200, 0.85), (257, 311, 1.2)])
-def test_cyl_warp_bit_exact(engine, orc, w, h, hf):
+@pytest.mark.parametrize("w,h,hf,focal", [(600, 400, 1.0, 37.0), (300, 200, 0.85, 37.0), (257, 311, 1.2, 37.0),
+                                          (300, 200, 1.0, 24.0), (257, 311, 0.85, 50.0)])
+def test_cyl_warp_bit_exact(engine, orc, w, h, hf, focal):
+    """FOCAL_LENGTH sets the cylinder radius (warp.cu)."""
     img = synth.make_canvas(h, w, 51)
     k = np.array([[10.5, -20.25], [-100.0, 50.0], [0.0, 0.0]])
-    assert engine.cyl_warp_shape(w, h, hf) == orc.cyl_warp_shape(w, h, hf)
-    ga, gk = engine.cyl_warp(img, k, hf)
-    oa, ok = orc.cyl_warp(img, k, hf)
+    p = default_params(focal_length=focal)
+    assert engine.cyl_warp_shape(w, h, hf, p) == orc.cyl_warp_shape(w, h, hf, p)
+    ga, gk = engine.cyl_warp(img, k, hf, p)
+    oa, ok = orc.cyl_warp(img, k, hf, p)
     assert np.array_equal(gk, ok)
     assert ga.shape == oa.shape
     assert np.array_equal(ga.view(np.uint32), oa.view(np.uint32)), np.abs(ga - oa).max()
@@ -139,12 +142,15 @@ def test_linear_blend_bit_exact(engine, orc, lazy, ordered):
     assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), np.abs(a - b).max()
 
 
+@pytest.mark.parametrize("gauss_window_factor", [6, 4, 8])
 @pytest.mark.parametrize("bands", [1, 2, 5])
-def test_multiband_blend_bit_exact(engine, orc, bands):
+def test_multiband_blend_bit_exact(engine, orc, bands, gauss_window_factor):
+    """GAUSS_WINDOW_FACTOR sets the multiband blender's tap count and halo (blend.cu)."""
     imgs, org = synth.make_stack(4, 300, 200, 100, 7)
     items, geom = synth.translation_blend_setup(org, 300, 200)
-    a = engine.blend(imgs, items, geom, bands)
-    b = orc.blend(imgs, items, geom, bands)
+    p = default_params(multiband=bands, gauss_window_factor=gauss_window_factor)
+    a = engine.blend(imgs, items, geom, bands, p)
+    b = orc.blend(imgs, items, geom, bands, p)
     assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), np.abs(a - b).max()
 
 
@@ -197,14 +203,15 @@ def test_match_tensor_path_equals_exact_path(engine, orc, monkeypatch, match_mod
     assert 50 < len(want) < 1300
 
 
+@pytest.mark.parametrize("gauss_window_factor", [6, 4, 8])
 @pytest.mark.parametrize("bands", [0, 2, 5])
-def test_blend_row_strips_equal_full_canvas(engine, bands):
+def test_blend_row_strips_equal_full_canvas(engine, bands, gauss_window_factor):
     """pano_blend_rows_dev: uneven row strips (the multi-GPU partition of the canvas) concatenate to
     exactly the mosaic pano_blend_dev produces — for the multiband blender through ROIs clipped to
-    the strip plus the summed blur half-widths."""
+    the strip plus the summed blur half-widths, which GAUSS_WINDOW_FACTOR sets."""
     imgs, org = synth.make_stack(5, 260, 200, 90, 77, rows=2, step_y=70)
     items, geom = synth.translation_blend_setup(org, 260, 200)
-    p = default_params(multiband=bands, lazy_read=0)
+    p = default_params(multiband=bands, lazy_read=0, gauss_window_factor=gauss_window_factor)
     shapes = [im.shape[:2] for im in imgs]
     tw, th = max(it[2] for it in items), max(it[3] for it in items)
     d_imgs = [engine.dev_alloc(im.nbytes) for im in imgs]
@@ -225,3 +232,120 @@ def test_blend_row_strips_equal_full_canvas(engine, bands):
         engine.dev_free(d)
     got = np.concatenate(parts)
     assert got.tobytes() == full.tobytes()
+
+
+# ----------------------------------------------------------------------------- matcher edges
+# The inputs come from tests/test_match_bound.py, whose CPU model checks tc_eps on the same sets.
+from tests import test_match_bound as mb  # noqa: E402
+
+
+def _match_both_ways(engine, orc, monkeypatch, a, b, params=None):
+    """a x b and b x a on the tensor path and on the exact fp32 path, each against the oracle."""
+    want = [orc.match(a, b, params), orc.match(b, a, params)]
+    for path in (None, "exact"):
+        if path:
+            monkeypatch.setenv("PANO_MATCH_PATH", path)
+        else:
+            monkeypatch.delenv("PANO_MATCH_PATH", raising=False)
+        got = [engine.match_bruteforce(a, b, params), engine.match_bruteforce(b, a, params)]
+        for g, w, d in zip(got, want, ("ab", "ba")):
+            assert np.array_equal(g, w), (path, d, len(g), len(w))
+    monkeypatch.delenv("PANO_MATCH_PATH", raising=False)
+    return want
+
+
+@pytest.mark.parametrize("ratio", [0.5, 0.6, 0.9, 0.95, 1.0])
+def test_match_ratios(engine, orc, monkeypatch, match_mode, ratio):
+    """MATCH_REJECT_NEXT_RATIO (refine_row's skip rule, every interval test of k_match_decide), on targets
+    with noise from 60 down to 10.  The first 150 targets come twice, so their rows tie exactly
+    (min == next_min): ratio 1.0 accepts those whose column test passes too."""
+    rng = np.random.RandomState(31)
+    a = synth.rootsift_like(400, 31)
+    level = np.linspace(60, 10, 320).astype(np.float32)[:, None]
+    noisy = a[rng.permutation(400)][:320] + rng.randn(320, 128).astype(np.float32) * level
+    b = np.concatenate([noisy[:150], noisy[:150], noisy[150:]])
+    want = _match_both_ways(engine, orc, monkeypatch, a, b, default_params(match_reject_next_ratio=ratio))
+    assert len(want[0]) > (150 if ratio == 1.0 else 40)
+
+
+EDGE_SIZES = [127, 128, 129, 255, 256, 257, 383, 385, 511, 512, 513]
+
+
+@pytest.mark.parametrize("n,m", list(zip(EDGE_SIZES, EDGE_SIZES[5:] + EDGE_SIZES[:5])))
+def test_match_block_edges(engine, orc, monkeypatch, match_mode, n, m):
+    """Set sizes at the edges of the 128-row query blocks, 256-row target tiles and 64-row exact tiles."""
+    a, b = mb.random_rows(n, m, n + m)
+    want = _match_both_ways(engine, orc, monkeypatch, a, b)
+    assert len(want[0]) > min(n, m) // 10
+
+
+@pytest.mark.parametrize("scale", mb.SCALES)
+def test_match_scaled_descriptors(engine, orc, monkeypatch, match_mode, scale):
+    """Descriptor norms other than 512 (DESC_INT_FACTOR): the fp16 scale s and tc_eps follow the norm."""
+    a, b = mb.scaled_rows(scale)
+    want = _match_both_ways(engine, orc, monkeypatch, a, b)
+    assert len(want[0]) > 20
+
+
+def _match_pairs_both_paths(engine, orc, monkeypatch, fs, sets, pairs, params=None):
+    """match_pairs on the tensor path and on the exact fp32 path, every pair against the oracle."""
+    want = [orc.match(sets[i], sets[j], params) for i, j in pairs]
+    for path in (None, "exact"):
+        if path:
+            monkeypatch.setenv("PANO_MATCH_PATH", path)
+        else:
+            monkeypatch.delenv("PANO_MATCH_PATH", raising=False)
+        for (i, j), g, w in zip(pairs, engine.match_pairs(fs, pairs, params), want):
+            assert np.array_equal(g, w), (path, i, j, len(g), len(w))
+    monkeypatch.delenv("PANO_MATCH_PATH", raising=False)
+    return want
+
+
+def test_match_mixed_norms_one_featureset(engine, orc, monkeypatch, match_mode):
+    """k_tc_maxnorm takes one maximum over the whole feature set: a norm-2 image is matched at the
+    scale of a norm-512 one."""
+    sets = mb.mixed_rows()
+    fs = engine.featureset_upload(sets)
+    pairs = [(0, 1), (1, 0), (2, 3), (3, 2), (0, 2), (2, 0), (3, 1), (1, 3)]
+    want = _match_pairs_both_paths(engine, orc, monkeypatch, fs, sets, pairs)
+    fs.free()
+    assert len(want[2]) > 20
+
+
+@pytest.mark.parametrize("factor", [100, 4096])
+def test_match_sift_features_other_desc_int_factor(engine, orc, monkeypatch, match_mode, factor):
+    imgs, _ = synth.make_stack(3, 360, 270, 120, 43)
+    p = default_params(desc_int_factor=factor)
+    fs = engine.sift_detect_batch(imgs, p)
+    descs = [fs.download(i)[1] for i in range(3)]
+    pairs = [(0, 1), (1, 0), (1, 2), (2, 1), (2, 0), (0, 2)]
+    want = _match_pairs_both_paths(engine, orc, monkeypatch, fs, descs, pairs, p)
+    fs.free()
+    assert sum(len(w) for w in want) > 30
+
+
+def test_match_adversarial_fp16_rounding(engine, orc, monkeypatch, match_mode):
+    """Rows whose fp16 rounding errors all have one sign (scores down to ~-1), exact duplicates,
+    near-duplicates across fp16 midpoints, permutations, and the ratio trap that a bound below ~40% of
+    tc_eps decides wrongly."""
+    a, b = mb.adversarial_rows(48, 2)
+    want = _match_both_ways(engine, orc, monkeypatch, a, b)
+    assert len(want[0]) > 40
+
+
+@pytest.mark.parametrize("parts,block_cap", [("2", None), ("3", None), ("8", None), (None, "1")])
+def test_match_adversarial_split_and_fallback(engine, orc, monkeypatch, match_mode, parts, block_cap):
+    """The adversarial rows under PANO_MATCH_PARTS column ranges (among 8200 far targets, so that 8 parts
+    keep 4 tiles each) and with PANO_MATCH_BLOCK_CAP=1 (every requested row re-scanned in full)."""
+    a, b = mb.adversarial_rows(48, 5)
+    far = (synth.rootsift_like(8200, 14) * np.float32(0.99)).astype(np.float32)
+    b = np.concatenate([far[:4000], b, far[4000:]])
+    for k, v in (("PANO_MATCH_PARTS", parts), ("PANO_MATCH_BLOCK_CAP", block_cap)):
+        if v:
+            monkeypatch.setenv(k, v)
+    got = [engine.match_bruteforce(a, b), engine.match_bruteforce(b, a)]
+    monkeypatch.delenv("PANO_MATCH_PARTS", raising=False)
+    monkeypatch.delenv("PANO_MATCH_BLOCK_CAP", raising=False)
+    assert np.array_equal(got[0], orc.match(a, b))
+    assert np.array_equal(got[1], orc.match(b, a))
+    assert len(got[0]) > 40

@@ -7,6 +7,7 @@ import pytest
 
 from openpano_b200 import synth
 from openpano_b200._abi import default_params
+from tests.test_oracle_vs_ref import SIFT_PARAM_SETS, min_points, sift_set_input
 
 pytestmark = pytest.mark.gpu
 
@@ -85,11 +86,11 @@ def test_sift_other_params(engine, orc):
     g.close(); o.close()
 
 
-@pytest.mark.parametrize("hist_scale,ori_radius", [(8, 4.5), (17, 9.0)])
+@pytest.mark.parametrize("hist_scale,ori_radius", [(8, 4.5), (17, 9.0), (20, 4.5)])
 def test_sift_wide_descriptor_windows(engine, orc, hist_scale, ori_radius):
     """Descriptor windows wider than one interval-table block of k_descriptor (96 columns: DESC_HIST_SCALE_FACTOR 8
-    gives windows of up to ~110 columns, 17 of up to ~215, close to the 255 the kernel's tables hold) and wide
-    orientation windows."""
+    gives windows of up to ~110 columns, 17 of up to ~215, 20 of up to ~250, close to the 255 the kernel's tables
+    hold) and wide orientation windows."""
     img = synth.make_canvas(360, 480, 41)
     p = default_params(desc_hist_scale_factor=hist_scale, ori_radius=ori_radius)
     c, d = engine.sift_detect(img, p)
@@ -118,3 +119,39 @@ def test_descriptor_properties_full_size(engine):
         assert d.min() >= 0 and d.max() <= 512
         assert np.all(np.abs(c[:, 0]) <= 1300 / 2) and np.all(np.abs(c[:, 1]) <= 867 / 2)
     fs.free()
+
+
+def test_sift_refuses_windows_beyond_the_tables():
+    """The descriptor-radius bound follows OFFSET_THRES: at 6 a refined scale index can pass nscale - 1, and
+    DESC_HIST_SCALE_FACTOR 17 (accepted at the default 0.5) gives windows past radius 127."""
+    from openpano_b200.capi import Engine, PanoError
+    e = Engine(0)
+    try:
+        with pytest.raises(PanoError) as ei:
+            e.sift_detect(synth.make_canvas(180, 260, 31), default_params(desc_hist_scale_factor=17, offset_thres=6.0))
+        assert ei.value.code == -2
+    finally:
+        e.close()
+
+
+@pytest.mark.parametrize("field,value", SIFT_PARAM_SETS)
+def test_sift_param_sets_bit_exact(engine, orc, field, value):
+    """The config values tests/test_oracle_vs_ref.py pins to the reference, on the same inputs.  Sets that
+    change the planes (NUM_SCALE, GAUSS_SIGMA) are compared stage by stage, the others through the batch
+    entry point."""
+    img, p = sift_set_input(field, value)
+    min_cand, min_desc = min_points(field, value)
+    if field in ("num_scale", "gauss_sigma", "all"):
+        g, o = engine.sift_trace(img, p), orc.sift_trace(img, p)
+        n = compare_trace(g, o, nscale=p.num_scale, noct=p.num_octave)
+        assert len(o.points(0)) >= min_cand
+        g.close(); o.close()
+    else:
+        fs = engine.sift_detect_batch([img], p)
+        c, d = fs.download(0)
+        fs.free()
+        co, do = orc.sift_detect(img, p)
+        assert_same("coor", c, co)
+        assert_same("desc", d, do)
+        n = len(d)
+    assert n >= min_desc

@@ -97,8 +97,11 @@ def test_repeat_and_new_images(monkeypatch, eng):
 
 def test_shapes_n_and_params_change(monkeypatch, eng):
     p, p5 = default_params(), default_params(num_octave=5, scale_factor=1.3)
+    # same shapes, other tables: the Gaussian taps, the orientation smoothing and the descriptor scale
+    pg, po, pd = default_params(gauss_sigma=1.6), default_params(ori_hist_smooth_count=0), default_params(desc_int_factor=100)
     full, other = _imgs(SHAPES, 21), _imgs([(517, 333), (800, 600), (641, 417)], 22)
-    cases = [(full, p), (full[:2], p), (other, p), (full, p5), (full, p), (full[1:], p5), (full, p)]
+    cases = [(full, p), (full[:2], p), (other, p), (full, p5), (full, p), (full[1:], p5), (full, p),
+             (full, pg), (full, po), (full, pd), (full, p)]
     for srcs, params in cases:
         b = Batch(eng, srcs)
         try:

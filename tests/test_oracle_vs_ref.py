@@ -67,7 +67,42 @@ def case_sift_other_params(chk):
     return _trace_outputs(chk.sift_trace(img, p), noct=3, nscale=6)
 
 
-WIDE_WINDOWS = [(8, 4.5), (17, 9.0)]
+# Config values off their defaults, each reaching its own device code; "all" changes them at once.
+SIFT_PARAM_SETS = [("gauss_sigma", 1.6), ("gauss_sigma", 2.0), ("num_scale", 4), ("num_scale", 5), ("num_scale", 8),
+                   ("num_scale", 9), ("num_octave", 8), ("pre_color_thres", 0.01), ("judge_extrema_diff_thres", 0.0),
+                   ("judge_extrema_diff_thres", 0.01), ("offset_thres", 0.3), ("ori_hist_smooth_count", 0),
+                   ("ori_hist_smooth_count", 5), ("desc_int_factor", 1), ("desc_int_factor", 100),
+                   ("desc_int_factor", 4096), ("all", 0)]
+ALL_CHANGED = dict(gauss_sigma=1.6, num_scale=9, num_octave=5, pre_color_thres=0.01, judge_extrema_diff_thres=1e-3,
+                   calc_offset_depth=8, offset_thres=0.3, ori_hist_smooth_count=0, desc_int_factor=100)
+
+
+def sift_set_input(field, value):
+    """(image, params) of one set.  NUM_SCALE 4 and 5 leave one and two admissible refined scale indices
+    (1 <= s <= nscale - 3): on the canvas the pre-colour and contrast thresholds remove every candidate,
+    so these two sets run on a uniform-noise image with both thresholds at 0."""
+    if field == "num_scale" and value <= 5:
+        img = np.random.RandomState(31).rand(180, 260, 3).astype(np.float32)
+        return img, default_params(num_scale=value, pre_color_thres=0.0, contrast_thres=0.0)
+    return synth.make_canvas(180, 260, 31), default_params(**(ALL_CHANGED if field == "all" else {field: value}))
+
+
+def min_points(field, value):
+    """(extremum candidates, descriptors) each set keeps at least on its input (the canvas keeps 171
+    descriptors at the defaults)."""
+    if field == "num_scale" and value <= 5:
+        return 100, 30
+    if field == "judge_extrema_diff_thres" and value > 2e-3:
+        return 1, 1
+    return 100, 100
+
+
+def case_sift_param_set(chk, field, value):
+    img, p = sift_set_input(field, value)
+    return _trace_outputs(chk.sift_trace(img, p), noct=p.num_octave, nscale=p.num_scale)
+
+
+WIDE_WINDOWS = [(8, 4.5), (17, 9.0), (20, 4.5)]
 
 
 def case_sift_wide_windows(chk, hist_scale, ori_radius):
@@ -153,13 +188,15 @@ def case_imgio_crop(chk):
     return out
 
 
-MATCH_RATIOS = [(0.6, 1, 60), (0.95, 150, 190)]
+MATCH_RATIOS = [(0.6, 1, 60), (0.95, 150, 190), (0.5, 60, 150), (1.0, 189, 190)]
+RATIO_NOISE = {0.5: 20.0}        # at noise 30 ratio 0.5 accepts nothing
 
 
-def case_match_other_ratios(chk, ratio):
+def case_match_other_ratios(chk, ratio, noise=None):
+    noise = RATIO_NOISE.get(ratio, 30.0) if noise is None else noise
     rng = np.random.RandomState(21)
     a = synth.rootsift_like(220, 22)
-    b = (a[rng.permutation(220)][:190] + rng.randn(190, 128).astype(np.float32) * 30).astype(np.float32)
+    b = (a[rng.permutation(220)][:190] + rng.randn(190, 128).astype(np.float32) * np.float32(noise)).astype(np.float32)
     p = default_params(match_reject_next_ratio=ratio)
     return [chk.match(a, b, p), chk.match(b, a, p)]
 
@@ -173,6 +210,13 @@ def case_blend_scaled_resolution(chk, lazy, ordered):
     assert geom["res_x"] > 2.0
     p = default_params(lazy_read=lazy, ordered_input=ordered)
     return [chk.blend(imgs, items, geom, 0, p), chk.blend(imgs, items, geom, 3, p)]
+
+
+def case_blend_window_factor(chk, factor):
+    """GAUSS_WINDOW_FACTOR in the multiband blender: its taps and the halo of every band."""
+    imgs, org = synth.make_stack(3, 160, 110, 60, 71)
+    items, geom = synth.translation_blend_setup(org, 160, 110)
+    return [chk.blend(imgs, items, geom, 3, default_params(multiband=3, gauss_window_factor=factor))]
 
 
 def case_cyl_warp_other_focal(chk):
@@ -210,6 +254,8 @@ def golden_cases():
               ("test_imgio_crop", case_imgio_crop, ()),
               ("test_cyl_warp_other_focal", case_cyl_warp_other_focal, ())]
     cases += [(case_key("test_sift_wide_windows", *a), case_sift_wide_windows, a) for a in WIDE_WINDOWS]
+    cases += [(case_key("test_sift_param_set", *a), case_sift_param_set, a) for a in SIFT_PARAM_SETS]
+    cases += [(case_key("test_blend_window_factor", f), case_blend_window_factor, (f,)) for f in (4,)]
     cases += [(case_key("test_cyl_warp", *a), case_cyl_warp, a) for a in CYL_WARPS]
     cases += [(case_key("test_blend_projections", p, b), case_blend_projections, (p, b)) for p in (0, 1, 2) for b in (0, 2)]
     cases += [(case_key("test_blend_scaled_resolution", *a), case_blend_scaled_resolution, a) for a in SCALED_BLENDS]
@@ -227,6 +273,23 @@ def test_sift_every_stage(orc, w, h, seed):
 
 def test_sift_other_params(orc):
     check("test_sift_other_params", case_sift_other_params(orc))
+
+
+@pytest.mark.parametrize("field,value", SIFT_PARAM_SETS)
+def test_sift_param_set(orc, field, value):
+    """Every stage at one config value off its default; the result must differ from the defaults' on the
+    same image, or the case would pin nothing.  (CALC_OFFSET_DEPTH alone leaves these images' features
+    unchanged: it is part of the "all" set.)"""
+    out = case_sift_param_set(orc, field, value)
+    img, p = sift_set_input(field, value)
+    base = _trace_outputs(orc.sift_trace(img))
+    assert not (np.array_equal(out[-2], base[-2]) and np.array_equal(out[-1], base[-1]))
+    tr = orc.sift_trace(img, p)
+    n_cand = len(tr.points(0))
+    tr.close()
+    min_cand, min_desc = min_points(field, value)
+    assert n_cand >= min_cand and len(out[-1]) >= min_desc, (n_cand, len(out[-1]))
+    check(case_key("test_sift_param_set", field, value), out)
 
 
 @pytest.mark.parametrize("hist_scale,ori_radius", WIDE_WINDOWS)
@@ -278,6 +341,7 @@ def test_match_other_ratios(orc, ratio, lo, hi):
     """MATCH_REJECT_NEXT_RATIO is a config value (config.cfg:33); the restatement takes it per call."""
     out = case_match_other_ratios(orc, ratio)
     assert lo <= len(out[0]) <= hi
+    assert not np.array_equal(out[0], case_match_other_ratios(orc, 0.8, RATIO_NOISE.get(ratio, 30.0))[0])
     check(case_key("test_match_other_ratios", ratio), out)
 
 
@@ -288,6 +352,12 @@ def test_blend_scaled_resolution(orc, lazy, ordered):
     out = case_blend_scaled_resolution(orc, lazy, ordered)
     assert (out[0] >= 0).mean() > 0.5
     check(case_key("test_blend_scaled_resolution", lazy, ordered), out)
+
+
+def test_blend_window_factor(orc):
+    out = case_blend_window_factor(orc, 4)
+    assert not gu.same_bits(out[0], case_blend_window_factor(orc, 6)[0])
+    check(case_key("test_blend_window_factor", 4), out)
 
 
 def test_cyl_warp_other_focal(orc):
