@@ -354,6 +354,14 @@ typedef struct pano_cyl_job {
   int n_kpts;
 } pano_cyl_job;
 int pano_cyl_warp_batch_dev(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double h_factor, const pano_params* p);
+/* pano_cyl_warp_batch_dev from device 8-bit sources: d_pix[k] is h×w×channels[k] interleaved u8 (channels 1
+ * or 3), jobs[k].d_rgb_hwc is ignored and may be NULL.  The warped images equal pano_cyl_warp_batch_dev's on
+ * pano_rgb8_to_mat32f_dev's images of the same pixels, bit for bit: every tap is converted as read_img
+ * converts it (a grey value is replicated to r, g, b without the division), and no f32 copy of a source is
+ * made.  Keypoints are rewritten as pano_cyl_warp_batch_dev rewrites them.  Null pointers, other channel
+ * counts, an image under 2×2 or an output size other than pano_cyl_warp_shape's return PANO_ERR_INVALID. */
+int pano_cyl_warp_batch_rgb8_dev(pano_ctx* ctx, int n, const pano_cyl_job* jobs, const unsigned char* const* d_pix,
+                                 const int* channels, double h_factor, const pano_params* p);
 
 /* ----------------------------------------------------------------- blend
  * Replaces BlenderBase::add_image + run (stitch/blender.hh:14-59) for
@@ -404,6 +412,14 @@ int pano_blend_rgb8_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
 int pano_blend_rows_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g,
                         int bands, const pano_params* p, float* d_out_rows, int out_w, int out_h,
                         int row0, int row1);
+/* The same strip from device 8-bit sources (d_pix / channels as for pano_blend_rgb8_dev): concatenated
+ * strips are pano_blend_rgb8_dev's mosaic, bit for bit, linear and multiband.  Only the images that reach
+ * the strip are read — for bands > 0 those whose ROI, clipped to [row0 - H, row1 + H), meets the canvas,
+ * for bands == 0 those whose ROI meets the strip — so a row-sharded caller needs in device memory only the
+ * sources of its strip; the pointers of the others are never dereferenced but must still be non-null. */
+int pano_blend_rows_rgb8_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const unsigned char* const* d_pix,
+                             const int* channels, const pano_blend_geom* g, int bands, const pano_params* p,
+                             float* d_out_rows, int out_w, int out_h, int row0, int row1);
 
 /* A blend whose sources arrive in windows: LAZY_READ's memory contract (config.cfg:10-11,
  * blender.cc:38-64, multiband.cc:27,49) on the device.  The mosaic is bit-identical to pano_blend's

@@ -89,6 +89,8 @@ def _load():
         "pano_cyl_warp": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, C.c_double, P, _fp, C.c_int,
                                     C.c_int, _dp, C.c_int]),
         "pano_cyl_warp_batch_dev": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoCylJob), C.c_double, P]),
+        "pano_cyl_warp_batch_rgb8_dev": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoCylJob), _vpp, _ip, C.c_double,
+                                                   P]),
         "pano_blend_target_size": (C.c_int, [C.c_int, C.POINTER(PanoBlendImage), _ip, _ip]),
         "pano_blend": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom),
                                  C.c_int, P, _fp, C.c_int, C.c_int]),
@@ -98,6 +100,9 @@ def _load():
                                           C.POINTER(PanoBlendGeom), C.c_int, P, C.c_void_p, C.c_int, C.c_int]),
         "pano_blend_rows_dev": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom),
                                           C.c_int, P, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),
+        "pano_blend_rows_rgb8_dev": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), _vpp, _ip,
+                                               C.POINTER(PanoBlendGeom), C.c_int, P, C.c_void_p, C.c_int, C.c_int,
+                                               C.c_int, C.c_int]),
         "pano_blend_stream_create": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom),
                                                C.c_int, P, C.c_int, C.c_int, _vpp]),
         "pano_blend_stream_add": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _vpp, C.c_int, C.c_int]),
@@ -602,6 +607,18 @@ class Engine:
         self._check(LIB.pano_blend_rows_dev(self._h, len(ptrs), arr, C.byref(g), bands, C.byref(params),
                                             C.c_void_p(d_out_rows), out_w, out_h, row0, row1))
 
+    def blend_rows_rgb8_dev(self, d_pix, channels, shapes, items, geom, d_out_rows, out_w, out_h, row0, row1, bands=0,
+                            params=None):
+        """blend_rows_dev from device h×w×channels u8 sources (channels 1 or 3 per image): rows [row0, row1) of
+        blend_rgb8_dev's mosaic.  Sources of images that do not reach the strip are never read."""
+        params = params or default_params()
+        n = len(d_pix)
+        arr, g = self._blend_args([None] * n, shapes, items, geom)
+        src = (C.c_void_p * max(n, 1))(*d_pix)
+        ch = (C.c_int * max(n, 1))(*channels)
+        self._check(LIB.pano_blend_rows_rgb8_dev(self._h, n, arr, src, ch, C.byref(g), bands, C.byref(params),
+                                                 C.c_void_p(d_out_rows), out_w, out_h, row0, row1))
+
     # -- matching
     def match_pairs(self, fs: FeatureSet, pairs, params=None, shard=(0, 1)):
         """shard=(s, S): decide only share s of S of every pair's smaller set (row-sharded multi-GPU
@@ -714,10 +731,7 @@ class Engine:
                                       _f(out), ow, oh, _d(k), len(k)))
         return out, k
 
-    def cyl_warp_batch_dev(self, src_ptrs, shapes, dst_ptrs, kpts=None, h_factor=1.0, params=None):
-        """Device pointers in, device pointers out (out sizes from cyl_warp_shape), asynchronous; kpts: optional
-        list of [n, 2] float64 arrays rewritten in place."""
-        params = params or default_params()
+    def _cyl_jobs(self, src_ptrs, shapes, dst_ptrs, kpts, h_factor, params):
         n = len(src_ptrs)
         arr = (PanoCylJob * max(n, 1))()
         for k in range(n):
@@ -728,7 +742,24 @@ class Engine:
             if kpts is not None and kpts[k] is not None and len(kpts[k]):
                 assert kpts[k].dtype == np.float64 and kpts[k].flags["C_CONTIGUOUS"]
                 arr[k].kpts_xy, arr[k].n_kpts = kpts[k].ctypes.data, len(kpts[k])
-        self._check(LIB.pano_cyl_warp_batch_dev(self._h, n, arr, h_factor, C.byref(params)))
+        return arr
+
+    def cyl_warp_batch_dev(self, src_ptrs, shapes, dst_ptrs, kpts=None, h_factor=1.0, params=None):
+        """Device pointers in, device pointers out (out sizes from cyl_warp_shape), asynchronous; kpts: optional
+        list of [n, 2] float64 arrays rewritten in place."""
+        params = params or default_params()
+        arr = self._cyl_jobs(src_ptrs, shapes, dst_ptrs, kpts, h_factor, params)
+        self._check(LIB.pano_cyl_warp_batch_dev(self._h, len(src_ptrs), arr, h_factor, C.byref(params)))
+
+    def cyl_warp_batch_rgb8_dev(self, src_ptrs, channels, shapes, dst_ptrs, kpts=None, h_factor=1.0, params=None):
+        """cyl_warp_batch_dev from device h×w×channels u8 sources (channels 1 or 3 per image): the warp of
+        cyl_warp_batch_dev on read_img's f32 images of the same pixels."""
+        params = params or default_params()
+        n = len(src_ptrs)
+        arr = self._cyl_jobs([None] * n, shapes, dst_ptrs, kpts, h_factor, params)
+        src = (C.c_void_p * max(n, 1))(*src_ptrs)
+        ch = (C.c_int * max(n, 1))(*channels)
+        self._check(LIB.pano_cyl_warp_batch_rgb8_dev(self._h, n, arr, src, ch, h_factor, C.byref(params)))
 
     # -- blend
     @staticmethod

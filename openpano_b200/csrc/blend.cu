@@ -694,7 +694,8 @@ static int blend_run(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands,
   return mb_levels(ctx, job, d, bands, d_out, row0, row1);
 }
 
-// pix / channels: 8-bit device sources (pano_blend_rgb8_dev), else null and imgs[k].rgb_hwc are the sources
+// pix / channels: 8-bit device sources (pano_blend_rgb8_dev, pano_blend_rows_rgb8_dev), else null and
+// imgs[k].rgb_hwc are the sources
 static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
                         const pano_params* p, float* d_out, int ow, int oh, int row0, int row1,
                         const unsigned char* const* pix = nullptr, const int* channels = nullptr) {
@@ -888,6 +889,15 @@ int pano_blend_rows_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
                         const pano_params* p, float* d_out_rows, int ow, int oh, int row0, int row1) {
   ctx_enter(ctx);
   return blend_device(ctx, n, imgs, g, bands, p, d_out_rows, ow, oh, row0, row1);
+}
+
+int pano_blend_rows_rgb8_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs, const unsigned char* const* d_pix,
+                             const int* channels, const pano_blend_geom* g, int bands, const pano_params* p,
+                             float* d_out_rows, int ow, int oh, int row0, int row1) {
+  ctx_enter(ctx);
+  if (!ctx) return PANO_ERR_INVALID;
+  if (!d_pix || !channels) return ctx_fail(ctx, PANO_ERR_INVALID, "blend rows rgb8: null source list");
+  return blend_device(ctx, n, imgs, g, bands, p, d_out_rows, ow, oh, row0, row1, d_pix, channels);
 }
 
 int pano_blend_stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,

@@ -10,7 +10,9 @@
 #include "common.cuh"
 #include <math.h>
 #include <float.h>
+#include <string.h>
 #include <vector>
+#include <algorithm>
 
 struct CylProj { double cx, cy; int r; int sizefactor; };
 
@@ -98,15 +100,34 @@ __global__ void k_cyl_warp(const float* __restrict__ src, int w, int h, float* _
 }
 
 // The same for a batch of device-resident images: blockIdx.z = image; per-image parameters and the
-// two per-column tables (concatenated) sit in device memory.
+// two per-column tables (concatenated) sit in device memory.  Src = SrcF32 reads h×w×3 f32 images,
+// Src = SrcRgb8 reads h×w×channels u8 pixels and converts every tap as read_img converts it, so the
+// warp of the pixels is the warp of read_img's f32 image, bit for bit.
 struct CylJobDev {
-  const float* src; float* dst;
+  union {
+    const float* src;           // SrcF32
+    const unsigned char* pix;   // SrcRgb8
+  };
+  float* dst;
   int w, h, ow, oh;
-  long long tab_off;           // first entry of this image's col_x[ow] followed by col_cos[ow]
+  int channels;                 // SrcRgb8 only: 1 or 3
+  long long tab_off;            // first entry of this image's col_x[ow] followed by col_cos[ow]
   double r, cy, offy, sizefactor_inv;
 };
 
+template <class Src> __device__ __forceinline__ Src cyl_src(const CylJobDev& jb, const float* lut);
+template <> __device__ __forceinline__ SrcF32 cyl_src<SrcF32>(const CylJobDev& jb, const float*) { return SrcF32{jb.src}; }
+template <> __device__ __forceinline__ SrcRgb8 cyl_src<SrcRgb8>(const CylJobDev& jb, const float* lut) {
+  return SrcRgb8{jb.pix, lut, jb.channels};
+}
+
+template <class Src>
 __global__ void k_cyl_warp_batch(const CylJobDev* __restrict__ jobs, const double* __restrict__ tabs) {
+  __shared__ float lut[Src::kLut ? 256 : 1];
+  if constexpr (Src::kLut) {      // every thread of the 256 takes part, before any leaves at the edge below
+    build_rgb8_lut(lut, threadIdx.y * blockDim.x + threadIdx.x);
+    __syncthreads();
+  }
   const CylJobDev jb = jobs[blockIdx.z];
   int j = blockIdx.x * blockDim.x + threadIdx.x;
   int i = blockIdx.y * blockDim.y + threadIdx.y;
@@ -119,16 +140,17 @@ __global__ void k_cyl_warp_batch(const CylJobDev* __restrict__ jobs, const doubl
   float o0 = -1.f, o1 = -1.f, o2 = -1.f;
   if (x >= 0 && x <= (double)(jb.w - 1) && y >= 0 && y <= (double)(jb.h - 1)) {
     float c0, c1, c2;
-    if (interpolate_rgb(jb.src, jb.w, jb.h, (float)y, (float)x, &c0, &c1, &c2)) { o0 = c0; o1 = c1; o2 = c2; }
+    if (interpolate_rgb(cyl_src<Src>(jb, lut), jb.w, jb.h, (float)y, (float)x, &c0, &c1, &c2)) { o0 = c0; o1 = c1; o2 = c2; }
   }
   float* p = jb.dst + ((size_t)i * jb.ow + j) * 3;
   p[0] = o0; p[1] = o1; p[2] = o2;
 }
 
-extern "C" {
-
-int pano_cyl_warp_batch_dev(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double h_factor, const pano_params* p) {
-  ctx_enter(ctx);
+// Both batch entry points.  pix / channels: 8-bit device sources (jobs[k].d_rgb_hwc ignored), else null
+// and jobs[k].d_rgb_hwc are the sources.  The keypoints and the per-column tables are host arithmetic on
+// the shapes alone, the same for both.
+static int cyl_warp_batch(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double h_factor, const pano_params* p,
+                          const unsigned char* const* pix = nullptr, const int* channels = nullptr) {
   if (!ctx || n < 0 || (n && !jobs) || !p) return PANO_ERR_INVALID;
   if (n == 0) return PANO_OK;
   std::vector<CylJobDev> dj(n);
@@ -136,8 +158,11 @@ int pano_cyl_warp_batch_dev(pano_ctx* ctx, int n, const pano_cyl_job* jobs, doub
   int max_ow = 0, max_oh = 0;
   for (int k = 0; k < n; ++k) {
     const pano_cyl_job& jb = jobs[k];
-    if (!jb.d_rgb_hwc || !jb.d_out_hwc || jb.w <= 1 || jb.h <= 1 || jb.n_kpts < 0 || (jb.n_kpts && !jb.kpts_xy))
+    if ((!pix && !jb.d_rgb_hwc) || !jb.d_out_hwc || jb.w <= 1 || jb.h <= 1 || jb.n_kpts < 0 || (jb.n_kpts && !jb.kpts_xy))
       return ctx_fail(ctx, PANO_ERR_INVALID, "cyl_warp_batch: job %d has a null pointer or an empty image", k);
+    if (pix && (!pix[k] || (channels[k] != 1 && channels[k] != 3)))
+      return ctx_fail(ctx, PANO_ERR_INVALID, "cyl_warp_batch rgb8: job %d has no pixels or %d channels (1 or 3)", k,
+                      channels[k]);
     CylProj c = get_projector(jb.w, jb.h, h_factor, p);
     if (c.r <= 0) return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder radius <= 0");
     int sw = jb.w, sh = jb.h;
@@ -154,7 +179,14 @@ int pano_cyl_warp_batch_dev(pano_ctx* ctx, int n, const pano_cyl_job* jobs, doub
       tabs[t0 + j] = c.r * tan(px) + c.cx;
       tabs[t0 + sw + j] = cos(px);
     }
-    dj[k] = CylJobDev{jb.d_rgb_hwc, jb.d_out_hwc, jb.w, jb.h, sw, sh, (long long)t0, (double)c.r, c.cy, offy, sizefactor_inv};
+    CylJobDev& d = dj[k];
+    memset(&d, 0, sizeof(d));
+    if (pix) { d.pix = pix[k]; d.channels = channels[k]; }
+    else { d.src = jb.d_rgb_hwc; d.channels = 3; }
+    d.dst = jb.d_out_hwc;
+    d.w = jb.w; d.h = jb.h; d.ow = sw; d.oh = sh;
+    d.tab_off = (long long)t0;
+    d.r = (double)c.r; d.cy = c.cy; d.offy = offy; d.sizefactor_inv = sizefactor_inv;
     max_ow = std::max(max_ow, sw); max_oh = std::max(max_oh, sh);
   }
   CylJobDev* d_jobs = nullptr;
@@ -168,16 +200,33 @@ int pano_cyl_warp_batch_dev(pano_ctx* ctx, int n, const pano_cyl_job* jobs, doub
   rc = ctx_put(ctx, d_jobs, dj.data(), dj.size() * sizeof(CylJobDev));
   if (!rc) rc = ctx_put(ctx, d_tabs, tabs.data(), tabs.size() * sizeof(double));
   if (!rc) {
-    dim3 b(32, 8), g(ceil_div(max_ow, 32), ceil_div(max_oh, 8), n);
+    dim3 b(32, 8), g(ceil_div(max_ow, 32), ceil_div(max_oh, 8), n);   // 256 threads: the 8-bit conversion table
+    const char* name = pix ? "k_cyl_warp_rgb8" : "k_cyl_warp";
     ctx->launches++;
-    if (ctx->profiling) ctx_prof_begin(ctx, "k_cyl_warp");
-    k_cyl_warp_batch<<<g, b, 0, ctx->stream>>>(d_jobs, d_tabs);
+    if (ctx->profiling) ctx_prof_begin(ctx, name);
+    if (pix) k_cyl_warp_batch<SrcRgb8><<<g, b, 0, ctx->stream>>>(d_jobs, d_tabs);
+    else k_cyl_warp_batch<SrcF32><<<g, b, 0, ctx->stream>>>(d_jobs, d_tabs);
     if (ctx->profiling) ctx_prof_end(ctx);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) rc = ctx_cuda(ctx, e, "k_cyl_warp_batch");
+    if (e != cudaSuccess) rc = ctx_cuda(ctx, e, name);
   }
   ctx_free(ctx, d_jobs); ctx_free(ctx, d_tabs);      // stream-ordered: released after the kernel
   return rc;
+}
+
+extern "C" {
+
+int pano_cyl_warp_batch_dev(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double h_factor, const pano_params* p) {
+  ctx_enter(ctx);
+  return cyl_warp_batch(ctx, n, jobs, h_factor, p);
+}
+
+int pano_cyl_warp_batch_rgb8_dev(pano_ctx* ctx, int n, const pano_cyl_job* jobs, const unsigned char* const* d_pix,
+                                 const int* channels, double h_factor, const pano_params* p) {
+  ctx_enter(ctx);
+  if (!ctx) return PANO_ERR_INVALID;
+  if (n > 0 && (!d_pix || !channels)) return ctx_fail(ctx, PANO_ERR_INVALID, "cyl_warp_batch rgb8: null source list");
+  return cyl_warp_batch(ctx, n, jobs, h_factor, p, d_pix, channels);
 }
 
 int pano_cyl_warp_shape(int w, int h, double h_factor, const pano_params* p, int* ow, int* oh, double* offx,

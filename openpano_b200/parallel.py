@@ -190,25 +190,35 @@ class DistributedStitcher:
     rank, `torch.distributed` initialised with the NCCL backend, the Engine created
     on torch's CURRENT non-default stream so engine kernels and NCCL order on it).
 
-      SIFT      owned images (k mod G)                              no collective
+      SIFT      owned images (k mod G), read as they were passed: f32 (run) or
+                8-bit pixels (run_rgb8)                             no collective
       C1        descriptors + coordinates: export_dev -> ncclAllGather -> import_dev
+                (run_rgb8: each image's channel count travels with its count)
       match     the dealt pair tasks against the gathered featureset  no collective
       results   match lists -> every rank (one padded int32 all-gather, a few KB)
-      images    every rank blends a strip of every image: ncclAllGather of the 8-bit
-                sources (3 B/px; run_rgb8) or of the f32 images (run), issued on a side
-                stream BEFORE SIFT so that it overlaps SIFT + C1 + matching
+      images    every rank blends a strip of every image: ncclAllGather of the sources
+                into slots of the largest H×W×3, issued on a side stream BEFORE SIFT
+                so that it overlaps SIFT + C1 + matching.  run moves and holds 12 B/px
+                of f32; run_rgb8 moves and holds 3 B/px of 8-bit pixels (a grey image
+                fills a third of its slot) and makes no f32 copy of any source
       blend     rows [r·H/G, (r+1)·H/G) of the canvas (LinearBlender pixels are
                 independent, blender.cc:37-96; MultiBandBlender strips are computed
-                from ROIs clipped to the strip + the summed blur half-widths)   no collective
+                from ROIs clipped to the strip + the summed blur half-widths), read
+                from the gathered sources as they are (pano_blend_rows_dev /
+                pano_blend_rows_rgb8_dev)                           no collective
       C2        strips -> ncclAllGather -> the mosaic (bit-identical to one GPU)
+
+    blend_params: the composite's parameters where they differ from detection and matching's (e.g. a
+    GAUSS_WINDOW_FACTOR wider than the SIFT blur's 31 taps allow); defaults to params.
     """
 
     PHASES = ("sift", "exchange_descriptors", "match", "gather_matches", "exchange_images", "blend_strip", "gather_strips")
 
-    def __init__(self, engine, params=None):
+    def __init__(self, engine, params=None, blend_params=None):
         from ._abi import default_params
         self.eng = engine
         self.params = params or default_params()
+        self.blend_params = blend_params or self.params
         self.ms = {}
         self.host_ms = {}         # host wall time spent inside each phase's calls (launch / sync overhead)
         self._side = None
@@ -242,8 +252,9 @@ class DistributedStitcher:
 
     def run_rgb8(self, owned_pix: dict, n_images: int, shapes, pairs, items, geom, bands: int = 0):
         """The same from decoded 8-bit pixels (what read_img starts from, imgio.cc:72): owned_pix =
-        {image index: cuda uint8 tensor H×W×3}.  The u8 -> f32 conversion (read_img's arithmetic)
-        runs on the device, and the image exchange moves 3 B/px instead of 12."""
+        {image index: contiguous cuda uint8 tensor H×W (grey) or H×W×3}.  SIFT and the strip read the
+        pixels themselves and convert every tap as read_img would (bit-identical to run on read_img's
+        f32 images); the image exchange moves 3 B/px instead of 12, and no f32 copy of a source is made."""
         return self._run(None, owned_pix, n_images, shapes, pairs, items, geom, bands)
 
     def _run(self, owned, owned_pix, n_images, shapes, pairs, items, geom, bands):
@@ -256,6 +267,15 @@ class DistributedStitcher:
         mine = owners[rank]
         rgb8 = owned_pix is not None
         assert sorted(owned_pix if rgb8 else owned) == mine, "images must follow shard_images()"
+        own_ch = {}
+        if rgb8:
+            for k in mine:
+                x = owned_pix[k]
+                if (x.dtype != torch.uint8 or not x.is_contiguous() or tuple(x.shape[:2]) != tuple(shapes[k])
+                        or not (x.dim() == 2 or (x.dim() == 3 and x.shape[2] in (1, 3)))):
+                    raise ValueError(f"run_rgb8: image {k} must be a contiguous H×W or H×W×{{1,3}} uint8 tensor of "
+                                     f"shape {tuple(shapes[k])}, got {x.dtype} {tuple(x.shape)}")
+                own_ch[k] = 1 if x.dim() == 2 else int(x.shape[2])
         self._events = []
         self.host_ms = {}
         main = torch.cuda.current_stream()
@@ -282,30 +302,28 @@ class DistributedStitcher:
             ev_i1.record()
         self._events.append(("exchange_images", ev_i0, ev_i1))
 
-        # ---- SIFT on the owned images
-        own_f32 = owned
-        if rgb8 and mine:
-            own_f32 = {k: torch.empty(tuple(shapes[k]) + (3,), dtype=torch.float32, device=dev) for k in mine}
-
+        # ---- SIFT on the owned images (8-bit: the caller's tensors are read until exchange() queries the counts)
         def sift():
             if not mine:
                 return None
+            ws, hs = [shapes[k][1] for k in mine], [shapes[k][0] for k in mine]
             if rgb8:
-                eng.rgb8_to_mat32f_batch_dev([owned_pix[k].data_ptr() for k in mine], [shapes[k][1] for k in mine],
-                                             [shapes[k][0] for k in mine], [3] * len(mine),
-                                             [own_f32[k].data_ptr() for k in mine])
-            return eng.sift_detect_batch_ptr([own_f32[k].data_ptr() for k in mine], [shapes[k][1] for k in mine],
-                                             [shapes[k][0] for k in mine], params, device=True)
+                return eng.sift_detect_batch_rgb8_ptr([owned_pix[k].data_ptr() for k in mine], ws, hs,
+                                                      [own_ch[k] for k in mine], params, device=True)
+            return eng.sift_detect_batch_ptr([owned[k].data_ptr() for k in mine], ws, hs, params, device=True)
         fs_local = self._timed("sift", sift)
 
-        # ---- C1: all-gather of the descriptor sets
+        # ---- C1: all-gather of the descriptor sets.  The counts' all-reduce also carries each image's channel
+        # count (run_rgb8), which every rank's strip needs and only the owner knows.
         def exchange():
-            arr = np.zeros(n_images, np.int64)
+            arr = np.zeros(2 * n_images, np.int64)
             for q, k in enumerate(mine):
                 arr[k] = fs_local.count(q)
+                arr[n_images + k] = own_ch.get(k, 3)
             counts_t = torch.from_numpy(arr).to(dev)
             dist.all_reduce(counts_t)
-            counts = [int(c) for c in counts_t.tolist()]
+            both = [int(c) for c in counts_t.tolist()]
+            counts, chans = both[:n_images], both[n_images:]
             rows = [sum(counts[k] for k in owners[r]) for r in range(world)]
             pad = max(max(rows), 1)
             my_d = torch.empty((pad, 128), dtype=torch.float32, device=dev)
@@ -324,8 +342,8 @@ class DistributedStitcher:
                     pc[k] = all_c.data_ptr() + (r * pad + off) * 16
                     off += counts[k]
             fs_all = eng.featureset_import_dev(counts, pd, pc)
-            return fs_all, counts, (all_d, all_c, my_d, my_c)
-        fs_all, counts, keep = self._timed("exchange_descriptors", exchange)
+            return fs_all, counts, chans, (all_d, all_c, my_d, my_c)
+        fs_all, counts, chans, keep = self._timed("exchange_descriptors", exchange)
         if fs_local is not None:
             fs_local.free()
 
@@ -378,32 +396,19 @@ class DistributedStitcher:
         rows_per = (th + world - 1) // world
         row0, row1 = min(th, rank * rows_per), min(th, (rank + 1) * rows_per)
         strip = torch.empty((rows_per, tw, 3), dtype=torch.float32, device=dev)
-        keep_f = None
+        bparams = self.blend_params
 
         def blend_strip():
-            nonlocal keep_f
             el = 1 if rgb8 else 4
             src_ptrs = [0] * n_images
             for r in range(world):
                 for q, k in enumerate(owners[r]):
                     src_ptrs[k] = all_i.data_ptr() + (r * per_rank + q) * max_el * el
             if rgb8:
-                # read_img's conversion of the gathered 8-bit sources (only images that reach this strip)
-                need = [k for k in range(n_images) if items[k][1] <= row1 + 256 and items[k][3] >= row0 - 256]   # strip + multiband halo
-                keep_f = torch.empty((max(len(need), 1), max_el), dtype=torch.float32, device=dev)
-                img_ptrs = list(src_ptrs)
-                if need:
-                    dst = [keep_f.data_ptr() + q * max_el * 4 for q in range(len(need))]
-                    eng.rgb8_to_mat32f_batch_dev([src_ptrs[k] for k in need], [shapes[k][1] for k in need],
-                                                 [shapes[k][0] for k in need], [3] * len(need), dst)
-                    for q, k in enumerate(need):
-                        img_ptrs[k] = dst[q]
-                # images that cannot reach the strip are never dereferenced: any valid pointer will do
-                spare, needed = keep_f.data_ptr(), set(need)
-                img_ptrs = [p if k in needed else spare for k, p in enumerate(img_ptrs)]
+                eng.blend_rows_rgb8_dev(src_ptrs, chans, shapes, items, geom, strip.data_ptr(), tw, th, row0, row1,
+                                        bands, bparams)
             else:
-                img_ptrs = src_ptrs
-            eng.blend_rows_dev(img_ptrs, shapes, items, geom, strip.data_ptr(), tw, th, row0, row1, bands, params)
+                eng.blend_rows_dev(src_ptrs, shapes, items, geom, strip.data_ptr(), tw, th, row0, row1, bands, bparams)
         self._timed("blend_strip", blend_strip)
         mosaic = torch.empty((world * rows_per, tw, 3), dtype=torch.float32, device=dev)
         self._timed("gather_strips", lambda: dist.all_gather_into_tensor(mosaic, strip))
@@ -416,5 +421,5 @@ class DistributedStitcher:
         for name, e0, e1 in self._events:
             self.ms[name] = self.ms.get(name, 0.0) + e0.elapsed_time(e1)
         fs_all.free()
-        del keep, my_i, all_i, keep_f
+        del keep, my_i, all_i
         return matches, mosaic[:th]
