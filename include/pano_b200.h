@@ -39,6 +39,14 @@ typedef enum pano_status {
   PANO_ERR_NO_FEATURE = -5   /* reference: error_exit("Cannot find feature…"), stitcherbase.cc:20 */
 } pano_status;
 
+/* Limits.  Pair lists have none: matching, RANSAC scoring and bundle adjustment accept any number of
+ * pairs.  Image counts are bounded: a featureset, a cylinder-warp or 8-bit conversion batch and a blend
+ * take at most PANO_MAX_IMAGES images, a bundle adjustment at most PANO_MAX_IMAGES cameras, and a SIFT
+ * batch at most PANO_MAX_SIFT_BATCH images (split larger batches).  Larger calls return
+ * PANO_ERR_INVALID and leave the context usable. */
+#define PANO_MAX_IMAGES 65535
+#define PANO_MAX_SIFT_BATCH 512
+
 /* Snapshot of the reference's mutable config globals (lib/config.hh:24-68,
  * defaults from config.cfg:2-69) that the hot path reads. */
 typedef struct pano_params {

@@ -46,36 +46,40 @@ __constant__ double c_dKd[3][9] = {{1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0}
 // 3..5 fromK*dRfromdvi[k]; 6 toKinv; 7..9 m*dKd{focal,ppx,ppy}, m = fromK*R_from*toRinv*toKinv;
 // 10..12 (fromK*R_from)*dRtodviT[k]
 __global__ void __launch_bounds__(128)
-k_ba_rows(const BaPairDev* __restrict__ pairs, const double2* __restrict__ pts_to, double* __restrict__ rows) {
+k_ba_rows(const BaPairDev* __restrict__ pairs, int n_pair, const double2* __restrict__ pts_to, double* __restrict__ rows) {
   __shared__ double s_m[13][9];
-  const BaPairDev& pr = pairs[blockIdx.y];
-  for (int q = threadIdx.x; q < 13 * 9; q += blockDim.x) s_m[q / 9][q % 9] = pr.m[q / 9][q % 9];
-  __syncthreads();
-  const int n = pr.n_match, begin = pr.match_begin;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double2 to = pts_to[begin + i];
-    const BaVec tov{to.x, to.y, 1.0};                    // trans(Vec2D) = trans(Vec(x, y, 1))
-    const BaVec homo = ba_trans(s_m[0], tov);
-    const float hzf = (float)homo.z;                     // sqr(float), lib/utils.hh:25
-    const double hz_sqr_inv = 1.0 / (double)(hzf * hzf);
-    const double hz_inv = 1.0 / homo.z;
-    double* out = rows + (size_t)(begin + i) * 24;       // row idx: dfrom.x[6], dto.x[6]; row idx+1: dfrom.y[6], dto.y[6]
-    auto drdv = [&](BaVec dhdv, int col) {
-      out[col] = -dhdv.x * hz_inv + dhdv.z * homo.x * hz_sqr_inv;
-      out[12 + col] = -dhdv.y * hz_inv + dhdv.z * homo.y * hz_sqr_inv;
-    };
-    BaVec dot_u2 = ba_trans(s_m[1], tov);
+  // pairs on gridDim.y (at most 65,535): the blocks of a y index take every gridDim.y-th pair
+  for (int p = blockIdx.y; p < n_pair; p += gridDim.y) {
+    const BaPairDev& pr = pairs[p];
+    __syncthreads();                                     // the previous pair's matrices are no longer read
+    for (int q = threadIdx.x; q < 13 * 9; q += blockDim.x) s_m[q / 9][q % 9] = pr.m[q / 9][q % 9];
+    __syncthreads();
+    const int n = pr.n_match, begin = pr.match_begin;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+      const double2 to = pts_to[begin + i];
+      const BaVec tov{to.x, to.y, 1.0};                    // trans(Vec2D) = trans(Vec(x, y, 1))
+      const BaVec homo = ba_trans(s_m[0], tov);
+      const float hzf = (float)homo.z;                     // sqr(float), lib/utils.hh:25
+      const double hz_sqr_inv = 1.0 / (double)(hzf * hzf);
+      const double hz_inv = 1.0 / homo.z;
+      double* out = rows + (size_t)(begin + i) * 24;       // row idx: dfrom.x[6], dto.x[6]; row idx+1: dfrom.y[6], dto.y[6]
+      auto drdv = [&](BaVec dhdv, int col) {
+        out[col] = -dhdv.x * hz_inv + dhdv.z * homo.x * hz_sqr_inv;
+        out[12 + col] = -dhdv.y * hz_inv + dhdv.z * homo.y * hz_sqr_inv;
+      };
+      BaVec dot_u2 = ba_trans(s_m[1], tov);
 #pragma unroll
-    for (int k = 0; k < 3; ++k) drdv(ba_trans(c_dKd[k], dot_u2), k);            // dfrom: focal, ppx, ppy
-    dot_u2 = ba_trans(s_m[2], tov);
+      for (int k = 0; k < 3; ++k) drdv(ba_trans(c_dKd[k], dot_u2), k);            // dfrom: focal, ppx, ppy
+      dot_u2 = ba_trans(s_m[2], tov);
 #pragma unroll
-    for (int k = 0; k < 3; ++k) drdv(ba_trans(s_m[3 + k], dot_u2), 3 + k);       // dfrom: rotation
-    const BaVec ku = ba_trans(s_m[6], tov);
-    dot_u2 = BaVec{ku.x * -1.0, ku.y * -1.0, ku.z * -1.0};                       // Vec::operator*(-1)
+      for (int k = 0; k < 3; ++k) drdv(ba_trans(s_m[3 + k], dot_u2), 3 + k);       // dfrom: rotation
+      const BaVec ku = ba_trans(s_m[6], tov);
+      dot_u2 = BaVec{ku.x * -1.0, ku.y * -1.0, ku.z * -1.0};                       // Vec::operator*(-1)
 #pragma unroll
-    for (int k = 0; k < 3; ++k) drdv(ba_trans(s_m[7 + k], dot_u2), 6 + k);       // dto: focal, ppx, ppy
+      for (int k = 0; k < 3; ++k) drdv(ba_trans(s_m[7 + k], dot_u2), 6 + k);       // dto: focal, ppx, ppy
 #pragma unroll
-    for (int k = 0; k < 3; ++k) drdv(ba_trans(s_m[10 + k], ku), 9 + k);          // dto: rotation
+      for (int k = 0; k < 3; ++k) drdv(ba_trans(s_m[10 + k], ku), 9 + k);          // dto: rotation
+    }
   }
 }
 
@@ -113,6 +117,8 @@ extern "C" int pano_ba_jacobian(pano_ctx* ctx, int n_cam, int n_pair, const pano
                                 double* j_rows, double* jtj) {
   ctx_enter(ctx);
   if (!ctx || n_cam <= 0 || n_pair < 0 || (n_pair && (!pairs || !pts_to)) || !jtj) return PANO_ERR_INVALID;
+  if (n_cam > PANO_MAX_IMAGES)   // J^T J blocks on (gridDim.x, gridDim.y)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "ba: %d cameras (limit %d)", n_cam, PANO_MAX_IMAGES);
   static_assert(sizeof(BaPairDev) == sizeof(pano_ba_pair), "pano_ba_pair layout");
   long long nm = 0;
   int max_match = 0;
@@ -145,8 +151,8 @@ extern "C" int pano_ba_jacobian(pano_ctx* ctx, int n_cam, int n_pair, const pano
     if (n_pair && max_match) {
       ctx->launches++;
       if (ctx->profiling) ctx_prof_begin(ctx, "k_ba_rows");
-      dim3 grid((unsigned)std::max(1, std::min((max_match + 127) / 128, 1024)), (unsigned)n_pair);
-      k_ba_rows<<<grid, 128, 0, ctx->stream>>>(d_pairs, d_pts, d_rows);
+      dim3 grid((unsigned)std::max(1, std::min((max_match + 127) / 128, 1024)), grid_y(n_pair));
+      k_ba_rows<<<grid, 128, 0, ctx->stream>>>(d_pairs, n_pair, d_pts, d_rows);
       if (ctx->profiling) ctx_prof_end(ctx);
     }
     ctx->launches++;
@@ -180,35 +186,38 @@ struct BaErrStats {
 // calcError's loop (:180-195): transformed = Hto_to_from.trans2d(to) (homography.hh:53-64), r = from - transformed;
 // also the FLOAT squares update_stats sums (error_func = sqr(diff), lib/utils.hh:25's float overload).
 __global__ void __launch_bounds__(128)
-k_ba_residuals(const BaPairDev* __restrict__ pairs, const double* __restrict__ hto, const double2* __restrict__ pts_to,
-               const double2* __restrict__ pts_from, double2* __restrict__ res, float2* __restrict__ sq,
+k_ba_residuals(const BaPairDev* __restrict__ pairs, int n_pair, const double* __restrict__ hto,
+               const double2* __restrict__ pts_to, const double2* __restrict__ pts_from, double2* __restrict__ res, float2* __restrict__ sq,
                BaErrStats* __restrict__ st, int* __restrict__ pair_nonfinite) {
   __shared__ double s_h[9];
-  const int p = blockIdx.y;
-  if (threadIdx.x < 9) s_h[threadIdx.x] = hto[(size_t)p * 9 + threadIdx.x];
-  __syncthreads();
-  const int n = pairs[p].n_match, begin = pairs[p].match_begin;
-  unsigned long long mx = 0ull;                           // update_max(max, fabs(e)) from max = 0
-  bool bad = false;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double2 to = pts_to[begin + i], fr = pts_from[begin + i];
-    const BaVec t = ba_trans(s_h, BaVec{to.x, to.y, 1.0});
-    const double denom = 1.0 / t.z;                       // trans_normalize
-    const double rx = fr.x - t.x * denom, ry = fr.y - t.y * denom;
-    res[begin + i] = make_double2(rx, ry);
-    const float fx = (float)rx, fy = (float)ry;
-    sq[begin + i] = make_float2(fx * fx, fy * fy);
-    bad |= !isfinite(rx) || !isfinite(ry);
-    const double ax = fabs(rx), ay = fabs(ry);            // dest < NaN is false: NaN never becomes the max
-    if (!isnan(ax)) mx = max(mx, (unsigned long long)__double_as_longlong(ax));
-    if (!isnan(ay)) mx = max(mx, (unsigned long long)__double_as_longlong(ay));
-  }
+  // pairs on gridDim.y (at most 65,535): the blocks of a y index take every gridDim.y-th pair
+  for (int p = blockIdx.y; p < n_pair; p += gridDim.y) {
+    __syncthreads();                                      // the previous pair's matrix is no longer read
+    if (threadIdx.x < 9) s_h[threadIdx.x] = hto[(size_t)p * 9 + threadIdx.x];
+    __syncthreads();
+    const int n = pairs[p].n_match, begin = pairs[p].match_begin;
+    unsigned long long mx = 0ull;                           // update_max(max, fabs(e)) from max = 0
+    bool bad = false;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+      const double2 to = pts_to[begin + i], fr = pts_from[begin + i];
+      const BaVec t = ba_trans(s_h, BaVec{to.x, to.y, 1.0});
+      const double denom = 1.0 / t.z;                       // trans_normalize
+      const double rx = fr.x - t.x * denom, ry = fr.y - t.y * denom;
+      res[begin + i] = make_double2(rx, ry);
+      const float fx = (float)rx, fy = (float)ry;
+      sq[begin + i] = make_float2(fx * fx, fy * fy);
+      bad |= !isfinite(rx) || !isfinite(ry);
+      const double ax = fabs(rx), ay = fabs(ry);            // dest < NaN is false: NaN never becomes the max
+      if (!isnan(ax)) mx = max(mx, (unsigned long long)__double_as_longlong(ax));
+      if (!isnan(ay)) mx = max(mx, (unsigned long long)__double_as_longlong(ay));
+    }
 #pragma unroll
-  for (int o = 16; o; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  bad = __any_sync(0xffffffffu, bad);
-  if ((threadIdx.x & 31) == 0) {
-    if (mx) atomicMax(&st->max_bits, mx);
-    if (bad) atomicOr(&pair_nonfinite[p], 1);
+    for (int o = 16; o; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    bad = __any_sync(0xffffffffu, bad);
+    if ((threadIdx.x & 31) == 0) {
+      if (mx) atomicMax(&st->max_bits, mx);
+      if (bad) atomicOr(&pair_nonfinite[p], 1);
+    }
   }
 }
 
@@ -321,6 +330,8 @@ extern "C" int pano_ba_session_create(pano_ctx* ctx, int n_cam, int n_pair, cons
   if (out) *out = nullptr;
   if (!ctx || !out || n_cam <= 0 || n_pair < 0 || (n_pair && !links)) return PANO_ERR_INVALID;
   ctx_enter(ctx);
+  if (n_cam > PANO_MAX_IMAGES)   // J^T J blocks on (gridDim.x, gridDim.y)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "ba session: %d cameras (limit %d)", n_cam, PANO_MAX_IMAGES);
   long long nm = 0;
   int max_match = 0;
   for (int k = 0; k < n_pair; ++k) {
@@ -416,8 +427,8 @@ extern "C" int pano_ba_error(pano_ba_session* s, int n_pair, const double* hto_t
     if (rc) return rc;
   }
   if (s->nm) {
-    dim3 grid((unsigned)std::max(1, std::min((s->max_match + 127) / 128, 1024)), (unsigned)n_pair);
-    PANO_LAUNCH(ctx, "k_ba_residuals", k_ba_residuals, grid, 128, 0, s->d_pairs, s->d_hto, s->d_to, s->d_from, s->d_res,
+    dim3 grid((unsigned)std::max(1, std::min((s->max_match + 127) / 128, 1024)), grid_y(n_pair));
+    PANO_LAUNCH(ctx, "k_ba_residuals", k_ba_residuals, grid, 128, 0, s->d_pairs, n_pair, s->d_hto, s->d_to, s->d_from, s->d_res,
                 s->d_sq, s->d_st, s->d_nonfinite);
   }
   PANO_LAUNCH(ctx, "k_ba_error_sum", k_ba_error_sum, 1, 1024, 0, (const float*)s->d_sq, 2 * s->nm, s->d_st, s->h_out);
@@ -449,8 +460,9 @@ extern "C" int pano_ba_normal_equations(pano_ba_session* s, int n_pair, const do
     if (rc) return rc;
   }
   if (n_pair && s->max_match) {
-    dim3 grid((unsigned)std::max(1, std::min((s->max_match + 127) / 128, 1024)), (unsigned)n_pair);
-    PANO_LAUNCH(ctx, "k_ba_rows", k_ba_rows, grid, 128, 0, (const BaPairDev*)s->d_pairs, (const double2*)s->d_to, s->d_rows);
+    dim3 grid((unsigned)std::max(1, std::min((s->max_match + 127) / 128, 1024)), grid_y(n_pair));
+    PANO_LAUNCH(ctx, "k_ba_rows", k_ba_rows, grid, 128, 0, (const BaPairDev*)s->d_pairs, n_pair, (const double2*)s->d_to,
+                s->d_rows);
   }
   PANO_LAUNCH(ctx, "k_ba_jtj", k_ba_jtj, dim3((unsigned)s->n_cam, (unsigned)s->n_cam), 64, 0, (const BaPairDev*)s->d_pairs,
               n_pair, s->n_cam, (const double*)s->d_rows, s->d_jtj);

@@ -700,6 +700,8 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
                         const pano_params* p, float* d_out, int ow, int oh, int row0, int row1,
                         const unsigned char* const* pix = nullptr, const int* channels = nullptr) {
   if (!ctx || n <= 0 || !imgs || !g || !p || !d_out || bands < 0) return PANO_ERR_INVALID;
+  if (n > PANO_MAX_IMAGES)   // images on gridDim.z of k_mb_first_level
+    return ctx_fail(ctx, PANO_ERR_INVALID, "blend: %d images (limit %d)", n, PANO_MAX_IMAGES);
   if (row0 < 0 || row1 > oh || row0 > row1)
     return ctx_fail(ctx, PANO_ERR_INVALID, "blend: rows [%d, %d) outside the %d-row canvas", row0, row1, oh);
   if (row0 == row1) return PANO_OK;
@@ -906,6 +908,8 @@ int pano_blend_stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs,
   if (!ctx || !out) return PANO_ERR_INVALID;
   *out = nullptr;
   if (n <= 0 || !imgs || !g || !p || bands < 0) return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: bad argument");
+  if (n > PANO_MAX_IMAGES)   // a window's images on gridDim.z of k_mb_first_level
+    return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: %d images (limit %d)", n, PANO_MAX_IMAGES);
   pano_blend_stream* s = new pano_blend_stream;
   s->ctx = ctx; s->n = n; s->bands = bands; s->lazy = p->lazy_read; s->ordered = p->ordered_input;
   int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, 0, oh, false, &s->job);
@@ -1006,6 +1010,7 @@ int pano_blend(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_bl
                const pano_params* p, float* out, int ow, int oh) {
   ctx_enter(ctx);
   if (!ctx || n <= 0 || !imgs || !out) return PANO_ERR_INVALID;
+  if (n > PANO_MAX_IMAGES) return ctx_fail(ctx, PANO_ERR_INVALID, "blend: %d images (limit %d)", n, PANO_MAX_IMAGES);
   std::vector<pano_blend_image> dimgs(imgs, imgs + n);
   std::vector<float*> bufs(n, nullptr);
   float* d_out = nullptr;

@@ -178,6 +178,9 @@ int ctx_tma_encode(pano_ctx* ctx, TmaDesc* out, void* base, int rank, const unsi
                    const unsigned long long* strides_bytes, const unsigned* box);
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+// gridDim.y for `count` items (at least 1 block).  CUDA refuses a grid.y above 65,535, so kernels whose
+// y index is an input count (pairs, sides, segments) loop: item = blockIdx.y; item < count; item += gridDim.y.
+static inline unsigned grid_y(long long count) { return (unsigned)(count < 1 ? 1 : count < 65535 ? count : 65535); }
 static inline size_t align_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 
 // Gaussian kernel exactly as GaussCache builds it (feature/gaussian.cc:17-40);

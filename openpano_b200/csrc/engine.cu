@@ -370,15 +370,19 @@ int ctx_store_many(pano_ctx* ctx, int n, void* const* h_pinned_dst, const void* 
 // Many device-to-device block moves in ONE launch (the descriptor exchange moves two blocks per
 // image: dozens of cudaMemcpyAsync calls cost more host time than the copies take on the GPU).
 struct CopySeg { void* dst; const void* src; unsigned long long bytes; };
-__global__ void k_copy_blocks(const CopySeg* __restrict__ segs) {
-  const CopySeg sg = segs[blockIdx.y];
-  const size_t n16 = sg.bytes >> 4;
-  const uint4* s4 = (const uint4*)sg.src;
-  uint4* d4 = (uint4*)sg.dst;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (size_t)gridDim.x * blockDim.x) d4[i] = s4[i];
-  const size_t tail0 = n16 << 4;
-  for (size_t i = tail0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < sg.bytes; i += (size_t)gridDim.x * blockDim.x)
-    ((unsigned char*)sg.dst)[i] = ((const unsigned char*)sg.src)[i];
+// Segments on gridDim.y (at most 65,535; two per image of a featureset): the blocks of a y index take
+// every gridDim.y-th segment.
+__global__ void k_copy_blocks(const CopySeg* __restrict__ segs, int n_segs) {
+  for (int s = blockIdx.y; s < n_segs; s += gridDim.y) {
+    const CopySeg sg = segs[s];
+    const size_t n16 = sg.bytes >> 4;
+    const uint4* s4 = (const uint4*)sg.src;
+    uint4* d4 = (uint4*)sg.dst;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (size_t)gridDim.x * blockDim.x) d4[i] = s4[i];
+    const size_t tail0 = n16 << 4;
+    for (size_t i = tail0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < sg.bytes; i += (size_t)gridDim.x * blockDim.x)
+      ((unsigned char*)sg.dst)[i] = ((const unsigned char*)sg.src)[i];
+  }
 }
 
 // dst / src must be 16-byte aligned device pointers (or bytes[i] < 16)
@@ -393,10 +397,10 @@ int ctx_copy_blocks(pano_ctx* ctx, int n, void* const* dst, const void* const* s
   int rc = ctx_alloc(ctx, (void**)&d_segs, segs.size() * sizeof(CopySeg));
   if (rc) return rc;
   if ((rc = ctx_put(ctx, d_segs, segs.data(), segs.size() * sizeof(CopySeg)))) { ctx_free(ctx, d_segs); return rc; }
-  dim3 grid((unsigned)std::min<size_t>(std::max<size_t>(mx / (16 * 256 * 4), 1), 64), (unsigned)segs.size());
+  dim3 grid((unsigned)std::min<size_t>(std::max<size_t>(mx / (16 * 256 * 4), 1), 64), grid_y((long long)segs.size()));
   ctx->launches++;
   if (ctx->profiling) ctx_prof_begin(ctx, "k_copy_blocks");
-  k_copy_blocks<<<grid, 256, 0, ctx->stream>>>(d_segs);
+  k_copy_blocks<<<grid, 256, 0, ctx->stream>>>(d_segs, (int)segs.size());
   if (ctx->profiling) ctx_prof_end(ctx);
   cudaError_t e = cudaGetLastError();
   ctx_free(ctx, d_segs);
@@ -799,6 +803,8 @@ static int featureset_build(pano_ctx* ctx, int n_images, const int* n_kp, const 
                             const double* const* coor, pano_featureset** out, bool from_device) {
   if (!ctx || !out || n_images <= 0 || !n_kp || !desc) return PANO_ERR_INVALID;
   *out = nullptr;
+  if (n_images > PANO_MAX_IMAGES)   // the matcher prepares its operands with images on gridDim.y
+    return ctx_fail(ctx, PANO_ERR_INVALID, "featureset: %d images (limit %d)", n_images, PANO_MAX_IMAGES);
   pano_featureset* fs = new pano_featureset;
   fs->ctx = ctx; fs->n_images = n_images;
   fs->base.resize(n_images); fs->h_count.resize(n_images);

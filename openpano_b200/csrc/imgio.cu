@@ -321,6 +321,9 @@ int pano_rgb8_to_mat32f_batch_dev(pano_ctx* ctx, int n, const unsigned char* con
   ctx_enter(ctx);
   if (!ctx || n < 0 || (n && (!d_pix || !w || !h || !channels || !d_out_hwc)))
     return ctx_fail(ctx, PANO_ERR_INVALID, "pano_rgb8_to_mat32f_batch_dev: bad argument");
+  if (n > PANO_MAX_IMAGES)   // images on gridDim.y
+    return ctx_fail(ctx, PANO_ERR_INVALID, "pano_rgb8_to_mat32f_batch_dev: %d images in one batch (limit %d): split the batch",
+                    n, PANO_MAX_IMAGES);
   if (n == 0) return PANO_OK;
   std::vector<Rgb8Job> jobs(n);
   long long max_px = 0;

@@ -217,13 +217,11 @@ __device__ __forceinline__ RowInfo refine_row(const float* __restrict__ desc, co
 
 // lazy != 0: the sides of the larger sets (odd side indices) have not been through the tensor
 // pass; their rows start unknown and are nominated on request (k_refine_gathered).
-__global__ void k_refine(const float* __restrict__ desc, const float* __restrict__ norms,
-                         const unsigned* __restrict__ maxnorm_bits, const SideMeta* __restrict__ sides,
-                         TcTop2* __restrict__ approx, long long res_total, float ratio_sqr, int lazy,
-                         RowInfo* __restrict__ info) {
-  const int side = blockIdx.y;
+__device__ __forceinline__ void refine_side_row(const float* __restrict__ desc, const float* __restrict__ norms,
+                                                const unsigned* __restrict__ maxnorm_bits, const SideMeta* __restrict__ sides,
+                                                TcTop2* __restrict__ approx, long long res_total, float ratio_sqr, int lazy,
+                                                RowInfo* __restrict__ info, int side, int r) {
   const SideMeta sm = sides[side];
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= sm.q_n) return;
   if (r < sm.r0 || r >= sm.r1) return;      // another shard's row: never decided, never a column here
   if (lazy && (side & 1) && sm.t_n > 0) {
@@ -244,6 +242,16 @@ __global__ void k_refine(const float* __restrict__ desc, const float* __restrict
     approx[sm.res_off + r] = ap;     // where the filter pass looks for the row's threshold
   }
   info[sm.res_off + r] = refine_row(desc, sm, r, ap, tc_eps(norms[sm.q_base + r], nmax), ratio_sqr);
+}
+
+// sides on gridDim.y, which stops at 65,535: the blocks of a y index take every gridDim.y-th side
+__global__ void k_refine(const float* __restrict__ desc, const float* __restrict__ norms,
+                         const unsigned* __restrict__ maxnorm_bits, const SideMeta* __restrict__ sides, int n_sides,
+                         TcTop2* __restrict__ approx, long long res_total, float ratio_sqr, int lazy,
+                         RowInfo* __restrict__ info) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int side = blockIdx.y; side < n_sides; side += gridDim.y)
+    refine_side_row(desc, norms, maxnorm_bits, sides, approx, res_total, ratio_sqr, lazy, info, side, r);
 }
 
 // The same certification for rows nominated on request: gathered row g carries (side, row) in
@@ -346,13 +354,13 @@ __device__ __forceinline__ void request_row(const SideMeta* __restrict__ sides, 
   }
 }
 
-__global__ void k_match_decide(const PairMeta* __restrict__ pairs, const SideMeta* __restrict__ sides,
-                               RowInfo* __restrict__ info, float ratio_sqr, int first_round,
-                               int* __restrict__ out, int* __restrict__ total,
-                               int* list_rows, int* list_unknown, int* __restrict__ side_cnt,
-                               int n_sides) {
-  const PairMeta pm = pairs[blockIdx.y];
-  const int k = pm.k0 + blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void match_decide_row(const PairMeta* __restrict__ pairs, const SideMeta* __restrict__ sides,
+                                                 RowInfo* __restrict__ info, float ratio_sqr, int first_round,
+                                                 int* __restrict__ out, int* __restrict__ total,
+                                                 int* list_rows, int* list_unknown, int* __restrict__ side_cnt,
+                                                 int n_sides, int pair, int row) {
+  const PairMeta pm = pairs[pair];
+  const int k = pm.k0 + row;
   if (k >= pm.k1) return;
   const size_t oslot = pm.out_off + k;
   if (!first_round && out[oslot] != OUT_PENDING) return;
@@ -405,6 +413,18 @@ __global__ void k_match_decide(const PairMeta* __restrict__ pairs, const SideMet
   }
   out[oslot] = result;
   if (result >= 0) atomicAdd(total, 1);
+}
+
+// pairs on gridDim.y, which stops at 65,535: the blocks of a y index take every gridDim.y-th pair
+__global__ void k_match_decide(const PairMeta* __restrict__ pairs, int n_pairs, const SideMeta* __restrict__ sides,
+                               RowInfo* __restrict__ info, float ratio_sqr, int first_round,
+                               int* __restrict__ out, int* __restrict__ total,
+                               int* list_rows, int* list_unknown, int* __restrict__ side_cnt,
+                               int n_sides) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int pair = blockIdx.y; pair < n_pairs; pair += gridDim.y)
+    match_decide_row(pairs, sides, info, ratio_sqr, first_round, out, total, list_rows, list_unknown, side_cnt, n_sides,
+                     pair, row);
 }
 
 // Plans the gathered second tensor pass: every side with requested rows gets
@@ -744,7 +764,8 @@ static int run_plan(pano_ctx* ctx, pano_featureset* fs, const MatchPlan& pl, flo
   }
   if (pl.pairs.empty()) return PANO_OK;
   const float rs = ratio * ratio;
-  dim3 gd(std::max(1, ceil_div(pl.max_small, 256)), (unsigned)pl.pairs.size());
+  const int n_pairs = (int)pl.pairs.size();
+  dim3 gd(std::max(1, ceil_div(pl.max_small, 256)), grid_y(n_pairs));
   if (!tensor) {
     const size_t smem = (size_t)2 * MT * MT_STRIDE * sizeof(float);
     if (!ctx->attr_match) {   // per device, hence per context (see match_tc.cu)
@@ -756,7 +777,7 @@ static int run_plan(pano_ctx* ctx, pano_featureset* fs, const MatchPlan& pl, flo
                   (const MatchTask*)b.tasks, b.info);
     if (pl.max_small > 0) {
       if ((rc = ctx_alloc(ctx, (void**)&b.list_rows, nres * sizeof(int)))) return rc;
-      PANO_LAUNCH(ctx, "k_match_decide", k_match_decide, gd, 256, 0, b.pairs, b.sides, b.info, rs, 1, b.out,
+      PANO_LAUNCH(ctx, "k_match_decide", k_match_decide, gd, 256, 0, b.pairs, n_pairs, b.sides, b.info, rs, 1, b.out,
                   b.counters, b.list_rows, b.list_rows, b.counters + MC_HEAD, n_sides);
     }
     return PANO_OK;
@@ -764,8 +785,8 @@ static int run_plan(pano_ctx* ctx, pano_featureset* fs, const MatchPlan& pl, flo
   rc = tc_run_top2(ctx, ops, (const TcTask*)b.tasks, (int)pl.tc_tasks.size(), b.approx);
   if (rc) return rc;
   if (pl.max_side_n > 0) {
-    dim3 gr(ceil_div(pl.max_side_n, 128), (unsigned)pl.sides.size());
-    PANO_LAUNCH(ctx, "k_refine", k_refine, gr, 128, 0, fs->d_desc, ops->d_norms, ops->d_maxnorm, b.sides, b.approx,
+    dim3 gr(ceil_div(pl.max_side_n, 128), grid_y(n_sides));
+    PANO_LAUNCH(ctx, "k_refine", k_refine, gr, 128, 0, fs->d_desc, ops->d_norms, ops->d_maxnorm, b.sides, n_sides, b.approx,
                 (long long)pl.res_total, rs, pl.lazy ? 1 : 0, b.info);
   }
   if (pl.max_small > 0) {
@@ -814,7 +835,7 @@ static int run_plan(pano_ctx* ctx, pano_featureset* fs, const MatchPlan& pl, flo
       int* side_cnt = b.counters + MC_HEAD + round * 2 * n_sides;
       int* fb_cnt = b.counters + MC_FB(round);
       int* n_blocks = b.counters + MC_BLK_FILTER(round);
-      PANO_LAUNCH(ctx, "k_match_decide", k_match_decide, gd, 256, 0, b.pairs, b.sides, b.info, rs, round == 0 ? 1 : 0,
+      PANO_LAUNCH(ctx, "k_match_decide", k_match_decide, gd, 256, 0, b.pairs, n_pairs, b.sides, b.info, rs, round == 0 ? 1 : 0,
                   b.out, b.counters, b.list_rows, list_unknown, side_cnt, n_sides);
       if (round == b.rounds) break;
       if (pl.lazy) {

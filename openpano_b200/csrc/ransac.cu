@@ -29,21 +29,24 @@ __device__ __forceinline__ bool ransac_inlier(const double* __restrict__ h, doub
   return dist < (double)inlier_dist;
 }
 
-// one warp per hypothesis: lanes stride over the pair's matches
+// one warp per hypothesis: lanes stride over the pair's matches; pairs on gridDim.y (at most 65,535:
+// the blocks of a y index take every gridDim.y-th pair)
 __global__ void __launch_bounds__(256)
-k_ransac_count(const RansacPair* __restrict__ pairs, const double2* __restrict__ kp1, const double2* __restrict__ kp2,
-               const double* __restrict__ homos, int* __restrict__ counts) {
-  const RansacPair pr = pairs[blockIdx.y];
+k_ransac_count(const RansacPair* __restrict__ pairs, int n_pairs, const double2* __restrict__ kp1,
+               const double2* __restrict__ kp2, const double* __restrict__ homos, int* __restrict__ counts) {
   const int lane = threadIdx.x & 31;
-  for (int k = blockIdx.x * 8 + (threadIdx.x >> 5); k < pr.n_hyp; k += gridDim.x * 8) {
-    double h[9];
+  for (int p = blockIdx.y; p < n_pairs; p += gridDim.y) {
+    const RansacPair pr = pairs[p];
+    for (int k = blockIdx.x * 8 + (threadIdx.x >> 5); k < pr.n_hyp; k += gridDim.x * 8) {
+      double h[9];
 #pragma unroll
-    for (int q = 0; q < 9; ++q) h[q] = __ldg(homos + (pr.hyp_off + k) * 9 + q);
-    int cnt = 0;
-    for (int i = lane; i < pr.n_match; i += 32)
-      cnt += ransac_inlier(h, kp2[pr.match_off + i], kp1[pr.match_off + i], pr.inlier_dist) ? 1 : 0;
-    for (int off = 16; off; off >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
-    if (lane == 0) counts[pr.hyp_off + k] = cnt;
+      for (int q = 0; q < 9; ++q) h[q] = __ldg(homos + (pr.hyp_off + k) * 9 + q);
+      int cnt = 0;
+      for (int i = lane; i < pr.n_match; i += 32)
+        cnt += ransac_inlier(h, kp2[pr.match_off + i], kp1[pr.match_off + i], pr.inlier_dist) ? 1 : 0;
+      for (int off = 16; off; off >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
+      if (lane == 0) counts[pr.hyp_off + k] = cnt;
+    }
   }
 }
 
@@ -128,8 +131,8 @@ extern "C" int pano_ransac_score_pairs(pano_ctx* ctx, int n_pairs, const pano_ra
   if (e == cudaSuccess) {
     ctx->launches += 2;
     if (ctx->profiling) ctx_prof_begin(ctx, "k_ransac_count");
-    dim3 grid((unsigned)std::max(1, std::min((max_hyp + 7) / 8, 64)), (unsigned)n_pairs);
-    k_ransac_count<<<grid, 256, 0, ctx->stream>>>(d_meta, d_kp1, d_kp2, d_h, d_counts);
+    dim3 grid((unsigned)std::max(1, std::min((max_hyp + 7) / 8, 64)), grid_y(n_pairs));
+    k_ransac_count<<<grid, 256, 0, ctx->stream>>>(d_meta, n_pairs, d_kp1, d_kp2, d_h, d_counts);
     if (ctx->profiling) { ctx_prof_end(ctx); ctx_prof_begin(ctx, "k_ransac_select"); }
     k_ransac_select<<<n_pairs, 256, 0, ctx->stream>>>(d_meta, d_kp1, d_kp2, d_h, d_counts, d_best, d_bcnt, d_flags);
     if (ctx->profiling) ctx_prof_end(ctx);

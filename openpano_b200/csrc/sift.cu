@@ -661,7 +661,7 @@ __global__ void k_refine(const OctMeta* __restrict__ octs, const float* __restri
 #define ORI_BINS 36
 #define ORI_WARPS 4
 
-#define SIFT_MAX_IMG 512                // images per SIFT batch (prefix tables in shared memory)
+#define SIFT_MAX_IMG PANO_MAX_SIFT_BATCH   // images per SIFT batch (prefix tables in shared memory)
 
 #define ORI_QUADS 8
 __global__ void __launch_bounds__(ORI_WARPS * 32)

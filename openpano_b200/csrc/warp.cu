@@ -152,6 +152,8 @@ __global__ void k_cyl_warp_batch(const CylJobDev* __restrict__ jobs, const doubl
 static int cyl_warp_batch(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double h_factor, const pano_params* p,
                           const unsigned char* const* pix = nullptr, const int* channels = nullptr) {
   if (!ctx || n < 0 || (n && !jobs) || !p) return PANO_ERR_INVALID;
+  if (n > PANO_MAX_IMAGES)   // images on gridDim.z
+    return ctx_fail(ctx, PANO_ERR_INVALID, "cyl warp: %d images in one batch (limit %d): split the batch", n, PANO_MAX_IMAGES);
   if (n == 0) return PANO_OK;
   std::vector<CylJobDev> dj(n);
   std::vector<double> tabs;
