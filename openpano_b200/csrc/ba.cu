@@ -138,35 +138,24 @@ extern "C" int pano_ba_jacobian(pano_ctx* ctx, int n_cam, int n_pair, const pano
   if (!st || !so) return ctx_fail(ctx, PANO_ERR_CUDA, "ba: pinned staging allocation failed");
   if (n_pair) memcpy(st, pairs, (size_t)n_pair * sizeof(BaPairDev));
   if (b_pts) memcpy(st + b_pairs, pts_to, b_pts);
-  char* d_in = nullptr; char* d_out = nullptr;
-  int rc = ctx_alloc(ctx, (void**)&d_in, b_pairs + b_pts + 64);
-  if (!rc) rc = ctx_alloc(ctx, (void**)&d_out, b_rows + b_jtj + 64);
-  if (rc) { ctx_free(ctx, d_in); ctx_free(ctx, d_out); return rc; }
-  cudaError_t e = cudaMemcpyAsync(d_in, st, b_pairs + b_pts, cudaMemcpyHostToDevice, ctx->stream);
-  const BaPairDev* d_pairs = (const BaPairDev*)d_in;
+  DevBuf<char> d_in, d_out;
+  int rc = d_in.alloc(ctx, b_pairs + b_pts + 64);
+  if (!rc) rc = d_out.alloc(ctx, b_rows + b_jtj + 64);
+  if (rc) return rc;
+  PANO_CUDA(ctx, cudaMemcpyAsync(d_in, st, b_pairs + b_pts, cudaMemcpyHostToDevice, ctx->stream));
+  const BaPairDev* d_pairs = (const BaPairDev*)d_in.get();
   const double2* d_pts = (const double2*)(d_in + b_pairs);
-  double* d_rows = (double*)d_out;
+  double* d_rows = (double*)d_out.get();
   double* d_jtj = (double*)(d_out + b_rows);
-  if (e == cudaSuccess) {
-    if (n_pair && max_match) {
-      ctx->launches++;
-      if (ctx->profiling) ctx_prof_begin(ctx, "k_ba_rows");
-      dim3 grid((unsigned)std::max(1, std::min((max_match + 127) / 128, 1024)), grid_y(n_pair));
-      k_ba_rows<<<grid, 128, 0, ctx->stream>>>(d_pairs, n_pair, d_pts, d_rows);
-      if (ctx->profiling) ctx_prof_end(ctx);
-    }
-    ctx->launches++;
-    if (ctx->profiling) ctx_prof_begin(ctx, "k_ba_jtj");
-    dim3 gj((unsigned)n_cam, (unsigned)n_cam);
-    k_ba_jtj<<<gj, 64, 0, ctx->stream>>>(d_pairs, n_pair, n_cam, d_rows, d_jtj);
-    if (ctx->profiling) ctx_prof_end(ctx);
-    e = cudaGetLastError();
+  if (n_pair && max_match) {
+    dim3 grid((unsigned)std::max(1, std::min((max_match + 127) / 128, 1024)), grid_y(n_pair));
+    PANO_LAUNCH(ctx, "k_ba_rows", k_ba_rows, grid, 128, 0, d_pairs, n_pair, d_pts, d_rows);
   }
-  if (e == cudaSuccess && j_rows && b_rows) e = cudaMemcpyAsync(so, d_rows, b_rows, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(so + (j_rows ? b_rows : 0), d_jtj, b_jtj, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  ctx_free(ctx, d_in); ctx_free(ctx, d_out);
-  if (e != cudaSuccess) return ctx_cuda(ctx, e, "ba jacobian");
+  dim3 gj((unsigned)n_cam, (unsigned)n_cam);
+  PANO_LAUNCH(ctx, "k_ba_jtj", k_ba_jtj, gj, 64, 0, d_pairs, n_pair, n_cam, d_rows, d_jtj);
+  if (j_rows && b_rows) PANO_CUDA(ctx, cudaMemcpyAsync(so, d_rows, b_rows, cudaMemcpyDeviceToHost, ctx->stream));
+  PANO_CUDA(ctx, cudaMemcpyAsync(so + (j_rows ? b_rows : 0), d_jtj, b_jtj, cudaMemcpyDeviceToHost, ctx->stream));
+  PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (j_rows && b_rows) memcpy(j_rows, so, b_rows);
   memcpy(jtj, so + (j_rows ? b_rows : 0), b_jtj);
   return PANO_OK;
@@ -314,7 +303,7 @@ struct pano_ba_session {
   long long nm = 0;
   bool have_error = false;                 // residuals of a pano_ba_error call are on the device
   std::vector<BaPairDev> table;            // links + the matrices of the last pano_ba_normal_equations
-  char* arena = nullptr;
+  DevBuf<char> arena;
   BaPairDev* d_pairs = nullptr;
   double2 *d_to = nullptr, *d_from = nullptr, *d_res = nullptr;
   double *d_rows = nullptr, *d_hto = nullptr, *d_jtj = nullptr, *d_b = nullptr;
@@ -357,7 +346,7 @@ extern "C" int pano_ba_session_create(pano_ctx* ctx, int n_cam, int n_pair, cons
   const size_t b_hto = align_up((size_t)n_pair * 72 + 16, 256), b_jtj = align_up(N * N * 8, 256), b_b = align_up(N * 8, 256);
   const size_t b_st = 256, b_flags = align_up((size_t)n_pair * 4 + 16, 256);
   const size_t total = b_pairs + 3 * b_pts + b_rows + b_sq + b_hto + b_jtj + b_b + b_st + b_flags;
-  int rc = ctx_alloc(ctx, (void**)&s->arena, total);
+  int rc = s->arena.alloc(ctx, total);
   if (rc) { delete s; return rc; }
   char* q = s->arena;
   s->d_pairs = (BaPairDev*)q; q += b_pairs;
@@ -400,7 +389,6 @@ extern "C" void pano_ba_session_free(pano_ba_session* s) {
   if (!s) return;
   ctx_enter(s->ctx);
   cudaStreamSynchronize(s->ctx->stream);                  // h_out may still be written by a queued kernel
-  if (s->arena) ctx_free(s->ctx, s->arena);
   if (s->h_out) ctx_small_pinned_put(s->ctx, s->h_out, s->h_out_cap);
   delete s;
 }

@@ -15,6 +15,7 @@
 #include <vector>
 #include <algorithm>
 #include <climits>
+#include <memory>
 
 struct BlendImg {
   union {
@@ -458,27 +459,17 @@ struct BlendJob {
 // The device state of one blend: image table, projection tables and, for multiband, the ROI level
 // buffers, masks, target mask and blur tables.
 struct BlendDev {
-  BlendImg* d_imgs = nullptr;
-  double* d_tab = nullptr;
-  float *d_cur = nullptr, *d_next = nullptr;
-  unsigned char *d_mask = nullptr, *d_tmask = nullptr;
-  MbPlane* d_planes = nullptr;
-  int2* d_span = nullptr;
-  TmaDesc* d_maps = nullptr;
+  DevBuf<BlendImg> d_imgs;
+  DevBuf<double> d_tab;
+  DevBuf<float> d_cur, d_next;
+  DevBuf<unsigned char> d_mask, d_tmask;
+  DevBuf<MbPlane> d_planes;
+  DevBuf<int2> d_span;
+  DevBuf<TmaDesc> d_maps;
   std::vector<int> centers;   // distinct TMA blur half-widths
   int n_planes = 0, n_tiles = 0;
   int wrow0 = 0, wrow1 = 0;   // rows the weight map is needed on
 };
-
-#define BL_LAUNCH(ctx, name, kernel, grid, block, smem, ...)                        \
-  do {                                                                              \
-    (ctx)->launches++;                                                              \
-    if ((ctx)->profiling) ctx_prof_begin((ctx), (name));                            \
-    kernel<<<(grid), (block), (smem), (ctx)->stream>>>(__VA_ARGS__);                \
-    if ((ctx)->profiling) ctx_prof_end((ctx));                                      \
-    cudaError_t _e = cudaGetLastError();                                            \
-    if (_e != cudaSuccess) return ctx_cuda((ctx), _e, name);                        \
-  } while (0)
 
 template <int C>
 static cudaError_t launch_mb_blur_tma(pano_ctx* ctx, int grid, const MbPlane* planes, const int2* span, int n_planes,
@@ -562,19 +553,12 @@ static int blend_plan(pano_ctx* ctx, int n, const pano_blend_image* imgs, const 
   return PANO_OK;
 }
 
-static void blend_dev_free(pano_ctx* ctx, BlendDev* d) {
-  ctx_free(ctx, d->d_imgs); ctx_free(ctx, d->d_tab); ctx_free(ctx, d->d_cur); ctx_free(ctx, d->d_next);
-  ctx_free(ctx, d->d_mask); ctx_free(ctx, d->d_tmask); ctx_free(ctx, d->d_planes); ctx_free(ctx, d->d_span);
-  ctx_free(ctx, d->d_maps);
-  *d = BlendDev();
-}
-
-// Allocates and uploads the device state of `job` (rows [row0, row1)); on failure the caller frees *d.
+// Allocates and uploads the device state of `job` (rows [row0, row1)).
 static int blend_dev_setup(pano_ctx* ctx, BlendJob* job, int bands, int row0, int row1, BlendDev* d) {
   const int n = (int)job->imgs.size(), tw = job->tw, th = job->th;
   int rc = 0;
-  if ((rc = ctx_alloc(ctx, (void**)&d->d_imgs, n * sizeof(BlendImg)))) return rc;
-  if ((rc = ctx_alloc(ctx, (void**)&d->d_tab, std::max<size_t>(job->tab.size(), 1) * sizeof(double)))) return rc;
+  if ((rc = d->d_imgs.alloc(ctx, n))) return rc;
+  if ((rc = d->d_tab.alloc(ctx, std::max<size_t>(job->tab.size(), 1)))) return rc;
   {
     void* dsts[2] = {d->d_imgs, d->d_tab};
     const void* srcs[2] = {job->imgs.data(), job->tab.data()};
@@ -584,14 +568,14 @@ static int blend_dev_setup(pano_ctx* ctx, BlendJob* job, int bands, int row0, in
   job->g.col_sin = d->d_tab; job->g.col_cos = d->d_tab + job->ncol; job->g.row_tan = d->d_tab + 2 * job->ncol;
   if (bands == 0) return PANO_OK;
   const size_t roi = (size_t)job->roi_floats;
-  if ((rc = ctx_alloc(ctx, (void**)&d->d_cur, roi * sizeof(float)))) return rc;
-  if ((rc = ctx_alloc(ctx, (void**)&d->d_next, roi * sizeof(float)))) return rc;
-  if ((rc = ctx_alloc(ctx, (void**)&d->d_mask, (size_t)job->mask_bytes))) return rc;
+  if ((rc = d->d_cur.alloc(ctx, roi))) return rc;
+  if ((rc = d->d_next.alloc(ctx, roi))) return rc;
+  if ((rc = d->d_mask.alloc(ctx, (size_t)job->mask_bytes))) return rc;
   const size_t strip_px = (size_t)tw * (row1 - row0);
   // the weight map is needed wherever a clipped ROI has pixels on the canvas
   d->wrow0 = std::max(0, std::max(row0 - job->halo, job->clip0));
   d->wrow1 = std::min(th, job->strip ? row1 + job->halo : th);
-  if ((rc = ctx_alloc(ctx, (void**)&d->d_tmask, strip_px))) return rc;
+  if ((rc = d->d_tmask.alloc(ctx, strip_px))) return rc;
   // plane table of the blur launches: (image, channel) -> offset, size; tiles of 64x32
   d->n_planes = 4 * n;
   std::vector<MbPlane> planes(d->n_planes);
@@ -604,8 +588,8 @@ static int blend_dev_setup(pano_ctx* ctx, BlendJob* job, int bands, int row0, in
       d->n_tiles += ceil_div(im.rw, BT_W) * ceil_div(im.rh, BT_H);
     }
   if (bands > 1) {
-    if ((rc = ctx_alloc(ctx, (void**)&d->d_planes, d->n_planes * sizeof(MbPlane)))) return rc;
-    if ((rc = ctx_alloc(ctx, (void**)&d->d_span, d->n_planes * sizeof(int2)))) return rc;
+    if ((rc = d->d_planes.alloc(ctx, d->n_planes))) return rc;
+    if ((rc = d->d_span.alloc(ctx, d->n_planes))) return rc;
     if ((rc = ctx_put(ctx, d->d_planes, planes.data(), d->n_planes * sizeof(MbPlane)))) return rc;
     if ((rc = ctx_put(ctx, d->d_span, span.data(), d->n_planes * sizeof(int2)))) return rc;
   }
@@ -627,7 +611,7 @@ static int blend_dev_setup(pano_ctx* ctx, BlendJob* job, int bands, int row0, in
                                    dims, strides, box)))
             return rc;
         }
-    if ((rc = ctx_alloc(ctx, (void**)&d->d_maps, maps.size() * sizeof(TmaDesc)))) return rc;
+    if ((rc = d->d_maps.alloc(ctx, maps.size()))) return rc;
     if ((rc = ctx_put(ctx, d->d_maps, maps.data(), maps.size() * sizeof(TmaDesc)))) return rc;
   }
   return PANO_OK;
@@ -639,7 +623,7 @@ static int mb_levels(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands,
   const int n = (int)job.imgs.size(), tw = job.tw;
   const dim3 b(32, 8);
   dim3 gw(ceil_div(tw, 32), ceil_div(d->wrow1 - d->wrow0, 8)), gs(ceil_div(tw, 32), ceil_div(row1 - row0, 8));
-  BL_LAUNCH(ctx, "k_mb_weight_argmax", k_mb_weight_argmax, gw, b, 0, d->d_imgs, n, d->d_cur, tw, d->wrow0, d->wrow1);
+  PANO_LAUNCH(ctx, "k_mb_weight_argmax", k_mb_weight_argmax, gw, b, 0, d->d_imgs, n, d->d_cur, tw, d->wrow0, d->wrow1);
   float *cur = d->d_cur, *next = d->d_next;
   int buf = 0;     // which level buffer `cur` currently is (0: the first allocation)
   for (int level = 0; level < bands; ++level) {
@@ -671,7 +655,7 @@ static int mb_levels(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands,
       if (ctx->profiling) ctx_prof_end(ctx);
       if (e != cudaSuccess) return ctx_cuda(ctx, e, "k_mb_blur");
     }
-    BL_LAUNCH(ctx, "k_mb_accumulate", k_mb_accumulate, gs, b, 0, d->d_imgs, n, cur, next, d->d_mask, level == 0 ? 1 : 0,
+    PANO_LAUNCH(ctx, "k_mb_accumulate", k_mb_accumulate, gs, b, 0, d->d_imgs, n, cur, next, d->d_mask, level == 0 ? 1 : 0,
               is_last, d_out, d->d_tmask, tw, row0, row1);
     if (!is_last) { std::swap(cur, next); buf ^= 1; }
   }
@@ -685,12 +669,12 @@ static int blend_run(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands,
   const dim3 b(32, 8);   // 256 threads: the 8-bit kernels' conversion table
   if (bands == 0) {
     dim3 gs(ceil_div(tw, 32), ceil_div(row1 - row0, 8));
-    BL_LAUNCH(ctx, Src::kLut ? "k_linear_blend_rgb8" : "k_linear_blend", k_linear_blend<Src>, gs, b, 0, d->d_imgs, n,
+    PANO_LAUNCH(ctx, Src::kLut ? "k_linear_blend_rgb8" : "k_linear_blend", k_linear_blend<Src>, gs, b, 0, d->d_imgs, n,
               job.g, p->lazy_read, p->ordered_input, d_out, tw, row0, row1);
     return PANO_OK;
   }
   dim3 gr(ceil_div(job.max_rw, 32), ceil_div(job.max_rh, 8), n);
-  BL_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<Src>, gr, b, 0, d->d_imgs, job.g, d->d_cur, d->d_mask);
+  PANO_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<Src>, gr, b, 0, d->d_imgs, job.g, d->d_cur, d->d_mask);
   return mb_levels(ctx, job, d, bands, d_out, row0, row1);
 }
 
@@ -714,11 +698,9 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
     return PANO_OK;
   }
   BlendDev dev;
-  rc = blend_dev_setup(ctx, &job, bands, row0, row1, &dev);
-  if (!rc) rc = pix ? blend_run<SrcRgb8>(ctx, job, &dev, bands, p, d_out, row0, row1)
-                    : blend_run<SrcF32>(ctx, job, &dev, bands, p, d_out, row0, row1);
-  blend_dev_free(ctx, &dev);
-  return rc;
+  if ((rc = blend_dev_setup(ctx, &job, bands, row0, row1, &dev))) return rc;
+  return pix ? blend_run<SrcRgb8>(ctx, job, &dev, bands, p, d_out, row0, row1)
+             : blend_run<SrcF32>(ctx, job, &dev, bands, p, d_out, row0, row1);
 }
 
 // ------------------------------------------------------------------ blend stream
@@ -732,31 +714,28 @@ struct pano_blend_stream {
   int n = 0, bands = 0, lazy = 0, ordered = 0;
   BlendJob job;
   BlendDev dev;
-  float* d_sum = nullptr;      // linear: tw×th×3 Σ c·w
-  float* d_wsum = nullptr;     // linear: tw×th Σ w
+  DevBuf<float> d_sum;         // linear: tw×th×3 Σ c·w
+  DevBuf<float> d_wsum;        // linear: tw×th Σ w
   int added = 0, windows = 0, err = 0;
   bool finished = false;
   cudaStream_t copy = nullptr;
   cudaEvent_t ev_copied[2] = {nullptr, nullptr};   // slot's upload done (copy stream)
   cudaEvent_t ev_done[2] = {nullptr, nullptr};     // slot's last reader done (context stream)
-  unsigned char* slot[2] = {nullptr, nullptr};
+  DevBuf<unsigned char> slot[2];
   size_t slot_cap[2] = {0, 0};
   unsigned char* stage[2] = {nullptr, nullptr};    // pinned staging of pageable sources
   size_t stage_cap[2] = {0, 0};
 };
 
+// the device blocks go with the stream's owners, after its copy stream has drained
 static void blend_stream_release(pano_blend_stream* s) {
-  pano_ctx* ctx = s->ctx;
   if (s->copy) cudaStreamSynchronize(s->copy);
   for (int b = 0; b < 2; ++b) {
-    ctx_free(ctx, s->slot[b]);
     if (s->stage[b]) cudaFreeHost(s->stage[b]);
     if (s->ev_copied[b]) cudaEventDestroy(s->ev_copied[b]);
     if (s->ev_done[b]) cudaEventDestroy(s->ev_done[b]);
   }
   if (s->copy) cudaStreamDestroy(s->copy);
-  ctx_free(ctx, s->d_sum); ctx_free(ctx, s->d_wsum);
-  blend_dev_free(ctx, &s->dev);
   delete s;
 }
 
@@ -788,10 +767,8 @@ static int stream_upload(pano_blend_stream* s, int first, int count, const void*
   // refills the staging buffer (an event never recorded counts as complete)
   STREAM_CUDA(s, cudaEventSynchronize(s->ev_copied[b]));
   if (s->slot_cap[b] < total) {
-    ctx_free(ctx, s->slot[b]);
-    s->slot[b] = nullptr; s->slot_cap[b] = 0;
-    int rc = ctx_alloc(ctx, (void**)&s->slot[b], total);
-    if (rc) return stream_fail(s, rc);
+    s->slot[b].reset(); s->slot_cap[b] = 0;
+    if (int rc = s->slot[b].alloc(ctx, total)) return stream_fail(s, rc);
     s->slot_cap[b] = total;
     STREAM_CUDA(s, cudaEventRecord(s->ev_done[b], ctx->stream));   // the block is ours from here on the context stream
   }
@@ -833,13 +810,13 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
     x1 = std::min(x1, job.tw); y1 = std::min(y1, job.th);
     if (x0 >= x1 || y0 >= y1) return PANO_OK;
     dim3 g(ceil_div(x1 - x0, 32), ceil_div(y1 - y0, 8));
-    BL_LAUNCH(ctx, "k_linear_accumulate", k_linear_accumulate<Src>, g, b, 0, d_win, count, job.g, s->lazy, s->ordered,
+    PANO_LAUNCH(ctx, "k_linear_accumulate", k_linear_accumulate<Src>, g, b, 0, d_win, count, job.g, s->lazy, s->ordered,
               s->d_sum, s->d_wsum, job.tw, x0, y0, x1, y1);
   } else {
     int rw = 0, rh = 0;
     for (int k = 0; k < count; ++k) { rw = std::max(rw, win[k].rw); rh = std::max(rh, win[k].rh); }
     dim3 g(ceil_div(rw, 32), ceil_div(rh, 8), count);
-    BL_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<Src>, g, b, 0, d_win, job.g, s->dev.d_cur, s->dev.d_mask);
+    PANO_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<Src>, g, b, 0, d_win, job.g, s->dev.d_cur, s->dev.d_mask);
   }
   return PANO_OK;
 }
@@ -910,31 +887,24 @@ int pano_blend_stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs,
   if (n <= 0 || !imgs || !g || !p || bands < 0) return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: bad argument");
   if (n > PANO_MAX_IMAGES)   // a window's images on gridDim.z of k_mb_first_level
     return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: %d images (limit %d)", n, PANO_MAX_IMAGES);
-  pano_blend_stream* s = new pano_blend_stream;
+  std::unique_ptr<pano_blend_stream, void (*)(pano_blend_stream*)> s(new pano_blend_stream, blend_stream_release);
   s->ctx = ctx; s->n = n; s->bands = bands; s->lazy = p->lazy_read; s->ordered = p->ordered_input;
   int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, 0, oh, false, &s->job);
   if (!rc) rc = blend_dev_setup(ctx, &s->job, bands, 0, oh, &s->dev);
-  const size_t npx = (size_t)ow * oh;
-  if (!rc && bands == 0) {
-    rc = ctx_alloc(ctx, (void**)&s->d_sum, npx * 3 * sizeof(float));
-    if (!rc) rc = ctx_alloc(ctx, (void**)&s->d_wsum, npx * sizeof(float));
-    if (!rc) {
-      k_fill<<<(unsigned)((npx * 3 + 255) / 256), 256, 0, ctx->stream>>>(s->d_sum, npx * 3, 0.f);
-      k_fill<<<(unsigned)((npx + 255) / 256), 256, 0, ctx->stream>>>(s->d_wsum, npx, 0.f);
-      ctx->launches += 2;
-      cudaError_t e = cudaGetLastError();
-      if (e != cudaSuccess) rc = ctx_cuda(ctx, e, "k_fill");
-    }
+  if (rc) return rc;
+  if (bands == 0) {
+    const size_t npx = (size_t)ow * oh;
+    if ((rc = s->d_sum.alloc(ctx, npx * 3)) || (rc = s->d_wsum.alloc(ctx, npx))) return rc;
+    PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx * 3 + 255) / 256), 256, 0, s->d_sum, npx * 3, 0.f);
+    PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx + 255) / 256), 256, 0, s->d_wsum, npx, 0.f);
   }
-  cudaError_t e = cudaSuccess;
-  if (!rc) e = cudaStreamCreateWithFlags(&s->copy, cudaStreamNonBlocking);
-  for (int b = 0; b < 2 && !rc && e == cudaSuccess; ++b) {
+  cudaError_t e = cudaStreamCreateWithFlags(&s->copy, cudaStreamNonBlocking);
+  for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
     e = cudaEventCreateWithFlags(&s->ev_copied[b], cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_done[b], cudaEventDisableTiming);
   }
-  if (!rc && e != cudaSuccess) rc = ctx_cuda(ctx, e, "blend stream: copy stream / events");
-  if (rc) { blend_stream_release(s); return rc; }
-  *out = s;
+  if (e != cudaSuccess) return ctx_cuda(ctx, e, "blend stream: copy stream / events");
+  *out = s.release();
   return PANO_OK;
 }
 
@@ -987,17 +957,18 @@ int pano_blend_stream_finish(pano_blend_stream* s, float* out) {
   ctx_enter(ctx);
   int rc = stream_finish_check(s, out);
   if (rc) return stream_fail(s, rc);
-  const size_t ob = (size_t)s->job.tw * s->job.th * 3 * sizeof(float);
+  const size_t nfl = (size_t)s->job.tw * s->job.th * 3;
+  DevBuf<float> d_tmp;
   float* d_out = s->d_sum;     // linear: resolved in place
-  if (s->bands > 0) rc = ctx_alloc(ctx, (void**)&d_out, ob);
-  if (!rc) rc = stream_resolve(s, d_out);
-  if (!rc) {
-    cudaError_t e = cudaMemcpyAsync(out, d_out, ob, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) rc = ctx_cuda(ctx, e, "blend stream download");
+  if (s->bands > 0) {
+    if ((rc = d_tmp.alloc(ctx, nfl))) return stream_fail(s, rc);
+    d_out = d_tmp;
   }
-  if (s->bands > 0) ctx_free(ctx, d_out);
-  return rc ? stream_fail(s, rc) : PANO_OK;
+  if ((rc = stream_resolve(s, d_out))) return stream_fail(s, rc);
+  STREAM_CUDA(s, cudaMemcpyAsync(out, d_out, nfl * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  STREAM_CUDA(s, cudaStreamSynchronize(ctx->stream));
+  d_tmp.reset();
+  return PANO_OK;
 }
 
 void pano_blend_stream_free(pano_blend_stream* s) {
@@ -1012,30 +983,22 @@ int pano_blend(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_bl
   if (!ctx || n <= 0 || !imgs || !out) return PANO_ERR_INVALID;
   if (n > PANO_MAX_IMAGES) return ctx_fail(ctx, PANO_ERR_INVALID, "blend: %d images (limit %d)", n, PANO_MAX_IMAGES);
   std::vector<pano_blend_image> dimgs(imgs, imgs + n);
-  std::vector<float*> bufs(n, nullptr);
-  float* d_out = nullptr;
+  std::vector<DevBuf<float>> bufs(n);
   int rc = 0;
-  cudaError_t e = cudaSuccess;
-  for (int k = 0; k < n && !rc; ++k) {
-    if (!imgs[k].rgb_hwc || imgs[k].w <= 0 || imgs[k].h <= 0) { rc = ctx_fail(ctx, PANO_ERR_INVALID, "blend: image %d empty", k); break; }
-    size_t bytes = (size_t)imgs[k].w * imgs[k].h * 3 * sizeof(float);
-    rc = ctx_alloc(ctx, (void**)&bufs[k], bytes);
-    if (rc) break;
-    e = cudaMemcpyAsync(bufs[k], imgs[k].rgb_hwc, bytes, cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) { rc = ctx_cuda(ctx, e, "blend image upload"); break; }
+  for (int k = 0; k < n; ++k) {
+    if (!imgs[k].rgb_hwc || imgs[k].w <= 0 || imgs[k].h <= 0) return ctx_fail(ctx, PANO_ERR_INVALID, "blend: image %d empty", k);
+    const size_t nfl = (size_t)imgs[k].w * imgs[k].h * 3;
+    if ((rc = bufs[k].alloc(ctx, nfl))) return rc;
+    PANO_CUDA(ctx, cudaMemcpyAsync(bufs[k], imgs[k].rgb_hwc, nfl * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     dimgs[k].rgb_hwc = bufs[k];
   }
-  size_t ob = (size_t)std::max(ow, 0) * std::max(oh, 0) * 3 * sizeof(float);
-  if (!rc) rc = ctx_alloc(ctx, (void**)&d_out, ob);
-  if (!rc) rc = blend_device(ctx, n, dimgs.data(), g, bands, p, d_out, ow, oh, 0, oh);
-  if (!rc) {
-    e = cudaMemcpyAsync(out, d_out, ob, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) rc = ctx_cuda(ctx, e, "blend download");
-  }
-  for (auto b : bufs) ctx_free(ctx, b);
-  ctx_free(ctx, d_out);
-  return rc;
+  const size_t nfl = (size_t)std::max(ow, 0) * std::max(oh, 0) * 3;
+  DevBuf<float> d_out;
+  if ((rc = d_out.alloc(ctx, nfl))) return rc;
+  if ((rc = blend_device(ctx, n, dimgs.data(), g, bands, p, d_out, ow, oh, 0, oh))) return rc;
+  PANO_CUDA(ctx, cudaMemcpyAsync(out, d_out, nfl * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return PANO_OK;
 }
 
 }  // extern "C"

@@ -132,19 +132,16 @@ int pano_comm_allgather_features(pano_comm* c, pano_featureset* local, int n_ima
   int rc = 0;
   if (local && (rc = featureset_sync_counts(local))) return rc;
   // ---- counts
-  int *d_cnt_send = nullptr, *d_cnt_all = nullptr;
-  if ((rc = ctx_alloc(ctx, (void**)&d_cnt_send, per_rank * sizeof(int))) ||
-      (rc = ctx_alloc(ctx, (void**)&d_cnt_all, (size_t)per_rank * W * sizeof(int))))
-    { ctx_free(ctx, d_cnt_send); ctx_free(ctx, d_cnt_all); return rc; }
+  DevBuf<int> d_cnt_send, d_cnt_all;
+  if ((rc = d_cnt_send.alloc(ctx, per_rank)) || (rc = d_cnt_all.alloc(ctx, (size_t)per_rank * W))) return rc;
   std::vector<int> cnt_mine(per_rank, 0);
   for (int q = 0; q < mine; ++q) cnt_mine[q] = local->h_count[q];
-  if ((rc = ctx_put(ctx, d_cnt_send, cnt_mine.data(), per_rank * sizeof(int)))) { ctx_free(ctx, d_cnt_send); ctx_free(ctx, d_cnt_all); return rc; }
+  if ((rc = ctx_put(ctx, d_cnt_send, cnt_mine.data(), per_rank * sizeof(int)))) return rc;
   PANO_NCCL(c, g_nccl.AllGather(d_cnt_send, d_cnt_all, per_rank, ncclInt32, c->comm, ctx->stream));
   std::vector<int> cnt_all((size_t)per_rank * W);
-  cudaError_t e = cudaMemcpyAsync(cnt_all.data(), d_cnt_all, cnt_all.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  ctx_free(ctx, d_cnt_send); ctx_free(ctx, d_cnt_all);
-  if (e != cudaSuccess) return ctx_cuda(ctx, e, "allgather_features: counts");
+  PANO_CUDA(ctx, cudaMemcpyAsync(cnt_all.data(), d_cnt_all, cnt_all.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  d_cnt_send.reset(); d_cnt_all.reset();   // before the payload buffers, which may take their blocks
   std::vector<int> counts(n_images_total);
   size_t pad = 1;
   for (int r = 0; r < W; ++r) {
@@ -153,11 +150,11 @@ int pano_comm_allgather_features(pano_comm* c, pano_featureset* local, int n_ima
     pad = std::max(pad, rows);
   }
   // ---- payload
-  float *d_send = nullptr, *d_all = nullptr;
-  double *c_send = nullptr, *c_all = nullptr;
-  if ((rc = ctx_alloc(ctx, (void**)&d_send, pad * 128 * sizeof(float))) || (rc = ctx_alloc(ctx, (void**)&d_all, pad * W * 128 * sizeof(float))) ||
-      (rc = ctx_alloc(ctx, (void**)&c_send, pad * 2 * sizeof(double))) || (rc = ctx_alloc(ctx, (void**)&c_all, pad * W * 2 * sizeof(double))))
-    goto done;
+  DevBuf<float> d_send, d_all;
+  DevBuf<double> c_send, c_all;
+  if ((rc = d_send.alloc(ctx, pad * 128)) || (rc = d_all.alloc(ctx, pad * W * 128)) || (rc = c_send.alloc(ctx, pad * 2)) ||
+      (rc = c_all.alloc(ctx, pad * W * 2)))
+    return rc;
   {
     // this rank's rows into the send buffers: one launch for all images
     std::vector<void*> dsts; std::vector<const void*> srcs; std::vector<size_t> sizes;
@@ -170,17 +167,15 @@ int pano_comm_allgather_features(pano_comm* c, pano_featureset* local, int n_ima
       }
       off += nq;
     }
-    if ((rc = ctx_copy_blocks(ctx, (int)dsts.size(), dsts.data(), srcs.data(), sizes.data()))) goto done;
+    if ((rc = ctx_copy_blocks(ctx, (int)dsts.size(), dsts.data(), srcs.data(), sizes.data()))) return rc;
   }
   {
     ncclResult_t r1 = g_nccl.GroupStart();
     ncclResult_t r2 = g_nccl.AllGather(d_send, d_all, pad * 128, ncclFloat32, c->comm, ctx->stream);
     ncclResult_t r3 = g_nccl.AllGather(c_send, c_all, pad * 2, ncclFloat64, c->comm, ctx->stream);
     ncclResult_t r4 = g_nccl.GroupEnd();
-    if (r1 != ncclSuccess || r2 != ncclSuccess || r3 != ncclSuccess || r4 != ncclSuccess) {
-      rc = ctx_fail(ctx, PANO_ERR_CUDA, "NCCL all-gather of the descriptor sets failed");
-      goto done;
-    }
+    if (r1 != ncclSuccess || r2 != ncclSuccess || r3 != ncclSuccess || r4 != ncclSuccess)
+      return ctx_fail(ctx, PANO_ERR_CUDA, "NCCL all-gather of the descriptor sets failed");
   }
   {
     std::vector<const float*> pd(n_images_total);
@@ -193,11 +188,8 @@ int pano_comm_allgather_features(pano_comm* c, pano_featureset* local, int n_ima
         off += counts[k];
       }
     }
-    rc = featureset_build_dev(ctx, n_images_total, counts.data(), pd.data(), pc.data(), all);
+    return featureset_build_dev(ctx, n_images_total, counts.data(), pd.data(), pc.data(), all);   // the buffers go after the import
   }
-done:
-  ctx_free(ctx, d_send); ctx_free(ctx, d_all); ctx_free(ctx, c_send); ctx_free(ctx, c_all);   // stream-ordered: after the import
-  return rc;
 }
 
 }  // extern "C"

@@ -69,7 +69,6 @@ struct pano_ctx {
   // recycled pinned blocks for per-featureset count read-backs (cudaHostAlloc / cudaFreeHost
   // are slow and cudaFreeHost synchronises the whole device)
   std::vector<std::pair<void*, size_t>> small_pinned;
-  std::vector<cudaEvent_t> sync_events;
   // completion markers: a word in pinned host memory the stream writes sequence numbers to
   volatile unsigned* flag = nullptr;
   unsigned flag_seq = 0;
@@ -99,6 +98,43 @@ int  ctx_cuda(pano_ctx* ctx, cudaError_t e, const char* what);
 int  ctx_alloc(pano_ctx* ctx, void** p, size_t bytes);
 void ctx_cache_release(pano_ctx* ctx, size_t keep_bytes);
 void ctx_free(pano_ctx* ctx, void* p);
+// Owner of one ctx_alloc block of T: the destructor and reset() give it back with ctx_free, so after
+// everything its scope enqueued (stream order); release() hands the pointer on without freeing it.
+// Reads as the raw pointer at kernel arguments and in pointer arithmetic.
+template <class T>
+class DevBuf {
+ public:
+  DevBuf() = default;
+  DevBuf(pano_ctx* ctx, T* p) : ctx_(ctx), p_(p) {}   // adopts a block ctx_alloc handed out
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : ctx_(o.ctx_), p_(o.release()) {}
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) { reset(); ctx_ = o.ctx_; p_ = o.release(); }
+    return *this;
+  }
+  ~DevBuf() { reset(); }
+  // `count` elements of T; a block already held is freed first
+  int alloc(pano_ctx* ctx, size_t count) {
+    reset();
+    ctx_ = ctx;
+    void* q = nullptr;
+    const int rc = ctx_alloc(ctx, &q, count * sizeof(T));
+    p_ = (T*)q;
+    return rc;
+  }
+  void reset() {
+    if (p_) ctx_free(ctx_, p_);
+    p_ = nullptr;
+  }
+  T* release() { T* q = p_; p_ = nullptr; return q; }
+  T* get() const { return p_; }
+  operator T*() const { return p_; }
+
+ private:
+  pano_ctx* ctx_ = nullptr;
+  T* p_ = nullptr;
+};
 void ctx_sift_plan_release(pano_ctx* ctx);   // frees the kept SIFT plan's blocks (into the cache)
 void* ctx_pinned(pano_ctx* ctx, size_t bytes);   // staging buffer A (inputs)
 void* ctx_pinned2(pano_ctx* ctx, size_t bytes);  // staging buffer B (results)
@@ -126,8 +162,6 @@ cudaError_t ctx_wait_signal(pano_ctx* ctx, unsigned token);
 void* ctx_ring(pano_ctx* ctx, size_t bytes);
 void* ctx_small_pinned_get(pano_ctx* ctx, size_t bytes, size_t* cap);
 void ctx_small_pinned_put(pano_ctx* ctx, void* p, size_t cap);
-cudaEvent_t ctx_sync_event_get(pano_ctx* ctx);
-void ctx_sync_event_put(pano_ctx* ctx, cudaEvent_t e);
 int  ctx_fetch(pano_ctx* ctx, void* d_dst, const void* h_pinned_src, size_t bytes);
 int  ctx_store(pano_ctx* ctx, void* h_pinned_dst, const void* d_src, size_t bytes);
 int  ctx_put(pano_ctx* ctx, void* d_dst, const void* h_src, size_t bytes);

@@ -93,7 +93,7 @@ void ctx_sift_plan_release(pano_ctx* ctx) {
   SiftPlan* plan = ctx->sift_plan;
   ctx->sift_plan = nullptr;
   ctx->sift_plan_bytes = 0;
-  sift_plan_free(ctx, plan);
+  delete plan;
 }
 
 static void* grow_pinned(void** buf, size_t* cap, size_t bytes) {
@@ -208,13 +208,6 @@ void* ctx_small_pinned_get(pano_ctx* ctx, size_t bytes, size_t* cap) {
   return p;
 }
 void ctx_small_pinned_put(pano_ctx* ctx, void* p, size_t cap) { if (p) ctx->small_pinned.emplace_back(p, cap); }
-cudaEvent_t ctx_sync_event_get(pano_ctx* ctx) {
-  if (!ctx->sync_events.empty()) { cudaEvent_t e = ctx->sync_events.back(); ctx->sync_events.pop_back(); return e; }
-  cudaEvent_t e = nullptr;
-  cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-  return e;
-}
-void ctx_sync_event_put(pano_ctx* ctx, cudaEvent_t e) { if (e) ctx->sync_events.push_back(e); }
 
 static unsigned small_grid(size_t words) { return (unsigned)std::min<size_t>(std::max<size_t>((words + 255) / 256, 1), 256); }
 
@@ -393,18 +386,13 @@ int ctx_copy_blocks(pano_ctx* ctx, int n, void* const* dst, const void* const* s
   for (int i = 0; i < n; ++i)
     if (bytes[i]) { segs.push_back(CopySeg{dst[i], src[i], (unsigned long long)bytes[i]}); mx = std::max(mx, bytes[i]); }
   if (segs.empty()) return PANO_OK;
-  CopySeg* d_segs = nullptr;
-  int rc = ctx_alloc(ctx, (void**)&d_segs, segs.size() * sizeof(CopySeg));
-  if (rc) return rc;
-  if ((rc = ctx_put(ctx, d_segs, segs.data(), segs.size() * sizeof(CopySeg)))) { ctx_free(ctx, d_segs); return rc; }
+  DevBuf<CopySeg> d_segs;
+  if (int rc = d_segs.alloc(ctx, segs.size())) return rc;
+  if (int rc = ctx_put(ctx, d_segs, segs.data(), segs.size() * sizeof(CopySeg))) return rc;
   dim3 grid((unsigned)std::min<size_t>(std::max<size_t>(mx / (16 * 256 * 4), 1), 64), grid_y((long long)segs.size()));
-  ctx->launches++;
-  if (ctx->profiling) ctx_prof_begin(ctx, "k_copy_blocks");
-  k_copy_blocks<<<grid, 256, 0, ctx->stream>>>(d_segs, (int)segs.size());
-  if (ctx->profiling) ctx_prof_end(ctx);
-  cudaError_t e = cudaGetLastError();
-  ctx_free(ctx, d_segs);
-  return e == cudaSuccess ? PANO_OK : ctx_cuda(ctx, e, "k_copy_blocks");
+  PANO_LAUNCH(ctx, "k_copy_blocks", k_copy_blocks, grid, 256, 0, d_segs, (int)segs.size());
+  d_segs.reset();
+  return PANO_OK;
 }
 
 static cudaEvent_t get_event(pano_ctx* ctx) {
@@ -532,7 +520,6 @@ void pano_destroy(pano_ctx* ctx) {
   if (ctx->ring) cudaFreeHost(ctx->ring);
   if (ctx->flag) cudaFreeHost((void*)ctx->flag);
   for (auto& sp : ctx->small_pinned) cudaFreeHost(sp.first);
-  for (auto e : ctx->sync_events) cudaEventDestroy(e);
   if (ctx->pool) cudaMemPoolDestroy(ctx->pool);   // released once the last block has been freed
   if (ctx->owns_stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
@@ -590,7 +577,7 @@ int pano_match_last_nominated_rows(const pano_ctx* ctx) {
 int pano_dev_alloc(pano_ctx* ctx, size_t bytes, void** d_ptr) {
   ctx_enter(ctx); return ctx_alloc(ctx, d_ptr, bytes); }
 int pano_dev_free(pano_ctx* ctx, void* d_ptr) {
-  ctx_enter(ctx); ctx_free(ctx, d_ptr); return PANO_OK; }
+  ctx_enter(ctx); DevBuf<unsigned char>(ctx, (unsigned char*)d_ptr).reset(); return PANO_OK; }
 int pano_dev_upload(pano_ctx* ctx, void* d_dst, const void* h_src, size_t bytes) {
   ctx_enter(ctx);
   PANO_CUDA(ctx, cudaMemcpyAsync(d_dst, h_src, bytes, cudaMemcpyHostToDevice, ctx->stream));
@@ -660,15 +647,10 @@ void pano_event_destroy(pano_event* ev) {
 
 // ---------------------------------------------------------------- features
 
+// the device blocks go with the featureset's owners
 static void featureset_release(pano_featureset* fs) {
   if (!fs) return;
   pano_ctx* ctx = fs->ctx;
-  if (ctx) {
-    ctx_free(ctx, fs->d_desc); ctx_free(ctx, fs->d_coor); ctx_free(ctx, fs->d_count);   // d_real lives inside d_coor
-    ctx_free(ctx, fs->owned_block);
-    tc_release(ctx, &fs->tc);
-  }
-  if (fs->counts_ready) { if (ctx) ctx_sync_event_put(ctx, fs->counts_ready); else cudaEventDestroy(fs->counts_ready); }
   if (fs->h_count_pinned) { if (ctx) ctx_small_pinned_put(ctx, fs->h_count_pinned, fs->h_count_cap); else cudaFreeHost(fs->h_count_pinned); }
   delete fs;
 }
@@ -708,9 +690,9 @@ bool host_is_pinned(const void* p) {
 
 // Uploads host images through one pinned staging buffer (async H2D on the ctx
 // stream), then runs the device path.  channels == nullptr: h×w×3 f32 images; otherwise
-// h×w×channels[i] u8 images.  Every image starts on a 256-byte boundary of *d_block.
+// h×w×channels[i] u8 images.  Every image starts on a 256-byte boundary of d_block.
 static int upload_images(pano_ctx* ctx, int n, const void* const* src, const int* channels, const int* w, const int* h,
-                         std::vector<const void*>& d_imgs, unsigned char** d_block) {
+                         std::vector<const void*>& d_imgs, DevBuf<unsigned char>& d_block) {
   size_t total = 0;
   std::vector<size_t> offs(n), bytes(n);
   for (int i = 0; i < n; ++i) {
@@ -719,8 +701,7 @@ static int upload_images(pano_ctx* ctx, int n, const void* const* src, const int
     bytes[i] = (size_t)w[i] * h[i] * (channels ? (size_t)channels[i] : 3 * sizeof(float));
     total += align_up(bytes[i], 256);
   }
-  int rc = ctx_alloc(ctx, (void**)d_block, total);
-  if (rc) return rc;
+  if (int rc = d_block.alloc(ctx, total)) return rc;
   // the staging buffer may still feed an earlier async copy
   PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   bool all_pinned = true;
@@ -734,8 +715,8 @@ static int upload_images(pano_ctx* ctx, int n, const void* const* src, const int
       memcpy(st + offs[i], src[i], bytes[i]);
       s = st + offs[i];
     }
-    PANO_CUDA(ctx, cudaMemcpyAsync(*d_block + offs[i], s, bytes[i], cudaMemcpyHostToDevice, ctx->stream));
-    d_imgs[i] = *d_block + offs[i];
+    PANO_CUDA(ctx, cudaMemcpyAsync(d_block + offs[i], s, bytes[i], cudaMemcpyHostToDevice, ctx->stream));
+    d_imgs[i] = d_block + offs[i];
   }
   return PANO_OK;
 }
@@ -745,11 +726,11 @@ static int upload_images(pano_ctx* ctx, int n, const void* const* src, const int
 static int sift_detect_host(pano_ctx* ctx, int n, const void* const* src, const int* channels, const int* w,
                             const int* h, const pano_params* p, pano_featureset** out) {
   std::vector<const void*> d_imgs;
-  unsigned char* d_block = nullptr;
-  int rc = upload_images(ctx, n, src, channels, w, h, d_imgs, &d_block);
+  DevBuf<unsigned char> d_block;
+  int rc = upload_images(ctx, n, src, channels, w, h, d_imgs, d_block);
   if (!rc) rc = sift_detect_dev(ctx, n, d_imgs.data(), channels, w, h, p, out);
-  if (rc) { ctx_free(ctx, d_block); return rc; }
-  (*out)->owned_block = d_block;
+  if (rc) return rc;
+  (*out)->owned_block = std::move(d_block);
   return rc;
 }
 
@@ -805,20 +786,19 @@ static int featureset_build(pano_ctx* ctx, int n_images, const int* n_kp, const 
   *out = nullptr;
   if (n_images > PANO_MAX_IMAGES)   // the matcher prepares its operands with images on gridDim.y
     return ctx_fail(ctx, PANO_ERR_INVALID, "featureset: %d images (limit %d)", n_images, PANO_MAX_IMAGES);
-  pano_featureset* fs = new pano_featureset;
+  std::unique_ptr<pano_featureset> fs(new pano_featureset);   // no pinned count block: a plain delete releases it
   fs->ctx = ctx; fs->n_images = n_images;
   fs->base.resize(n_images); fs->h_count.resize(n_images);
   long long total = 0;
   for (int i = 0; i < n_images; ++i) {
-    if (n_kp[i] < 0) { featureset_release(fs); return ctx_fail(ctx, PANO_ERR_INVALID, "negative count"); }
+    if (n_kp[i] < 0) return ctx_fail(ctx, PANO_ERR_INVALID, "negative count");
     fs->base[i] = total; fs->h_count[i] = n_kp[i];
     total += (n_kp[i] + 31) / 32 * 32;  // keep rows 32-aligned per image
   }
-  int rc = ctx_alloc(ctx, (void**)&fs->d_desc, (size_t)std::max(total, 1LL) * 128 * sizeof(float));
-  if (!rc) rc = ctx_alloc(ctx, (void**)&fs->d_count, n_images * sizeof(int));
-  if (!rc && coor) rc = ctx_alloc(ctx, (void**)&fs->d_coor, (size_t)std::max(total, 1LL) * 2 * sizeof(double));
-  if (rc) { featureset_release(fs); return rc; }
-  cudaError_t e = cudaSuccess;
+  int rc = fs->d_desc.alloc(ctx, (size_t)std::max(total, 1LL) * 128);
+  if (!rc) rc = fs->d_count.alloc(ctx, n_images);
+  if (!rc && coor) rc = fs->d_coor.alloc(ctx, (size_t)std::max(total, 1LL) * 2);
+  if (rc) return rc;
   if (from_device) {
     // every image's rows in one launch (sources are device blocks of the exchange buffers)
     std::vector<void*> dsts; std::vector<const void*> srcs; std::vector<size_t> sizes;
@@ -827,26 +807,22 @@ static int featureset_build(pano_ctx* ctx, int n_images, const int* n_kp, const 
       dsts.push_back(fs->d_desc + fs->base[i] * 128); srcs.push_back(desc[i]); sizes.push_back((size_t)n_kp[i] * 128 * sizeof(float));
       if (coor && coor[i]) { dsts.push_back(fs->d_coor + fs->base[i] * 2); srcs.push_back(coor[i]); sizes.push_back((size_t)n_kp[i] * 2 * sizeof(double)); }
     }
-    if (ctx_copy_blocks(ctx, (int)dsts.size(), dsts.data(), srcs.data(), sizes.data())) e = cudaErrorUnknown;
+    if ((rc = ctx_copy_blocks(ctx, (int)dsts.size(), dsts.data(), srcs.data(), sizes.data()))) return rc;
+    if ((rc = ctx_put(ctx, fs->d_count, fs->h_count.data(), n_images * sizeof(int)))) return rc;
   } else {
-    for (int i = 0; i < n_images && e == cudaSuccess; ++i) {
+    for (int i = 0; i < n_images; ++i) {
       if (!n_kp[i]) continue;
-      e = cudaMemcpyAsync(fs->d_desc + fs->base[i] * 128, desc[i], (size_t)n_kp[i] * 128 * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
-      if (e == cudaSuccess && coor && coor[i])
-        e = cudaMemcpyAsync(fs->d_coor + fs->base[i] * 2, coor[i], (size_t)n_kp[i] * 2 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
+      PANO_CUDA(ctx, cudaMemcpyAsync(fs->d_desc + fs->base[i] * 128, desc[i], (size_t)n_kp[i] * 128 * sizeof(float),
+                                     cudaMemcpyHostToDevice, ctx->stream));
+      if (coor && coor[i])
+        PANO_CUDA(ctx, cudaMemcpyAsync(fs->d_coor + fs->base[i] * 2, coor[i], (size_t)n_kp[i] * 2 * sizeof(double),
+                                       cudaMemcpyHostToDevice, ctx->stream));
     }
+    PANO_CUDA(ctx, cudaMemcpyAsync(fs->d_count, fs->h_count.data(), n_images * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // sources are pageable host memory
   }
-  if (e == cudaSuccess) {
-    if (from_device) {
-      if (ctx_put(ctx, fs->d_count, fs->h_count.data(), n_images * sizeof(int))) e = cudaErrorUnknown;
-    } else {
-      e = cudaMemcpyAsync(fs->d_count, fs->h_count.data(), n_images * sizeof(int), cudaMemcpyHostToDevice, ctx->stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);  // sources are pageable host memory
-    }
-  }
-  if (e != cudaSuccess) { rc = ctx_cuda(ctx, e, "featureset upload"); featureset_release(fs); return rc; }
   fs->counts_on_host = true;
-  *out = fs;
+  *out = fs.release();
   return PANO_OK;
 }
 
@@ -958,9 +934,9 @@ void pano_featureset_free(pano_featureset* fs) {
 
 struct pano_sift_trace {
   pano_ctx* ctx;
-  SiftWork* wk;
+  std::unique_ptr<SiftWork> wk;
   pano_featureset* fs;
-  void* d_img;
+  DevBuf<unsigned char> d_img;
 };
 
 int pano_sift_trace_run(pano_ctx* ctx, const float* rgb, int w, int h, const pano_params* p, pano_sift_trace** out) {
@@ -968,29 +944,28 @@ int pano_sift_trace_run(pano_ctx* ctx, const float* rgb, int w, int h, const pan
   if (!ctx || !rgb || !p || !out) return PANO_ERR_INVALID;
   *out = nullptr;
   std::vector<const void*> d_imgs;
-  unsigned char* d_block = nullptr;
+  DevBuf<unsigned char> d_block;
   const void* src = rgb;
-  int rc = upload_images(ctx, 1, &src, nullptr, &w, &h, d_imgs, &d_block);
-  if (rc) { ctx_free(ctx, d_block); return rc; }
+  int rc = upload_images(ctx, 1, &src, nullptr, &w, &h, d_imgs, d_block);
+  if (rc) return rc;
   pano_featureset* fs = new pano_featureset;
   fs->ctx = ctx;
-  SiftWork* wk = nullptr;
+  std::unique_ptr<SiftWork> wk;
   // the trace keeps the work buffers of ONE run, so it grows the lists itself
   for (int cap = SIFT_CAP_DEFAULT;; cap *= 2) {
     rc = sift_run_batch(ctx, 1, d_imgs.data(), nullptr, &w, &h, p, fs, &wk, cap);
-    if (rc) { featureset_release(fs); ctx_free(ctx, d_block); return rc; }
+    if (rc) break;
     rc = featureset_sync_counts(fs);
     if (rc == PANO_ERR_CAPACITY && cap < SIFT_CAP_MAX) {
-      sift_work_free(ctx, wk); wk = nullptr;
-      ctx_free(ctx, fs->d_desc); ctx_free(ctx, fs->d_coor); ctx_free(ctx, fs->d_count);
-      fs->d_desc = nullptr; fs->d_coor = nullptr; fs->d_real = nullptr; fs->d_count = nullptr; fs->error = 0;
+      wk.reset();
+      fs->d_desc.reset(); fs->d_coor.reset(); fs->d_count.reset();
+      fs->d_real = nullptr; fs->error = 0;
       continue;
     }
     break;
   }
-  if (rc) { sift_work_free(ctx, wk); featureset_release(fs); ctx_free(ctx, d_block); return rc; }
-  pano_sift_trace* t = new pano_sift_trace{ctx, wk, fs, d_block};
-  *out = t;
+  if (rc) { featureset_release(fs); return rc; }
+  *out = new pano_sift_trace{ctx, std::move(wk), fs, std::move(d_block)};
   return PANO_OK;
 }
 
@@ -1010,7 +985,7 @@ int pano_sift_trace_octave_size(const pano_sift_trace* t, int o, int* w, int* h)
 int pano_sift_trace_plane(pano_sift_trace* t, int kind, int o, int level, float* out) {
   if (t) ctx_enter(t->ctx);
   pano_ctx* ctx = t->ctx;
-  SiftWork* wk = t->wk;
+  SiftWork* wk = t->wk.get();
   if (kind == 0) {
     const ImgMeta& im = wk->h_img[0];
     return pano_dev_download(ctx, out, wk->arena + im.work_off, (size_t)im.w0 * im.h0 * 3 * sizeof(float));
@@ -1044,7 +1019,7 @@ int pano_sift_trace_plane(pano_sift_trace* t, int kind, int o, int level, float*
 int pano_sift_trace_points(pano_sift_trace* t, int stage, int cap, pano_sspoint* out) {
   if (t) ctx_enter(t->ctx);
   pano_ctx* ctx = t->ctx;
-  SiftWork* wk = t->wk;
+  SiftWork* wk = t->wk.get();
   int n_raw = 0, n_desc = t->fs->h_count[0];
   if (pano_dev_download(ctx, &n_raw, wk->cand_count, sizeof(int))) return PANO_ERR_CUDA;
   n_raw = std::min(n_raw, wk->cap);
@@ -1096,9 +1071,7 @@ int pano_sift_trace_descriptors(pano_sift_trace* t, int cap, double* coor_xy, fl
 void pano_sift_trace_free(pano_sift_trace* t) {
   if (t) ctx_enter(t->ctx);
   if (!t) return;
-  sift_work_free(t->ctx, t->wk);
   featureset_release(t->fs);
-  ctx_free(t->ctx, t->d_img);
   delete t;
 }
 

@@ -337,18 +337,12 @@ int pano_rgb8_to_mat32f_batch_dev(pano_ctx* ctx, int n, const unsigned char* con
     jobs[i] = Rgb8Job{d_pix[i], d_out_hwc[i], (long long)w[i] * h[i], channels[i], 0};
     max_px = std::max(max_px, jobs[i].n_px);
   }
-  Rgb8Job* d_jobs = nullptr;
-  if (int rc = ctx_alloc(ctx, (void**)&d_jobs, sizeof(Rgb8Job) * n)) return rc;
-  if (int rc = ctx_put(ctx, d_jobs, jobs.data(), sizeof(Rgb8Job) * n)) { ctx_free(ctx, d_jobs); return rc; }
+  DevBuf<Rgb8Job> d_jobs;
+  if (int rc = d_jobs.alloc(ctx, n)) return rc;
+  if (int rc = ctx_put(ctx, d_jobs, jobs.data(), sizeof(Rgb8Job) * n)) return rc;
   long long per_img = (max_px * 3 / 4 + 255) / 256;
   int gx = (int)std::min<long long>(std::max<long long>(per_img, 1), std::max(1, ctx->num_sms * 8 / n));
-  ctx->launches++;
-  if (ctx->profiling) ctx_prof_begin(ctx, "k_rgb8_to_f32");
-  k_rgb8_to_f32<<<dim3(gx, n), 256, 0, ctx->stream>>>(d_jobs);
-  if (ctx->profiling) ctx_prof_end(ctx);
-  const cudaError_t le = cudaGetLastError();
-  ctx_free(ctx, d_jobs);
-  if (le != cudaSuccess) return ctx_cuda(ctx, le, "k_rgb8_to_f32");
+  PANO_LAUNCH(ctx, "k_rgb8_to_f32", k_rgb8_to_f32, dim3(gx, n), 256, 0, d_jobs);
   return PANO_OK;
 }
 
@@ -364,21 +358,18 @@ int pano_crop_rect_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h, int*
   const int chunks = ceil_div(h, CROP_CHUNK);
   const size_t smem = sizeof(int) * ((size_t)w + 4 * CROP_RUN_CAP + 1);   // l1/l2 of the fallback fit in the run arrays
   if (smem > 200 * 1024) return ctx_fail(ctx, PANO_ERR_INVALID, "pano_crop_rect_dev: width %d exceeds the %d-column limit", w, 40000);
-  unsigned* d_masks = nullptr;
-  int* d_carry = nullptr;
-  CropLineBest* d_best = nullptr;
-  if (int rc = ctx_alloc(ctx, (void**)&d_masks, sizeof(unsigned) * (size_t)chunks * w)) return rc;
-  if (int rc = ctx_alloc(ctx, (void**)&d_carry, sizeof(int) * (size_t)chunks * w)) { ctx_free(ctx, d_masks); return rc; }
-  if (int rc = ctx_alloc(ctx, (void**)&d_best, sizeof(CropLineBest) * (size_t)h)) { ctx_free(ctx, d_masks); ctx_free(ctx, d_carry); return rc; }
+  DevBuf<unsigned> d_masks;
+  DevBuf<int> d_carry;
+  DevBuf<CropLineBest> d_best;
+  if (int rc = d_masks.alloc(ctx, (size_t)chunks * w)) return rc;
+  if (int rc = d_carry.alloc(ctx, (size_t)chunks * w)) return rc;
+  if (int rc = d_best.alloc(ctx, (size_t)h)) return rc;
   if (smem > 48 * 1024)
     PANO_CUDA(ctx, cudaFuncSetAttribute(k_crop_line, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   PANO_LAUNCH(ctx, "k_crop_masks", k_crop_masks, dim3(ceil_div(w, 128), chunks), 128, 0, d_mat_hwc, w, h, d_masks);
   PANO_LAUNCH(ctx, "k_crop_carry", k_crop_carry, ceil_div(w, 128), 128, 0, d_masks, w, chunks, d_carry);
   PANO_LAUNCH(ctx, "k_crop_line", k_crop_line, h, 256, smem, d_masks, d_carry, w, h, d_best);
   PANO_LAUNCH(ctx, "k_crop_final", k_crop_final, 1, 256, 0, d_best, h, d_rect);
-  ctx_free(ctx, d_masks);
-  ctx_free(ctx, d_carry);
-  ctx_free(ctx, d_best);
   return PANO_OK;
 }
 

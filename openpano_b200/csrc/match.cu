@@ -710,51 +710,40 @@ static int build_plan(pano_ctx* ctx, pano_featureset* fs, int n_pairs, const int
 }
 
 struct MatchBuffers {
-  void* tasks = nullptr; PairMeta* pairs = nullptr; SideMeta* sides = nullptr;
-  RowInfo* info = nullptr; TcTop2* approx = nullptr;
-  int2* list = nullptr;        // full re-scan (fallback) list
-  int* counters = nullptr;     // [0] matches, [1..3] fallback rows per round, [4..6] gather blocks per round,
+  DevBuf<unsigned char> tasks; DevBuf<PairMeta> pairs; DevBuf<SideMeta> sides;
+  DevBuf<RowInfo> info; DevBuf<TcTop2> approx;
+  DevBuf<int2> list;           // full re-scan (fallback) list
+  DevBuf<int> counters;        // [0] matches, [1..3] fallback rows per round, [4..6] gather blocks per round,
                                // then side_cnt[round][side]
   int n_counters = 0;
-  int* out = nullptr;
+  DevBuf<int> out;
   // gathered second tensor pass
-  TcGatherSide* gsides = nullptr; int* list_rows = nullptr; TcTask* gtasks = nullptr; unsigned char* gq = nullptr;
-  int2* g_meta = nullptr; int* g_thr = nullptr; int* cand_cnt = nullptr; int* cand = nullptr;
+  DevBuf<TcGatherSide> gsides; DevBuf<int> list_rows; DevBuf<TcTask> gtasks; DevBuf<unsigned char> gq;
+  DevBuf<int2> g_meta; DevBuf<int> g_thr; DevBuf<int> cand_cnt; DevBuf<int> cand;
   // columns on demand: gathered nomination pass over requested rows that are still unknown
-  int* list_unknown = nullptr; TcTask* ntasks = nullptr; unsigned char* nq = nullptr; int2* n_meta = nullptr;
-  TcTop2* n_approx = nullptr;
+  DevBuf<int> list_unknown; DevBuf<TcTask> ntasks; DevBuf<unsigned char> nq; DevBuf<int2> n_meta;
+  DevBuf<TcTop2> n_approx;
   int rounds = 2;              // gather rounds run (the decide after the last one must leave nothing pending)
 };
 
-static void free_buffers(pano_ctx* ctx, MatchBuffers& b, bool keep_out) {
-  ctx_free(ctx, b.tasks); ctx_free(ctx, b.pairs); ctx_free(ctx, b.sides); ctx_free(ctx, b.info);
-  ctx_free(ctx, b.approx); ctx_free(ctx, b.list);
-  ctx_free(ctx, b.gsides); ctx_free(ctx, b.list_rows); ctx_free(ctx, b.gtasks); ctx_free(ctx, b.gq);
-  ctx_free(ctx, b.g_meta); ctx_free(ctx, b.g_thr); ctx_free(ctx, b.cand_cnt); ctx_free(ctx, b.cand);
-  ctx_free(ctx, b.list_unknown); ctx_free(ctx, b.ntasks); ctx_free(ctx, b.nq); ctx_free(ctx, b.n_meta);
-  ctx_free(ctx, b.n_approx);
-  if (!keep_out) { ctx_free(ctx, b.out); ctx_free(ctx, b.counters); b.out = nullptr; b.counters = nullptr; }
-}
-
-// Runs the plan; leaves per-row decisions in b.out and counters in b.counters (caller frees both).
+// Runs the plan; leaves per-row decisions in b.out and counters in b.counters.
 static int run_plan(pano_ctx* ctx, pano_featureset* fs, const MatchPlan& pl, float ratio, bool tensor,
                     const TcOperands* ops, MatchBuffers& b) {
   int rc = 0;
   const size_t bt = tensor ? pl.tc_tasks.size() * sizeof(TcTask) : pl.exact_tasks.size() * sizeof(MatchTask);
   const size_t bp = pl.pairs.size() * sizeof(PairMeta), bs = pl.sides.size() * sizeof(SideMeta);
   const long long nres = std::max<long long>(pl.res_total, 1);
-  if ((rc = ctx_alloc(ctx, &b.tasks, bt)) || (rc = ctx_alloc(ctx, (void**)&b.pairs, bp)) ||
-      (rc = ctx_alloc(ctx, (void**)&b.sides, bs)) || (rc = ctx_alloc(ctx, (void**)&b.info, nres * sizeof(RowInfo))) ||
-      (rc = ctx_alloc(ctx, (void**)&b.approx, nres * std::max(pl.parts, 1) * sizeof(TcTop2))) ||
-      (rc = ctx_alloc(ctx, (void**)&b.list, nres * sizeof(int2))) ||
-      (rc = ctx_alloc(ctx, (void**)&b.out, std::max<long long>(pl.out_total, 1) * sizeof(int))))
+  if ((rc = b.tasks.alloc(ctx, bt)) || (rc = b.pairs.alloc(ctx, pl.pairs.size())) ||
+      (rc = b.sides.alloc(ctx, pl.sides.size())) || (rc = b.info.alloc(ctx, nres)) ||
+      (rc = b.approx.alloc(ctx, nres * std::max(pl.parts, 1))) || (rc = b.list.alloc(ctx, nres)) ||
+      (rc = b.out.alloc(ctx, std::max<long long>(pl.out_total, 1))))
     return rc;
   const int n_sides = (int)pl.sides.size();
   b.n_counters = MC_HEAD + MC_ROUNDS * 2 * n_sides;
-  if ((rc = ctx_alloc(ctx, (void**)&b.counters, b.n_counters * sizeof(int)))) return rc;
+  if ((rc = b.counters.alloc(ctx, b.n_counters))) return rc;
   const void* tsrc = tensor ? (const void*)pl.tc_tasks.data() : (const void*)pl.exact_tasks.data();
   const size_t bg = tensor ? pl.gsides.size() * sizeof(TcGatherSide) : 0;
-  if (bg && (rc = ctx_alloc(ctx, (void**)&b.gsides, bg))) return rc;
+  if (bg && (rc = b.gsides.alloc(ctx, pl.gsides.size()))) return rc;
   {
     // plan tables + counter reset in one launch
     void* dsts[5] = {b.tasks, b.pairs, b.sides, b.counters, b.gsides};
@@ -774,15 +763,15 @@ static int run_plan(pano_ctx* ctx, pano_featureset* fs, const MatchPlan& pl, flo
     }
     if (!pl.exact_tasks.empty())
       PANO_LAUNCH(ctx, "k_match_top2", k_match_top2, (unsigned)pl.exact_tasks.size(), MT_THREADS, smem, fs->d_desc,
-                  (const MatchTask*)b.tasks, b.info);
+                  (const MatchTask*)b.tasks.get(), b.info);
     if (pl.max_small > 0) {
-      if ((rc = ctx_alloc(ctx, (void**)&b.list_rows, nres * sizeof(int)))) return rc;
+      if ((rc = b.list_rows.alloc(ctx, nres))) return rc;
       PANO_LAUNCH(ctx, "k_match_decide", k_match_decide, gd, 256, 0, b.pairs, n_pairs, b.sides, b.info, rs, 1, b.out,
                   b.counters, b.list_rows, b.list_rows, b.counters + MC_HEAD, n_sides);
     }
     return PANO_OK;
   }
-  rc = tc_run_top2(ctx, ops, (const TcTask*)b.tasks, (int)pl.tc_tasks.size(), b.approx);
+  rc = tc_run_top2(ctx, ops, (const TcTask*)b.tasks.get(), (int)pl.tc_tasks.size(), b.approx);
   if (rc) return rc;
   if (pl.max_side_n > 0) {
     dim3 gr(ceil_div(pl.max_side_n, 128), grid_y(n_sides));
@@ -801,13 +790,10 @@ static int run_plan(pano_ctx* ctx, pano_featureset* fs, const MatchPlan& pl, flo
     if (const char* e = getenv("PANO_MATCH_BLOCK_CAP")) block_cap = std::max(1, std::min(block_cap, atoi(e)));   // test hook: force the full re-scan fallback
     const size_t grow = (size_t)block_cap * 128;
     TcFilter f;
-    if ((rc = ctx_alloc(ctx, (void**)&b.list_rows, nres * sizeof(int))) ||
-        (rc = ctx_alloc(ctx, (void**)&b.gtasks, (size_t)block_cap * sizeof(TcTask))) ||
-        (rc = ctx_alloc(ctx, (void**)&b.gq, (size_t)block_cap * tc_block_bytes())) ||
-        (rc = ctx_alloc(ctx, (void**)&b.g_meta, grow * sizeof(int2))) ||
-        (rc = ctx_alloc(ctx, (void**)&b.g_thr, grow * sizeof(int))) ||
-        (rc = ctx_alloc(ctx, (void**)&b.cand_cnt, grow * sizeof(int))) ||
-        (rc = ctx_alloc(ctx, (void**)&b.cand, grow * TC_CAND_CAP * sizeof(int))))
+    if ((rc = b.list_rows.alloc(ctx, nres)) || (rc = b.gtasks.alloc(ctx, block_cap)) ||
+        (rc = b.gq.alloc(ctx, (size_t)block_cap * tc_block_bytes())) || (rc = b.g_meta.alloc(ctx, grow)) ||
+        (rc = b.g_thr.alloc(ctx, grow)) || (rc = b.cand_cnt.alloc(ctx, grow)) ||
+        (rc = b.cand.alloc(ctx, grow * TC_CAND_CAP)))
       return rc;
     f.gq = b.gq; f.tasks = b.gtasks; f.gsides = b.gsides; f.list_rows = b.list_rows; f.approx = b.approx;
     f.g_meta = b.g_meta; f.g_thr = b.g_thr; f.cand_cnt = b.cand_cnt; f.cand = b.cand;
@@ -817,11 +803,9 @@ static int run_plan(pano_ctx* ctx, pano_featureset* fs, const MatchPlan& pl, flo
     if (pl.lazy) {
       nom_cap = (int)std::min<long long>(std::max<long long>(pl.large_blocks, 1), 8192);
       const size_t nrow = (size_t)nom_cap * 128;
-      if ((rc = ctx_alloc(ctx, (void**)&b.list_unknown, nres * sizeof(int))) ||
-          (rc = ctx_alloc(ctx, (void**)&b.ntasks, (size_t)nom_cap * sizeof(TcTask))) ||
-          (rc = ctx_alloc(ctx, (void**)&b.nq, (size_t)nom_cap * tc_block_bytes())) ||
-          (rc = ctx_alloc(ctx, (void**)&b.n_meta, nrow * sizeof(int2))) ||
-          (rc = ctx_alloc(ctx, (void**)&b.n_approx, nrow * sizeof(TcTop2))))
+      if ((rc = b.list_unknown.alloc(ctx, nres)) || (rc = b.ntasks.alloc(ctx, nom_cap)) ||
+          (rc = b.nq.alloc(ctx, (size_t)nom_cap * tc_block_bytes())) || (rc = b.n_meta.alloc(ctx, nrow)) ||
+          (rc = b.n_approx.alloc(ctx, nrow)))
         return rc;
       nf.gq = b.nq; nf.tasks = b.ntasks; nf.gsides = b.gsides; nf.list_rows = b.list_unknown; nf.approx = nullptr;
       nf.g_meta = b.n_meta; nf.g_thr = nullptr; nf.cand_cnt = nullptr; nf.cand = nullptr;
@@ -905,32 +889,26 @@ int pano_match_pairs_shard(pano_ctx* ctx, pano_featureset* fs, int n_pairs, cons
   MatchPlan pl;
   MatchBuffers b;
   int rc = match_common(ctx, fs, n_pairs, ij, p, shard, n_shards, pl, b);
-  if (rc) { free_buffers(ctx, b, false); return rc; }
+  if (rc) return rc;
   // count -> offsets -> ordered compaction on the device; one read-back of header + matches
   const size_t n_hdr = 3 + 2 * (size_t)n_pairs;
   const size_t cap = (size_t)std::max<long long>(pl.out_total, 1) * 2;
-  int *d_hdr = nullptr, *d_dense = nullptr;
-  if ((rc = ctx_alloc(ctx, (void**)&d_hdr, n_hdr * sizeof(int))) || (rc = ctx_alloc(ctx, (void**)&d_dense, cap * sizeof(int)))) {
-    ctx_free(ctx, d_hdr); ctx_free(ctx, d_dense); free_buffers(ctx, b, false); return rc;
-  }
+  DevBuf<int> d_hdr, d_dense;
+  if ((rc = d_hdr.alloc(ctx, n_hdr)) || (rc = d_dense.alloc(ctx, cap))) return rc;
   int* h_stage = (int*)ctx_ring(ctx, (n_hdr + cap) * sizeof(int));
-  if (!h_stage) { ctx_free(ctx, d_hdr); ctx_free(ctx, d_dense); free_buffers(ctx, b, false); return ctx_fail(ctx, PANO_ERR_CUDA, "pinned ring allocation failed"); }
-  auto finish = [&](int code) { ctx_free(ctx, d_hdr); ctx_free(ctx, d_dense); free_buffers(ctx, b, false); return code; };
-  if ((rc = ctx_zero(ctx, d_hdr, 2 * sizeof(int)))) return finish(rc);
+  if (!h_stage) return ctx_fail(ctx, PANO_ERR_CUDA, "pinned ring allocation failed");
+  if ((rc = ctx_zero(ctx, d_hdr, 2 * sizeof(int)))) return rc;
   if (n_pairs > 0) {
-    ctx->launches += 4;
-    k_match_count<<<n_pairs, 256, 0, ctx->stream>>>(b.pairs, b.out, n_pairs, d_hdr);
-    k_match_offsets<<<1, 1024, 0, ctx->stream>>>(n_pairs, d_hdr);
-    k_match_write<<<n_pairs, 256, 0, ctx->stream>>>(b.pairs, b.out, n_pairs, d_hdr, d_dense);
-    k_match_download<<<std::max(1, std::min(ctx->num_sms, (int)(cap / 4096) + 1)), 256, 0, ctx->stream>>>(h_stage + n_hdr, d_dense, d_hdr);
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return finish(ctx_cuda(ctx, le, "match result compaction"));
+    PANO_LAUNCH(ctx, "k_match_count", k_match_count, n_pairs, 256, 0, b.pairs, b.out, n_pairs, d_hdr);
+    PANO_LAUNCH(ctx, "k_match_offsets", k_match_offsets, 1, 1024, 0, n_pairs, d_hdr);
+    PANO_LAUNCH(ctx, "k_match_write", k_match_write, n_pairs, 256, 0, b.pairs, b.out, n_pairs, d_hdr, d_dense);
+    PANO_LAUNCH(ctx, "k_match_download", k_match_download, std::max(1, std::min(ctx->num_sms, (int)(cap / 4096) + 1)), 256, 0,
+                h_stage + n_hdr, d_dense, d_hdr);
   }
   rc = ctx_store(ctx, h_stage, d_hdr, n_hdr * sizeof(int));
   cudaError_t e = ctx_spin_stream(ctx);
-  if (rc) return finish(rc);
-  if (e != cudaSuccess) return finish(ctx_cuda(ctx, e, "match download"));
-  finish(0);
+  if (rc) return rc;
+  if (e != cudaSuccess) return ctx_cuda(ctx, e, "match download");
   if (n_pairs > 0 && h_stage[1] != 0) return ctx_fail(ctx, PANO_ERR_CUDA, "match: %d undecided rows (internal error)", h_stage[1]);
   const int total = n_pairs > 0 ? h_stage[0] : 0;
   out->n_pairs = n_pairs;
@@ -963,13 +941,12 @@ int pano_match_pairs_dev_shard(pano_ctx* ctx, pano_featureset* fs, int n_pairs, 
   MatchPlan pl;
   MatchBuffers b;
   int rc = match_common(ctx, fs, n_pairs, ij, p, shard, n_shards, pl, b);
-  if (rc) { free_buffers(ctx, b, false); return rc; }
+  if (rc) return rc;
   int* h = (int*)ctx_ring(ctx, (size_t)std::max(b.n_counters, MC_HEAD) * sizeof(int));
-  if (!h) { free_buffers(ctx, b, false); return ctx_fail(ctx, PANO_ERR_CUDA, "pinned ring allocation failed"); }
+  if (!h) return ctx_fail(ctx, PANO_ERR_CUDA, "pinned ring allocation failed");
   const int n_counters = b.n_counters, n_sides = (int)pl.sides.size(), rounds = b.rounds;
   rc = b.counters ? ctx_store(ctx, h, b.counters, (size_t)n_counters * sizeof(int)) : 0;
   cudaError_t e = ctx_spin_stream(ctx);
-  free_buffers(ctx, b, false);
   if (rc) return rc;
   if (e != cudaSuccess) return ctx_cuda(ctx, e, "match total download");
   if (n_counters < MC_HEAD) { *total_matches = 0; return PANO_OK; }

@@ -420,11 +420,10 @@ int tc_prepare(pano_ctx* ctx, const float* d_desc, const std::vector<TcImage>& i
   int max_pad = 0;
   for (auto& im : imgs) { rows = std::max<long long>(rows, im.row0 + im.n); blocks = std::max<long long>(blocks, im.blk0 + im.n_pad / 128); max_pad = std::max(max_pad, im.n_pad); }
   int rc = 0;
-  if ((rc = ctx_alloc(ctx, (void**)&ops->d_imgs, n * sizeof(TcImage))) ||
-      (rc = ctx_alloc(ctx, (void**)&ops->d_norms, std::max<long long>(rows, 1) * sizeof(float))) ||
-      (rc = ctx_alloc(ctx, (void**)&ops->d_maxnorm, sizeof(unsigned))) ||
-      (rc = ctx_alloc(ctx, (void**)&ops->qbuf, (size_t)std::max<long long>(blocks, 1) * TC_BLOCK_BYTES)) ||
-      (rc = ctx_alloc(ctx, (void**)&ops->tbuf, (size_t)std::max<long long>(blocks, 1) * TC_BLOCK_BYTES)))
+  if ((rc = ops->d_imgs.alloc(ctx, n)) || (rc = ops->d_norms.alloc(ctx, std::max<long long>(rows, 1))) ||
+      (rc = ops->d_maxnorm.alloc(ctx, 1)) ||
+      (rc = ops->qbuf.alloc(ctx, (size_t)std::max<long long>(blocks, 1) * TC_BLOCK_BYTES)) ||
+      (rc = ops->tbuf.alloc(ctx, (size_t)std::max<long long>(blocks, 1) * TC_BLOCK_BYTES)))
     return rc;
   if ((rc = ctx_put(ctx, ops->d_imgs, imgs.data(), n * sizeof(TcImage)))) return rc;
   if ((rc = ctx_zero(ctx, ops->d_maxnorm, sizeof(unsigned)))) return rc;
@@ -433,12 +432,6 @@ int tc_prepare(pano_ctx* ctx, const float* d_desc, const std::vector<TcImage>& i
   PANO_LAUNCH(ctx, "k_tc_maxnorm", k_tc_maxnorm, g1, 128, 0, d_desc, ops->d_imgs, n, ops->d_norms, ops->d_maxnorm);
   PANO_LAUNCH(ctx, "k_tc_prep", k_tc_prep, g1, 128, 0, d_desc, ops->d_norms, ops->d_maxnorm, ops->d_imgs, ops->qbuf, ops->tbuf);
   return PANO_OK;
-}
-
-void tc_release(pano_ctx* ctx, TcOperands* ops) {
-  ctx_free(ctx, ops->d_imgs); ctx_free(ctx, ops->d_norms); ctx_free(ctx, ops->d_maxnorm);
-  ctx_free(ctx, ops->qbuf); ctx_free(ctx, ops->tbuf);
-  *ops = TcOperands();
 }
 
 // function attributes are per DEVICE: one process may hold contexts on several GPUs

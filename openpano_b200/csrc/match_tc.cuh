@@ -47,15 +47,14 @@ struct TcFilter {       // device buffers of one gathered pass
 };
 
 struct TcOperands {
-  TcImage* d_imgs = nullptr;
-  float* d_norms = nullptr;        // |x|^2 per descriptor row (f32)
-  unsigned* d_maxnorm = nullptr;   // bits of max |x|^2
-  unsigned char* qbuf = nullptr;   // query-form fp16 blocks
-  unsigned char* tbuf = nullptr;   // target-form fp16 blocks
+  DevBuf<TcImage> d_imgs;
+  DevBuf<float> d_norms;           // |x|^2 per descriptor row (f32)
+  DevBuf<unsigned> d_maxnorm;      // bits of max |x|^2
+  DevBuf<unsigned char> qbuf;      // query-form fp16 blocks
+  DevBuf<unsigned char> tbuf;      // target-form fp16 blocks
 };
 
 int  tc_prepare(pano_ctx* ctx, const float* d_desc, const std::vector<TcImage>& imgs, TcOperands* ops);
-void tc_release(pano_ctx* ctx, TcOperands* ops);
 int  tc_run_top2(pano_ctx* ctx, const TcOperands* ops, const TcTask* d_tasks, int n_tasks, TcTop2* d_res);
 int  tc_run_filter(pano_ctx* ctx, const TcOperands* ops, const TcFilter* f, int max_blocks);
 int  tc_run_nominate(pano_ctx* ctx, const TcOperands* ops, const TcFilter* f, int max_blocks, TcTop2* d_res);

@@ -101,21 +101,15 @@ int pano_planet(pano_ctx* ctx, const float* rgb_hwc, int w, int h, float* out_hw
   if (!ctx) return PANO_ERR_INVALID;
   if (!rgb_hwc || !out_hwc || w < 1 || h < 1)
     return ctx_fail(ctx, PANO_ERR_INVALID, "planet: null pointer or empty %dx%d input", w, h);
-  const size_t bs = (size_t)w * h * 3 * sizeof(float), bd = kPixels * 3 * sizeof(float);
-  float *d_src = nullptr, *d_dst = nullptr;
+  const size_t ns = (size_t)w * h * 3, nd = (size_t)kPixels * 3;
+  DevBuf<float> d_src, d_dst;
   int rc = 0;
-  if ((rc = ctx_alloc(ctx, (void**)&d_src, bs)) || (rc = ctx_alloc(ctx, (void**)&d_dst, bd))) {
-    ctx_free(ctx, d_src); ctx_free(ctx, d_dst);
-    return rc;
-  }
-  cudaError_t e = cudaMemcpyAsync(d_src, rgb_hwc, bs, cudaMemcpyHostToDevice, ctx->stream);
-  if (e != cudaSuccess) rc = ctx_cuda(ctx, e, "planet upload");
-  if (!rc) rc = pano_planet_dev(ctx, d_src, w, h, d_dst);
-  if (!rc && (e = cudaMemcpyAsync(out_hwc, d_dst, bd, cudaMemcpyDeviceToHost, ctx->stream)) != cudaSuccess)
-    rc = ctx_cuda(ctx, e, "planet download");
-  if (!rc && (e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess) rc = ctx_cuda(ctx, e, "pano_planet");
-  ctx_free(ctx, d_src); ctx_free(ctx, d_dst);
-  return rc;
+  if ((rc = d_src.alloc(ctx, ns)) || (rc = d_dst.alloc(ctx, nd))) return rc;
+  PANO_CUDA(ctx, cudaMemcpyAsync(d_src, rgb_hwc, ns * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = pano_planet_dev(ctx, d_src, w, h, d_dst))) return rc;
+  PANO_CUDA(ctx, cudaMemcpyAsync(out_hwc, d_dst, nd * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+  PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return PANO_OK;
 }
 
 }  // extern "C"

@@ -118,30 +118,22 @@ extern "C" int pano_ransac_score_pairs(pano_ctx* ctx, int n_pairs, const pano_ra
     if (p.n_hyp) memcpy(sh + meta[k].hyp_off * 9, p.homos, (size_t)p.n_hyp * 72);
   }
   memcpy(st + 2 * b_kp + b_h, meta.data(), b_meta);
-  char* d_in = nullptr; char* d_out = nullptr;
-  int rc = ctx_alloc(ctx, (void**)&d_in, 2 * b_kp + b_h + b_meta + 64);
-  if (!rc) rc = ctx_alloc(ctx, (void**)&d_out, b_out + 64);
-  if (rc) { ctx_free(ctx, d_in); ctx_free(ctx, d_out); return rc; }
-  cudaError_t e = cudaMemcpyAsync(d_in, st, 2 * b_kp + b_h + b_meta, cudaMemcpyHostToDevice, ctx->stream);
-  const double2* d_kp1 = (const double2*)d_in; const double2* d_kp2 = (const double2*)(d_in + b_kp);
+  DevBuf<char> d_in, d_out;
+  int rc = d_in.alloc(ctx, 2 * b_kp + b_h + b_meta + 64);
+  if (!rc) rc = d_out.alloc(ctx, b_out + 64);
+  if (rc) return rc;
+  PANO_CUDA(ctx, cudaMemcpyAsync(d_in, st, 2 * b_kp + b_h + b_meta, cudaMemcpyHostToDevice, ctx->stream));
+  const double2* d_kp1 = (const double2*)d_in.get(); const double2* d_kp2 = (const double2*)(d_in + b_kp);
   const double* d_h = (const double*)(d_in + 2 * b_kp);
   const RansacPair* d_meta = (const RansacPair*)(d_in + 2 * b_kp + b_h);
-  int* d_counts = (int*)d_out; int* d_best = d_counts + nh; int* d_bcnt = d_best + n_pairs;
+  int* d_counts = (int*)d_out.get(); int* d_best = d_counts + nh; int* d_bcnt = d_best + n_pairs;
   unsigned char* d_flags = (unsigned char*)(d_bcnt + n_pairs);
-  if (e == cudaSuccess) {
-    ctx->launches += 2;
-    if (ctx->profiling) ctx_prof_begin(ctx, "k_ransac_count");
-    dim3 grid((unsigned)std::max(1, std::min((max_hyp + 7) / 8, 64)), grid_y(n_pairs));
-    k_ransac_count<<<grid, 256, 0, ctx->stream>>>(d_meta, n_pairs, d_kp1, d_kp2, d_h, d_counts);
-    if (ctx->profiling) { ctx_prof_end(ctx); ctx_prof_begin(ctx, "k_ransac_select"); }
-    k_ransac_select<<<n_pairs, 256, 0, ctx->stream>>>(d_meta, d_kp1, d_kp2, d_h, d_counts, d_best, d_bcnt, d_flags);
-    if (ctx->profiling) ctx_prof_end(ctx);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(so, d_out, b_out, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  ctx_free(ctx, d_in); ctx_free(ctx, d_out);
-  if (e != cudaSuccess) return ctx_cuda(ctx, e, "ransac scoring");
+  dim3 grid((unsigned)std::max(1, std::min((max_hyp + 7) / 8, 64)), grid_y(n_pairs));
+  PANO_LAUNCH(ctx, "k_ransac_count", k_ransac_count, grid, 256, 0, d_meta, n_pairs, d_kp1, d_kp2, d_h, d_counts);
+  PANO_LAUNCH(ctx, "k_ransac_select", k_ransac_select, n_pairs, 256, 0, d_meta, d_kp1, d_kp2, d_h, d_counts, d_best, d_bcnt,
+              d_flags);
+  PANO_CUDA(ctx, cudaMemcpyAsync(so, d_out, b_out, cudaMemcpyDeviceToHost, ctx->stream));
+  PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   const int* h_counts = (const int*)so;
   const int* h_best = h_counts + nh;
   const int* h_bcnt = h_best + n_pairs;

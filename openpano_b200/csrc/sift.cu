@@ -1120,16 +1120,6 @@ int host_gauss_kernel(float sigma, int window_factor, float* taps, int cap) {
   return kw;
 }
 
-void sift_work_free(pano_ctx* ctx, SiftWork* wk) {
-  if (!wk) return;
-  ctx_free(ctx, wk->arena); ctx_free(ctx, wk->d_img); ctx_free(ctx, wk->d_oct); ctx_free(ctx, wk->d_maps); ctx_free(ctx, wk->d_tilespan);
-  ctx_free(ctx, wk->cand_count); ctx_free(ctx, wk->cand_keys); ctx_free(ctx, wk->seam_keys); ctx_free(ctx, wk->sorted_keys);
-  ctx_free(ctx, wk->refined); ctx_free(ctx, wk->kp_valid); ctx_free(ctx, wk->npeaks);
-  ctx_free(ctx, wk->dirs); ctx_free(ctx, wk->n_refined);
-  ctx_free(ctx, wk->desc_cand); ctx_free(ctx, wk->desc_dir);
-  delete wk;
-}
-
 // cuTensorMapEncodeTiled through the runtime's driver-entry-point lookup: the library links
 // cudart statically and has no link-time dependency on libcuda.
 typedef CUresult (*tma_encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -1159,12 +1149,6 @@ int ctx_tma_encode(pano_ctx* ctx, TmaDesc* out, void* base, int rank, const unsi
   return PANO_OK;
 }
 
-void sift_plan_free(pano_ctx* ctx, SiftPlan* plan) {
-  if (!plan) return;
-  sift_work_free(ctx, plan->wk);
-  delete plan;
-}
-
 // Everything that shapes a plan: its layout, tables and kernel arguments all follow from these.
 static std::vector<int> sift_plan_key(int n, const int* channels, const int* w, const int* h, const pano_params* p,
                                       int cap) {
@@ -1184,11 +1168,12 @@ static std::vector<int> sift_plan_key(int n, const int* channels, const int* w, 
   return key;
 }
 
-static int plan_alloc(pano_ctx* ctx, SiftPlan* plan, void** q, size_t bytes) {
-  const int rc = ctx_alloc(ctx, q, bytes);
+template <class T>
+static int plan_alloc(pano_ctx* ctx, SiftPlan* plan, DevBuf<T>& buf, size_t count) {
+  const int rc = buf.alloc(ctx, count);
   if (rc == PANO_OK) {
-    auto f = ctx->live.find(*q);   // a cached block may be larger than asked for
-    plan->bytes += f != ctx->live.end() ? f->second : bytes;
+    auto f = ctx->live.find(buf.get());   // a cached block may be larger than asked for
+    plan->bytes += f != ctx->live.end() ? f->second : count * sizeof(T);
   }
   return rc;
 }
@@ -1207,7 +1192,7 @@ static cudaError_t sift_smem_limit(pano_ctx* ctx, const void* fn, size_t bytes) 
 }
 
 int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w, const int* h,
-                   const pano_params* p, pano_featureset* fs, SiftWork** keep, int cap) {
+                   const pano_params* p, pano_featureset* fs, std::unique_ptr<SiftWork>* keep, int cap) {
   if (n <= 0 || !d_src || !w || !h || !p || !fs) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: bad argument");
   if (n > SIFT_MAX_IMG) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: %d images in one batch (limit %d): split the batch", n, SIFT_MAX_IMG);
   const int n_oct = p->num_octave, n_scale = p->num_scale;
@@ -1234,24 +1219,21 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
   // Reusing the buffers is safe in stream order only: every reader of the scratch buffers is a kernel of
   // one batch on ctx->stream, queued before the next batch's metadata upload overwrites them.
   std::vector<int> key = sift_plan_key(n, channels, w, h, p, cap);
-  SiftPlan* plan = nullptr;
+  std::unique_ptr<SiftPlan> plan;
   if (!keep) {
-    plan = ctx->sift_plan;
+    plan.reset(ctx->sift_plan);
     ctx->sift_plan = nullptr;
     ctx->sift_plan_bytes = 0;
-    if (plan && plan->key != key) { sift_plan_free(ctx, plan); plan = nullptr; }
+    if (plan && plan->key != key) plan.reset();
   }
   const bool fresh = plan == nullptr;
 
-#define SIFT_FAIL(...) do { sift_plan_free(ctx, plan); return ctx_fail(ctx, __VA_ARGS__); } while (0)
-#define SIFT_TRY(call) do { int _rc = (call); if (_rc != 0) { sift_plan_free(ctx, plan); return _rc; } } while (0)
-#define SIFT_CUDA(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { int _rc = ctx_cuda(ctx, _e, #call); sift_plan_free(ctx, plan); return _rc; } } while (0)
-
   std::vector<int2> tilespan;     // uploaded when the plan is built
   if (fresh) {
-    plan = new SiftPlan;
+    plan.reset(new SiftPlan);
     plan->key = std::move(key);
-    SiftWork* wk = plan->wk = new SiftWork;
+    plan->wk.reset(new SiftWork);
+    SiftWork* wk = plan->wk.get();
     wk->n_img = n; wk->n_oct = n_oct; wk->n_scale = n_scale; wk->cap = cap;
     wk->h_img.resize(n);
     wk->h_oct.resize((size_t)n * n_oct);
@@ -1261,16 +1243,16 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
     size_t seam_cap = 0;            // most tile-perimeter (pixel, scale) pairs of one image
     tilespan.resize((size_t)n * n_oct);
     for (int i = 0; i < n; ++i) {
-      if (w[i] < 2 || h[i] < 2) SIFT_FAIL(PANO_ERR_INVALID, "sift: image too small");
+      if (w[i] < 2 || h[i] < 2) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: image too small");
       if (channels && (channels[i] != 1 && channels[i] != 3))
-        SIFT_FAIL(PANO_ERR_INVALID, "sift: image %d has %d channels (1 or 3)", i, channels[i]);
+        return ctx_fail(ctx, PANO_ERR_INVALID, "sift: image %d has %d channels (1 or 3)", i, channels[i]);
       ImgMeta& im = wk->h_img[i];
       im.channels = channels ? channels[i] : 3;
       im.in_w = w[i]; im.in_h = h[i];
       // feature/feature.cc:33-34
       float ratio = p->sift_working_size * 2.0f / (w[i] + h[i]);
       im.h0 = (int)(h[i] * ratio); im.w0 = (int)(w[i] * ratio);
-      if (im.w0 < 8 || im.h0 < 8 || im.w0 > 8191 || im.h0 > 8191) SIFT_FAIL(PANO_ERR_INVALID, "sift: working size out of range");
+      if (im.w0 < 8 || im.h0 < 8 || im.w0 > 8191 || im.h0 > 8191) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: working size out of range");
       float fx = (float)im.h0 / h[i], fy = (float)im.w0 / w[i];
       im.ifx = 1.f / fx; im.ify = 1.f / fy;
       im.work_off = (long long)off;
@@ -1284,7 +1266,7 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
         else {  // feature/dog.cc:105-107
           float factor = (float)pow((double)p->scale_factor, (double)-o);
           om.w = (int)ceilf(im.w0 * factor); om.h = (int)ceilf(im.h0 * factor);
-          if (om.w <= 5 || om.h <= 5) SIFT_FAIL(PANO_ERR_INVALID, "sift: octave too small");
+          if (om.w <= 5 || om.h <= 5) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: octave too small");
           float ofx = (float)om.h / im.h0, ofy = (float)om.w / im.w0;
           om.ifx = 1.f / ofx; om.ify = 1.f / ofy;
         }
@@ -1309,7 +1291,7 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
       float sigma = p->gauss_sigma;  // feature/gaussian.hh:99-102
       for (int s = 0; s < gt.nlev; ++s) {
         int kw = host_gauss_kernel(sigma, p->gauss_window_factor, gt.taps[s], SIFT_MAX_TAPS);
-        if (kw < 0) SIFT_FAIL(PANO_ERR_INVALID, "sift: gaussian window %d too wide", -kw);
+        if (kw < 0) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: gaussian window %d too wide", -kw);
         gt.center[s] = kw / 2;
         gt.rmax = std::max(gt.rmax, kw / 2);
         sigma *= p->scale_factor;
@@ -1319,27 +1301,27 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
     for (int s = 0; s < gt.nlev; ++s) plan->fast = plan->fast && (gt.center[s] == 3 || gt.center[s] == 6);
     const int R = gt.rmax;
     if (((size_t)(BT_H + 2 * R) * (BT_W + 2 * R) + (size_t)BT_H * (BT_W + 2 * R)) * sizeof(float) > 200 * 1024)
-      SIFT_FAIL(PANO_ERR_INVALID, "sift: blur halo too large");
+      return ctx_fail(ctx, PANO_ERR_INVALID, "sift: blur halo too large");
 
     const size_t nlist = (size_t)n * cap;
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->arena, off * sizeof(float)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->d_img, n * sizeof(ImgMeta)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->d_oct, wk->h_oct.size() * sizeof(OctMeta)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->d_maps, (size_t)n * n_oct * sizeof(TmaDesc)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->d_tilespan, tilespan.size() * sizeof(int2)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->cand_count, (2 * n + 2) * sizeof(int)));   // [n], [n+1] = work counters, then seam counts
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->seam_keys, (size_t)n * seam_cap * sizeof(uint32_t)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->cand_keys, nlist * sizeof(uint32_t)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->sorted_keys, nlist * sizeof(uint32_t)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->refined, nlist * sizeof(pano_sspoint)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->kp_valid, nlist));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->npeaks, nlist * sizeof(int)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->dirs, nlist * SIFT_MAX_PEAKS * sizeof(float)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->n_refined, n * sizeof(int)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->desc_cand, nlist * sizeof(int)));
-    SIFT_TRY(plan_alloc(ctx, plan, (void**)&wk->desc_dir, nlist * sizeof(float)));
+    if (int rc = plan_alloc(ctx, plan.get(), wk->arena, off)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->d_img, n)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->d_oct, wk->h_oct.size())) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->d_maps, (size_t)n * n_oct)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->d_tilespan, tilespan.size())) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->cand_count, 2 * n + 2)) return rc;   // [n], [n+1] = work counters, then seam counts
+    if (int rc = plan_alloc(ctx, plan.get(), wk->seam_keys, (size_t)n * seam_cap)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->cand_keys, nlist)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->sorted_keys, nlist)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->refined, nlist)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->kp_valid, nlist)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->npeaks, nlist)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->dirs, nlist * SIFT_MAX_PEAKS)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->n_refined, n)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->desc_cand, nlist)) return rc;
+    if (int rc = plan_alloc(ctx, plan.get(), wk->desc_dir, nlist)) return rc;
   }
-  SiftWork* wk = plan->wk;
+  SiftWork* wk = plan->wk.get();
   const GaussTable& gt = plan->gt;
   const bool fast = plan->fast;
   const size_t seam_cap = plan->seam_cap;
@@ -1352,10 +1334,10 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
   const size_t nlist = (size_t)n * cap;
   const int n_om = n * n_oct;
   fs->ctx = ctx; fs->n_images = n; fs->cap = cap;
-  SIFT_TRY(ctx_alloc(ctx, (void**)&fs->d_desc, nlist * 128 * sizeof(float)));
-  SIFT_TRY(ctx_alloc(ctx, (void**)&fs->d_coor, nlist * 4 * sizeof(double)));   // scaled coordinates, then real_coor
+  if (int rc = fs->d_desc.alloc(ctx, nlist * 128)) return rc;
+  if (int rc = fs->d_coor.alloc(ctx, nlist * 4)) return rc;   // scaled coordinates, then real_coor
   fs->d_real = fs->d_coor + nlist * 2;
-  SIFT_TRY(ctx_alloc(ctx, (void**)&fs->d_count, n * sizeof(int)));
+  if (int rc = fs->d_count.alloc(ctx, n)) return rc;
   fs->base.resize(n);
   for (int i = 0; i < n; ++i) fs->base[i] = (long long)i * cap;
 
@@ -1366,7 +1348,7 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
     const void* srcs[4] = {wk->h_img.data(), nullptr, wk->h_oct.data(), tilespan.data()};
     size_t sizes[4] = {n * sizeof(ImgMeta), (2 * n + 2) * sizeof(int), wk->h_oct.size() * sizeof(OctMeta),
                        tilespan.size() * sizeof(int2)};
-    SIFT_TRY(ctx_put_many(ctx, fresh ? 4 : 2, dsts, srcs, sizes));
+    if (int rc = ctx_put_many(ctx, fresh ? 4 : 2, dsts, srcs, sizes)) return rc;
   }
   if (fresh && fast) {
     // one TMA descriptor per grey plane: f32 tensor (w, h), row stride pitch*4, box = tile + halo
@@ -1377,27 +1359,18 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
       unsigned long long dims[2] = {(unsigned long long)om.w, (unsigned long long)om.h};
       unsigned long long strides[1] = {(unsigned long long)om.pitch * sizeof(float)};
       unsigned box[2] = {(unsigned)(BT_W + 2 * ((R + 3) & ~3)), (unsigned)(BT_H + 2 * R)};
-      SIFT_TRY(ctx_tma_encode(ctx, &maps[k], wk->arena + om.gauss_off, 2, dims, strides, box));
+      if (int rc = ctx_tma_encode(ctx, &maps[k], wk->arena + om.gauss_off, 2, dims, strides, box)) return rc;
     }
-    SIFT_TRY(ctx_put(ctx, wk->d_maps, maps.data(), maps.size() * sizeof(TmaDesc)));
+    if (int rc = ctx_put(ctx, wk->d_maps, maps.data(), maps.size() * sizeof(TmaDesc))) return rc;
   }
-
-#define SIFT_LAUNCH(name, kernel, grid, block, smem, ...)                                   \
-  do {                                                                                      \
-    ctx->launches++;                                                                        \
-    if (ctx->profiling) ctx_prof_begin(ctx, name);                                          \
-    kernel<<<(grid), (block), (smem), ctx->stream>>>(__VA_ARGS__);                          \
-    if (ctx->profiling) ctx_prof_end(ctx);                                                  \
-    SIFT_CUDA(cudaGetLastError());                                                          \
-  } while (0)
 
   {
     dim3 g(ceil_div(plan->max_w0, PG_TW), ceil_div(plan->max_h0, PG_TH), n);
-    float* work = keep ? wk->arena : nullptr;
+    float* work = keep ? wk->arena.get() : nullptr;
     if (channels)
-      SIFT_LAUNCH("k_pyramid_grey_rgb8", k_pyramid_grey<SrcRgb8>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);
+      PANO_LAUNCH(ctx, "k_pyramid_grey_rgb8", k_pyramid_grey<SrcRgb8>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);
     else
-      SIFT_LAUNCH("k_pyramid_grey", k_pyramid_grey<SrcF32>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);
+      PANO_LAUNCH(ctx, "k_pyramid_grey", k_pyramid_grey<SrcF32>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);
   }
   {
     const ExtremaParams ep{n_scale, p->pre_color_thres, p->judge_extrema_diff_thres, cap, wk->cand_count, wk->cand_keys,
@@ -1409,17 +1382,17 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
       const int GW = BT_W + 2 * ((R + 3) & ~3), GH = BT_H + 2 * R;
       const size_t gsz = ((size_t)GH * GW + 31) & ~(size_t)31;
       size_t smf = (2 * gsz + (size_t)BLUR_COLBUF_FLOATS(6) + (size_t)BT_H * (BT_W + 1) + EX_RING_FLOATS) * sizeof(float);
-      SIFT_CUDA(sift_smem_limit(ctx, (const void*)k_blur_extrema, smf));
+      PANO_CUDA(ctx, sift_smem_limit(ctx, (const void*)k_blur_extrema, smf));
       const int grid = std::min(wk->n_tiles, ctx->num_sms * 3);
-      SIFT_LAUNCH("k_blur_extrema", k_blur_extrema, grid, BT_THREADS, smf, wk->d_oct, wk->d_tilespan, n_om, wk->n_tiles,
+      PANO_LAUNCH(ctx, "k_blur_extrema", k_blur_extrema, grid, BT_THREADS, smf, wk->d_oct, wk->d_tilespan, n_om, wk->n_tiles,
                   wk->d_maps, wk->arena, gt, ep);
       // grid sized for typical counts (a few thousand pairs per image); it strides over the real one
-      SIFT_LAUNCH("k_extrema_seams", k_extrema_seams, dim3(8, n), 256, 0, wk->d_oct, n_oct, wk->arena, ep);
+      PANO_LAUNCH(ctx, "k_extrema_seams", k_extrema_seams, dim3(8, n), 256, 0, wk->d_oct, n_oct, wk->arena, ep);
     } else {
       if (smem > 48 * 1024)
-        SIFT_CUDA(sift_smem_limit(ctx, (const void*)k_blur_dog, smem));
-      SIFT_LAUNCH("k_blur_dog_generic", k_blur_dog, wk->n_tiles, BT_THREADS, smem, wk->d_oct, wk->d_tilespan, n_om, wk->arena, gt);
-      SIFT_LAUNCH("k_extrema_scan", k_extrema_scan, wk->n_tiles, EXS_THREADS, 0, wk->d_oct, wk->d_tilespan, n_om,
+        PANO_CUDA(ctx, sift_smem_limit(ctx, (const void*)k_blur_dog, smem));
+      PANO_LAUNCH(ctx, "k_blur_dog_generic", k_blur_dog, wk->n_tiles, BT_THREADS, smem, wk->d_oct, wk->d_tilespan, n_om, wk->arena, gt);
+      PANO_LAUNCH(ctx, "k_extrema_scan", k_extrema_scan, wk->n_tiles, EXS_THREADS, 0, wk->d_oct, wk->d_tilespan, n_om,
                   wk->arena, ep);
     }
   }
@@ -1427,22 +1400,22 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
     // latency kernels: grids sized for typical counts (a few thousand candidates per image);
     // they stride over the real device-side count, so nothing is launched per capacity slot
     dim3 g(8, n);
-    SIFT_LAUNCH("k_rank_sort", k_rank_sort, g, 256, 0, wk->cand_count, wk->cand_keys, wk->sorted_keys, cap);
+    PANO_LAUNCH(ctx, "k_rank_sort", k_rank_sort, g, 256, 0, wk->cand_count, wk->cand_keys, wk->sorted_keys, cap);
     RefineParams rp{n_scale, p->calc_offset_depth, p->offset_thres, p->contrast_thres, p->edge_ratio,
                     p->gauss_sigma, p->scale_factor};
     dim3 g4(16, n);
-    SIFT_LAUNCH("k_refine", k_refine, g4, 128, 0, wk->d_oct, wk->arena, n_oct, wk->cand_count, wk->sorted_keys, rp, cap,
+    PANO_LAUNCH(ctx, "k_refine", k_refine, g4, 128, 0, wk->d_oct, wk->arena, n_oct, wk->cand_count, wk->sorted_keys, rp, cap,
                 wk->refined, wk->kp_valid);
-    SIFT_LAUNCH("k_orientation", k_orientation, ctx->num_sms * 8, ORI_WARPS * 32, 0, wk->d_oct, wk->arena, n_oct, n, cap,
+    PANO_LAUNCH(ctx, "k_orientation", k_orientation, ctx->num_sms * 8, ORI_WARPS * 32, 0, wk->d_oct, wk->arena, n_oct, n, cap,
                 wk->cand_count, wk->refined, wk->kp_valid, p->ori_radius, p->ori_hist_smooth_count, wk->npeaks, wk->dirs,
                 wk->cand_count + n + 1);
-    SIFT_LAUNCH("k_expand_scan", k_expand_scan, n, SCAN_THREADS, 0, wk->cand_count, wk->kp_valid, wk->npeaks,
+    PANO_LAUNCH(ctx, "k_expand_scan", k_expand_scan, n, SCAN_THREADS, 0, wk->cand_count, wk->kp_valid, wk->npeaks,
                 wk->dirs, cap, fs->d_count, wk->n_refined, wk->desc_cand, wk->desc_dir);
     DescParams dp{p->desc_hist_scale_factor, p->desc_int_factor};
     const size_t dsm = sizeof(DescQuadSmem) * DESC_WARPS;
-    SIFT_CUDA(sift_smem_limit(ctx, (const void*)k_descriptor, dsm));
+    PANO_CUDA(ctx, sift_smem_limit(ctx, (const void*)k_descriptor, dsm));
     const int grid = ctx->num_sms * DESC_MIN_CTAS;
-    SIFT_LAUNCH("k_descriptor", k_descriptor, grid, DESC_THREADS, dsm, wk->d_oct, wk->d_img, wk->arena, n_oct, n, cap,
+    PANO_LAUNCH(ctx, "k_descriptor", k_descriptor, grid, DESC_THREADS, dsm, wk->d_oct, wk->d_img, wk->arena, n_oct, n, cap,
                 wk->refined, fs->d_count, wk->desc_cand, wk->desc_dir, dp, fs->d_desc, fs->d_coor, wk->cand_count + n);
   }
   wk->n_desc = fs->d_count;
@@ -1450,34 +1423,26 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
   // counts to the host (pinned, async); consumers wait on the completion marker queued behind them
   if (!fs->h_count_pinned) {
     fs->h_count_pinned = (int*)ctx_small_pinned_get(ctx, (size_t)2 * n * sizeof(int) + 16, &fs->h_count_cap);
-    if (!fs->h_count_pinned) SIFT_FAIL(PANO_ERR_CUDA, "pinned allocation failed");
+    if (!fs->h_count_pinned) return ctx_fail(ctx, PANO_ERR_CUDA, "pinned allocation failed");
   }
   {
     void* dsts[2] = {fs->h_count_pinned, fs->h_count_pinned + n};
     const void* srcs[2] = {fs->d_count, wk->cand_count};
     size_t sizes[2] = {n * sizeof(int), n * sizeof(int)};
-    SIFT_TRY(ctx_store_many(ctx, 2, dsts, srcs, sizes));
+    if (int rc = ctx_store_many(ctx, 2, dsts, srcs, sizes)) return rc;
   }
-  SIFT_CUDA(ctx_signal(ctx, &fs->counts_token));
+  PANO_CUDA(ctx, ctx_signal(ctx, &fs->counts_token));
   fs->counts_pending = true;
   fs->counts_on_host = false;
 
   if (keep) {
-    *keep = wk;
-    plan->wk = nullptr;
-    delete plan;
+    *keep = std::move(plan->wk);
   } else if (ctx->cache_limit && plan->bytes <= ctx->cache_limit) {
-    ctx->sift_plan = plan;
     ctx->sift_plan_bytes = plan->bytes;
-    if (ctx->cached_bytes + plan->bytes > ctx->cache_limit) ctx_cache_release(ctx, ctx->cache_limit - plan->bytes);
-  } else {
-    sift_plan_free(ctx, plan);
+    ctx->sift_plan = plan.release();
+    if (ctx->cached_bytes + ctx->sift_plan_bytes > ctx->cache_limit) ctx_cache_release(ctx, ctx->cache_limit - ctx->sift_plan_bytes);
   }
-  return PANO_OK;
-#undef SIFT_FAIL
-#undef SIFT_TRY
-#undef SIFT_CUDA
-#undef SIFT_LAUNCH
+  return PANO_OK;   // a plan nobody took is freed here
 }
 
 
@@ -1506,8 +1471,8 @@ int featureset_sync_counts(pano_featureset* fs) {
     if (cap < worst || fs->src.empty())
       return fs->error = ctx_fail(ctx, PANO_ERR_CAPACITY, "sift: %d list entries in one image exceed the capacity %d", worst, fs->cap);
     // run again with larger lists; the old outputs go back to the pool in stream order
-    ctx_free(ctx, fs->d_desc); ctx_free(ctx, fs->d_coor); ctx_free(ctx, fs->d_count);
-    fs->d_desc = nullptr; fs->d_coor = nullptr; fs->d_real = nullptr; fs->d_count = nullptr;
+    fs->d_desc.reset(); fs->d_coor.reset(); fs->d_count.reset();
+    fs->d_real = nullptr;
     ctx->sift_cap = cap;
     const std::vector<const void*> src = fs->src;
     const std::vector<int> channels = fs->src_channels;
@@ -1515,7 +1480,7 @@ int featureset_sync_counts(pano_featureset* fs) {
                             fs->src_h.data(), &fs->src_params, fs, nullptr, cap);
     if (rc) return fs->error = rc;
   }
-  if (fs->owned_block) { ctx_free(ctx, fs->owned_block); fs->owned_block = nullptr; }
+  fs->owned_block.reset();
   fs->counts_on_host = true;
   return PANO_OK;
 }

@@ -2,6 +2,7 @@
 #pragma once
 #include "common.cuh"
 #include "match_tc.cuh"
+#include <memory>
 
 #define SIFT_MAX_OCT 8
 #define SIFT_MAX_LEVELS 8        // nscale-1 blurred levels
@@ -47,27 +48,27 @@ struct SiftWork {
   int n_img = 0, n_oct = 0, n_scale = 0;
   std::vector<ImgMeta> h_img;
   std::vector<OctMeta> h_oct;     // n_img * n_oct
-  float* arena = nullptr;
+  DevBuf<float> arena;
   size_t arena_floats = 0;
-  ImgMeta* d_img = nullptr;
-  OctMeta* d_oct = nullptr;
-  int2* d_tilespan = nullptr;
-  TmaDesc* d_maps = nullptr;      // [n_img * n_oct]
+  DevBuf<ImgMeta> d_img;
+  DevBuf<OctMeta> d_oct;
+  DevBuf<int2> d_tilespan;
+  DevBuf<TmaDesc> d_maps;         // [n_img * n_oct]
   int n_tiles = 0;
   int cap = SIFT_CAP_DEFAULT;     // per-image capacity of every candidate / descriptor list below
   // keypoint state, all [n_img * cap] unless noted
-  int* cand_count = nullptr;      // [n_img] + work counters (see sift.cu)
-  uint32_t* cand_keys = nullptr;
-  uint32_t* seam_keys = nullptr;   // [n_img * seam capacity]: tile-perimeter pairs for k_extrema_seams
-  uint32_t* sorted_keys = nullptr;
-  pano_sspoint* refined = nullptr;  // valid flag in .dir < 0 ? no: see kp_valid
-  unsigned char* kp_valid = nullptr;
-  int* npeaks = nullptr;
-  float* dirs = nullptr;            // [n_img * cap * SIFT_MAX_PEAKS]
-  int* n_desc = nullptr;            // [n_img]
-  int* n_refined = nullptr;         // [n_img] (for traces)
-  int* desc_cand = nullptr;         // [n_img * cap] candidate index of descriptor
-  float* desc_dir = nullptr;        // [n_img * cap]
+  DevBuf<int> cand_count;         // [n_img] + work counters (see sift.cu)
+  DevBuf<uint32_t> cand_keys;
+  DevBuf<uint32_t> seam_keys;     // [n_img * seam capacity]: tile-perimeter pairs for k_extrema_seams
+  DevBuf<uint32_t> sorted_keys;
+  DevBuf<pano_sspoint> refined;   // valid flag in .dir < 0 ? no: see kp_valid
+  DevBuf<unsigned char> kp_valid;
+  DevBuf<int> npeaks;
+  DevBuf<float> dirs;             // [n_img * cap * SIFT_MAX_PEAKS]
+  int* n_desc = nullptr;          // [n_img]: the featureset's d_count
+  DevBuf<int> n_refined;          // [n_img] (for traces)
+  DevBuf<int> desc_cand;          // [n_img * cap] candidate index of descriptor
+  DevBuf<float> desc_dir;         // [n_img * cap]
 };
 
 // What a batch's shape alone decides, kept by the context (pano_ctx::sift_plan) for the next batch of the
@@ -76,7 +77,7 @@ struct SiftWork {
 // ImgMeta (the source pointers) and resets the counters.
 struct SiftPlan {
   std::vector<int> key;           // see sift_plan_key: n, cap, every (w, h, source kind), pano_params
-  SiftWork* wk = nullptr;
+  std::unique_ptr<SiftWork> wk;
   size_t bytes = 0;               // device bytes held (counted against the context's cache_limit)
   GaussTable gt;
   bool fast = true;
@@ -87,14 +88,13 @@ struct SiftPlan {
 struct pano_featureset {
   pano_ctx* ctx = nullptr;
   int n_images = 0;
-  float* d_desc = nullptr;    // rows of 128 f32
-  double* d_coor = nullptr;   // rows of 2 f64 (may be null for uploaded sets)
+  DevBuf<float> d_desc;       // rows of 128 f32
+  DevBuf<double> d_coor;      // rows of 2 f64 (may be null for uploaded sets)
   double* d_real = nullptr;   // SIFT sets: unscaled real_coor in [0,1), rows of 2 f64 (second half of d_coor's block)
-  int* d_count = nullptr;     // [n_images]
+  DevBuf<int> d_count;        // [n_images]
   std::vector<long long> base;  // first row of image i
   std::vector<int> h_count;
   bool counts_on_host = false;
-  cudaEvent_t counts_ready = nullptr;   // unused by the SIFT path (kept for uploaded sets)
   unsigned counts_token = 0;            // completion marker of the count read-back (ctx_signal)
   bool counts_pending = false;
   int* h_count_pinned = nullptr;
@@ -109,12 +109,10 @@ struct pano_featureset {
   std::vector<int> src_channels;        // u8 sources: channels per image; empty: f32 sources
   std::vector<int> src_w, src_h;
   pano_params src_params;
-  void* owned_block = nullptr;          // staged upload of the host entry points, freed after the count sync
+  DevBuf<unsigned char> owned_block;    // staged upload of the host entry points, freed after the count sync
 };
 
 // d_src: h×w×3 f32 device images when channels is null, else h×w×channels[i] u8 device images
 int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w, const int* h,
-                   const pano_params* p, pano_featureset* fs, SiftWork** keep, int cap);
-void sift_work_free(pano_ctx* ctx, SiftWork* wk);
-void sift_plan_free(pano_ctx* ctx, SiftPlan* plan);
+                   const pano_params* p, pano_featureset* fs, std::unique_ptr<SiftWork>* keep, int cap);
 int featureset_sync_counts(pano_featureset* fs);

@@ -191,29 +191,16 @@ static int cyl_warp_batch(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double
     d.r = (double)c.r; d.cy = c.cy; d.offy = offy; d.sizefactor_inv = sizefactor_inv;
     max_ow = std::max(max_ow, sw); max_oh = std::max(max_oh, sh);
   }
-  CylJobDev* d_jobs = nullptr;
-  double* d_tabs = nullptr;
+  DevBuf<CylJobDev> d_jobs;
+  DevBuf<double> d_tabs;
   int rc = 0;
-  if ((rc = ctx_alloc(ctx, (void**)&d_jobs, dj.size() * sizeof(CylJobDev))) ||
-      (rc = ctx_alloc(ctx, (void**)&d_tabs, tabs.size() * sizeof(double)))) {
-    ctx_free(ctx, d_jobs); ctx_free(ctx, d_tabs);
-    return rc;
-  }
-  rc = ctx_put(ctx, d_jobs, dj.data(), dj.size() * sizeof(CylJobDev));
-  if (!rc) rc = ctx_put(ctx, d_tabs, tabs.data(), tabs.size() * sizeof(double));
-  if (!rc) {
-    dim3 b(32, 8), g(ceil_div(max_ow, 32), ceil_div(max_oh, 8), n);   // 256 threads: the 8-bit conversion table
-    const char* name = pix ? "k_cyl_warp_rgb8" : "k_cyl_warp";
-    ctx->launches++;
-    if (ctx->profiling) ctx_prof_begin(ctx, name);
-    if (pix) k_cyl_warp_batch<SrcRgb8><<<g, b, 0, ctx->stream>>>(d_jobs, d_tabs);
-    else k_cyl_warp_batch<SrcF32><<<g, b, 0, ctx->stream>>>(d_jobs, d_tabs);
-    if (ctx->profiling) ctx_prof_end(ctx);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) rc = ctx_cuda(ctx, e, name);
-  }
-  ctx_free(ctx, d_jobs); ctx_free(ctx, d_tabs);      // stream-ordered: released after the kernel
-  return rc;
+  if ((rc = d_jobs.alloc(ctx, dj.size())) || (rc = d_tabs.alloc(ctx, tabs.size()))) return rc;
+  if ((rc = ctx_put(ctx, d_jobs, dj.data(), dj.size() * sizeof(CylJobDev)))) return rc;
+  if ((rc = ctx_put(ctx, d_tabs, tabs.data(), tabs.size() * sizeof(double)))) return rc;
+  dim3 b(32, 8), g(ceil_div(max_ow, 32), ceil_div(max_oh, 8), n);   // 256 threads: the 8-bit conversion table
+  if (pix) PANO_LAUNCH(ctx, "k_cyl_warp_rgb8", k_cyl_warp_batch<SrcRgb8>, g, b, 0, d_jobs, d_tabs);
+  else PANO_LAUNCH(ctx, "k_cyl_warp", k_cyl_warp_batch<SrcF32>, g, b, 0, d_jobs, d_tabs);
+  return PANO_OK;   // stream-ordered: the blocks are released after the kernel
 }
 
 extern "C" {
@@ -260,30 +247,20 @@ int pano_cyl_warp(pano_ctx* ctx, const float* rgb, int w, int h, double h_factor
     tab[j] = c.r * tan(px) + c.cx;
     tab[ow + j] = cos(px);
   }
-  float *d_src = nullptr, *d_dst = nullptr;
-  double* d_tab = nullptr;
+  DevBuf<float> d_src, d_dst;
+  DevBuf<double> d_tab;
   size_t bs = (size_t)w * h * 3 * sizeof(float), bd = (size_t)ow * oh * 3 * sizeof(float);
   int rc = 0;
-  if ((rc = ctx_alloc(ctx, (void**)&d_src, bs)) || (rc = ctx_alloc(ctx, (void**)&d_dst, bd)) ||
-      (rc = ctx_alloc(ctx, (void**)&d_tab, tab.size() * sizeof(double)))) {
-    ctx_free(ctx, d_src); ctx_free(ctx, d_dst); ctx_free(ctx, d_tab);
+  if ((rc = d_src.alloc(ctx, (size_t)w * h * 3)) || (rc = d_dst.alloc(ctx, (size_t)ow * oh * 3)) ||
+      (rc = d_tab.alloc(ctx, tab.size())))
     return rc;
-  }
-  cudaError_t e = cudaMemcpyAsync(d_src, rgb, bs, cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_tab, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream);
-  if (e == cudaSuccess) {
-    dim3 b(32, 8), g(ceil_div(ow, 32), ceil_div(oh, 8));
-    ctx->launches++;
-    if (ctx->profiling) ctx_prof_begin(ctx, "k_cyl_warp");
-    k_cyl_warp<<<g, b, 0, ctx->stream>>>(d_src, w, h, d_dst, ow, oh, d_tab, d_tab + ow, (double)c.r, c.cy, offy,
-                                        sizefactor_inv);
-    if (ctx->profiling) ctx_prof_end(ctx);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_dst, bd, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  ctx_free(ctx, d_src); ctx_free(ctx, d_dst); ctx_free(ctx, d_tab);
-  if (e != cudaSuccess) return ctx_cuda(ctx, e, "pano_cyl_warp");
+  PANO_CUDA(ctx, cudaMemcpyAsync(d_src, rgb, bs, cudaMemcpyHostToDevice, ctx->stream));
+  PANO_CUDA(ctx, cudaMemcpyAsync(d_tab, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+  dim3 b(32, 8), g(ceil_div(ow, 32), ceil_div(oh, 8));
+  PANO_LAUNCH(ctx, "k_cyl_warp", k_cyl_warp, g, b, 0, d_src, w, h, d_dst, ow, oh, d_tab, d_tab + ow, (double)c.r, c.cy, offy,
+              sizefactor_inv);
+  PANO_CUDA(ctx, cudaMemcpyAsync(out, d_dst, bd, cudaMemcpyDeviceToHost, ctx->stream));
+  PANO_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return PANO_OK;
 }
 
