@@ -298,6 +298,10 @@ k_ba_jtr(const BaPairDev* __restrict__ pairs, int n_pair, const double* __restri
 }
 
 struct pano_ba_session {
+  ~pano_ba_session() {
+    cudaStreamSynchronize(ctx->stream);   // h_out may still be written by a queued kernel
+    ctx_small_pinned_put(ctx, std::move(h_out));
+  }
   pano_ctx* ctx = nullptr;
   int n_cam = 0, n_pair = 0, max_match = 0;
   long long nm = 0;
@@ -310,8 +314,7 @@ struct pano_ba_session {
   float2* d_sq = nullptr;
   BaErrStats* d_st = nullptr;
   int* d_nonfinite = nullptr;              // per pair: one of its residuals is inf or NaN
-  double* h_out = nullptr;                 // host-mapped {avg, max}
-  size_t h_out_cap = 0;
+  PinnedBuf h_out;                         // host-mapped {avg, max}
 };
 
 extern "C" int pano_ba_session_create(pano_ctx* ctx, int n_cam, int n_pair, const pano_ba_link* links, const double* pts,
@@ -332,7 +335,7 @@ extern "C" int pano_ba_session_create(pano_ctx* ctx, int n_cam, int n_pair, cons
   }
   if (nm && !pts) return ctx_fail(ctx, PANO_ERR_INVALID, "ba session: %lld matches but no coordinates", nm);
   if (2 * nm > 0x7fffffffll) return ctx_fail(ctx, PANO_ERR_INVALID, "ba session: %lld matches is too many", nm);
-  pano_ba_session* s = new pano_ba_session;
+  std::unique_ptr<pano_ba_session> s(new pano_ba_session);
   s->ctx = ctx; s->n_cam = n_cam; s->n_pair = n_pair; s->nm = nm; s->max_match = max_match;
   s->table.resize(n_pair);
   for (int k = 0; k < n_pair; ++k) {
@@ -347,7 +350,7 @@ extern "C" int pano_ba_session_create(pano_ctx* ctx, int n_cam, int n_pair, cons
   const size_t b_st = 256, b_flags = align_up((size_t)n_pair * 4 + 16, 256);
   const size_t total = b_pairs + 3 * b_pts + b_rows + b_sq + b_hto + b_jtj + b_b + b_st + b_flags;
   int rc = s->arena.alloc(ctx, total);
-  if (rc) { delete s; return rc; }
+  if (rc) return rc;
   char* q = s->arena;
   s->d_pairs = (BaPairDev*)q; q += b_pairs;
   s->d_to = (double2*)q; q += b_pts;
@@ -360,14 +363,14 @@ extern "C" int pano_ba_session_create(pano_ctx* ctx, int n_cam, int n_pair, cons
   s->d_b = (double*)q; q += b_b;
   s->d_st = (BaErrStats*)q; q += b_st;
   s->d_nonfinite = (int*)q;
-  s->h_out = (double*)ctx_small_pinned_get(ctx, 64, &s->h_out_cap);
-  if (!s->h_out) { pano_ba_session_free(s); return ctx_fail(ctx, PANO_ERR_CUDA, "ba session: pinned allocation failed"); }
+  s->h_out = ctx_small_pinned_get(ctx, 64);
+  if (!s->h_out.get()) return ctx_fail(ctx, PANO_ERR_CUDA, "ba session: pinned allocation failed");
   // one-time upload of the pair table and the coordinates, split into p.first (to) and p.second (from)
   const size_t up = (size_t)n_pair * sizeof(BaPairDev) + (size_t)nm * 32;
   if (up) {
     cudaError_t e = cudaStreamSynchronize(ctx->stream);  // the staging buffer may still feed earlier copies
     char* st = (char*)ctx_pinned(ctx, up + 64);
-    if (e != cudaSuccess || !st) { pano_ba_session_free(s); return e != cudaSuccess ? ctx_cuda(ctx, e, "ba session") : ctx_fail(ctx, PANO_ERR_CUDA, "ba session: pinned staging allocation failed"); }
+    if (e != cudaSuccess || !st) return e != cudaSuccess ? ctx_cuda(ctx, e, "ba session") : ctx_fail(ctx, PANO_ERR_CUDA, "ba session: pinned staging allocation failed");
     if (n_pair) memcpy(st, s->table.data(), (size_t)n_pair * sizeof(BaPairDev));
     double* to = (double*)(st + (size_t)n_pair * sizeof(BaPairDev));
     double* fr = to + 2 * nm;
@@ -379,17 +382,14 @@ extern "C" int pano_ba_session_create(pano_ctx* ctx, int n_cam, int n_pair, cons
     if (e == cudaSuccess && nm) e = cudaMemcpyAsync(s->d_to, to, (size_t)nm * 16, cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess && nm) e = cudaMemcpyAsync(s->d_from, fr, (size_t)nm * 16, cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { pano_ba_session_free(s); return ctx_cuda(ctx, e, "ba session upload"); }
+    if (e != cudaSuccess) return ctx_cuda(ctx, e, "ba session upload");
   }
-  *out = s;
+  *out = s.release();
   return PANO_OK;
 }
 
 extern "C" void pano_ba_session_free(pano_ba_session* s) {
-  if (!s) return;
-  ctx_enter(s->ctx);
-  cudaStreamSynchronize(s->ctx->stream);                  // h_out may still be written by a queued kernel
-  if (s->h_out) ctx_small_pinned_put(s->ctx, s->h_out, s->h_out_cap);
+  if (s) ctx_enter(s->ctx);
   delete s;
 }
 
@@ -419,11 +419,12 @@ extern "C" int pano_ba_error(pano_ba_session* s, int n_pair, const double* hto_t
     PANO_LAUNCH(ctx, "k_ba_residuals", k_ba_residuals, grid, 128, 0, s->d_pairs, n_pair, s->d_hto, s->d_to, s->d_from, s->d_res,
                 s->d_sq, s->d_st, s->d_nonfinite);
   }
-  PANO_LAUNCH(ctx, "k_ba_error_sum", k_ba_error_sum, 1, 1024, 0, (const float*)s->d_sq, 2 * s->nm, s->d_st, s->h_out);
+  double* h_out = (double*)s->h_out.get();
+  PANO_LAUNCH(ctx, "k_ba_error_sum", k_ba_error_sum, 1, 1024, 0, (const float*)s->d_sq, 2 * s->nm, s->d_st, h_out);
   if (so) PANO_CUDA(ctx, cudaMemcpyAsync(so, s->d_res, b_res, cudaMemcpyDeviceToHost, ctx->stream));
   PANO_CUDA(ctx, ctx_spin_stream(ctx));
-  *avg = s->h_out[0];
-  *max = s->h_out[1];
+  *avg = h_out[0];
+  *max = h_out[1];
   if (so) memcpy(residuals, so, b_res);
   s->have_error = true;
   return PANO_OK;

@@ -710,6 +710,8 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
 // two-slot device ring.  Window k's upload runs on the stream's copy stream into slot k & 1 while
 // window k-1's kernels run on the context's stream; events order the slot's reuse.
 struct pano_blend_stream {
+  // the copy stream drains before the staging and slot memory go
+  ~pano_blend_stream() { if (copy) cudaStreamSynchronize(copy.get()); }
   pano_ctx* ctx = nullptr;
   int n = 0, bands = 0, lazy = 0, ordered = 0;
   BlendJob job;
@@ -718,26 +720,13 @@ struct pano_blend_stream {
   DevBuf<float> d_wsum;        // linear: tw×th Σ w
   int added = 0, windows = 0, err = 0;
   bool finished = false;
-  cudaStream_t copy = nullptr;
-  cudaEvent_t ev_copied[2] = {nullptr, nullptr};   // slot's upload done (copy stream)
-  cudaEvent_t ev_done[2] = {nullptr, nullptr};     // slot's last reader done (context stream)
+  StreamPtr copy;
+  EventPtr ev_copied[2];   // slot's upload done (copy stream)
+  EventPtr ev_done[2];     // slot's last reader done (context stream)
   DevBuf<unsigned char> slot[2];
   size_t slot_cap[2] = {0, 0};
-  unsigned char* stage[2] = {nullptr, nullptr};    // pinned staging of pageable sources
-  size_t stage_cap[2] = {0, 0};
+  PinnedBuf stage[2];      // pinned staging of pageable sources
 };
-
-// the device blocks go with the stream's owners, after its copy stream has drained
-static void blend_stream_release(pano_blend_stream* s) {
-  if (s->copy) cudaStreamSynchronize(s->copy);
-  for (int b = 0; b < 2; ++b) {
-    if (s->stage[b]) cudaFreeHost(s->stage[b]);
-    if (s->ev_copied[b]) cudaEventDestroy(s->ev_copied[b]);
-    if (s->ev_done[b]) cudaEventDestroy(s->ev_done[b]);
-  }
-  if (s->copy) cudaStreamDestroy(s->copy);
-  delete s;
-}
 
 // every failure is sticky: the canvas state is undefined after it
 static int stream_fail(pano_blend_stream* s, int rc) { s->err = rc; return rc; }
@@ -765,32 +754,28 @@ static int stream_upload(pano_blend_stream* s, int first, int count, const void*
   }
   // slot b and its staging were last used by window - 2: its upload must be over before the host
   // refills the staging buffer (an event never recorded counts as complete)
-  STREAM_CUDA(s, cudaEventSynchronize(s->ev_copied[b]));
+  STREAM_CUDA(s, cudaEventSynchronize(s->ev_copied[b].get()));
   if (s->slot_cap[b] < total) {
     s->slot[b].reset(); s->slot_cap[b] = 0;
     if (int rc = s->slot[b].alloc(ctx, total)) return stream_fail(s, rc);
     s->slot_cap[b] = total;
-    STREAM_CUDA(s, cudaEventRecord(s->ev_done[b], ctx->stream));   // the block is ours from here on the context stream
+    STREAM_CUDA(s, cudaEventRecord(s->ev_done[b].get(), ctx->stream));   // the block is ours from here on the context stream
   }
-  if (!all_pinned && s->stage_cap[b] < total) {
-    if (s->stage[b]) cudaFreeHost(s->stage[b]);
-    s->stage[b] = nullptr; s->stage_cap[b] = 0;
-    STREAM_CUDA(s, cudaMallocHost((void**)&s->stage[b], total));
-    s->stage_cap[b] = total;
-  }
+  if (!all_pinned) STREAM_CUDA(s, s->stage[b].grow(total, total, cudaHostAllocDefault));
   // the copy must not overwrite the slot before window - 2's kernels have read it
-  STREAM_CUDA(s, cudaStreamWaitEvent(s->copy, s->ev_done[b], 0));
+  STREAM_CUDA(s, cudaStreamWaitEvent(s->copy.get(), s->ev_done[b].get(), 0));
+  unsigned char* stage = (unsigned char*)s->stage[b].get();
   for (int k = 0; k < count; ++k) {
     const void* src = srcs[k];
     if (!host_is_pinned(src)) {               // pageable: staged, the caller may reuse it on return
-      memcpy(s->stage[b] + off[k], src, bytes[k]);
-      src = s->stage[b] + off[k];
+      memcpy(stage + off[k], src, bytes[k]);
+      src = stage + off[k];
     }
-    STREAM_CUDA(s, cudaMemcpyAsync(s->slot[b] + off[k], src, bytes[k], cudaMemcpyHostToDevice, s->copy));
+    STREAM_CUDA(s, cudaMemcpyAsync(s->slot[b] + off[k], src, bytes[k], cudaMemcpyHostToDevice, s->copy.get()));
     win[k].pix = s->slot[b] + off[k];
   }
-  STREAM_CUDA(s, cudaEventRecord(s->ev_copied[b], s->copy));
-  STREAM_CUDA(s, cudaStreamWaitEvent(ctx->stream, s->ev_copied[b], 0));
+  STREAM_CUDA(s, cudaEventRecord(s->ev_copied[b].get(), s->copy.get()));
+  STREAM_CUDA(s, cudaStreamWaitEvent(ctx->stream, s->ev_copied[b].get(), 0));
   *slot_out = b;
   return PANO_OK;
 }
@@ -887,7 +872,7 @@ int pano_blend_stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs,
   if (n <= 0 || !imgs || !g || !p || bands < 0) return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: bad argument");
   if (n > PANO_MAX_IMAGES)   // a window's images on gridDim.z of k_mb_first_level
     return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: %d images (limit %d)", n, PANO_MAX_IMAGES);
-  std::unique_ptr<pano_blend_stream, void (*)(pano_blend_stream*)> s(new pano_blend_stream, blend_stream_release);
+  std::unique_ptr<pano_blend_stream> s(new pano_blend_stream);
   s->ctx = ctx; s->n = n; s->bands = bands; s->lazy = p->lazy_read; s->ordered = p->ordered_input;
   int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, 0, oh, false, &s->job);
   if (!rc) rc = blend_dev_setup(ctx, &s->job, bands, 0, oh, &s->dev);
@@ -898,10 +883,10 @@ int pano_blend_stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs,
     PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx * 3 + 255) / 256), 256, 0, s->d_sum, npx * 3, 0.f);
     PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx + 255) / 256), 256, 0, s->d_wsum, npx, 0.f);
   }
-  cudaError_t e = cudaStreamCreateWithFlags(&s->copy, cudaStreamNonBlocking);
+  cudaError_t e = make_stream(&s->copy);
   for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
-    e = cudaEventCreateWithFlags(&s->ev_copied[b], cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_done[b], cudaEventDisableTiming);
+    e = make_event(&s->ev_copied[b], cudaEventDisableTiming);
+    if (e == cudaSuccess) e = make_event(&s->ev_done[b], cudaEventDisableTiming);
   }
   if (e != cudaSuccess) return ctx_cuda(ctx, e, "blend stream: copy stream / events");
   *out = s.release();
@@ -936,7 +921,7 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
   rc = u8 ? stream_launch<SrcRgb8>(s, d_win, win.data(), count) : stream_launch<SrcF32>(s, d_win, win.data(), count);
   if (rc) return stream_fail(s, rc);
   if (slot >= 0) {
-    STREAM_CUDA(s, cudaEventRecord(s->ev_done[slot], ctx->stream));
+    STREAM_CUDA(s, cudaEventRecord(s->ev_done[slot].get(), ctx->stream));
     ++s->windows;
   }
   s->added += count;
@@ -972,9 +957,8 @@ int pano_blend_stream_finish(pano_blend_stream* s, float* out) {
 }
 
 void pano_blend_stream_free(pano_blend_stream* s) {
-  if (!s) return;
-  ctx_enter(s->ctx);
-  blend_stream_release(s);
+  if (s) ctx_enter(s->ctx);
+  delete s;
 }
 
 int pano_blend(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,

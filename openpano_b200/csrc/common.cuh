@@ -15,74 +15,14 @@
 #include <string>
 #include <vector>
 #include <map>
+#include <memory>
+#include <type_traits>
 #include <unordered_map>
 
 #include "../../include/pano_b200.h"
 
-// ------------------------------------------------------------------ context
+// ------------------------------------------------------------------ owners
 
-struct ProfEvent {
-  const char* name;
-  cudaEvent_t start, stop;
-};
-
-struct SiftPlan;   // sift.cuh
-
-struct pano_ctx {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  bool owns_stream = false;
-  cudaMemPool_t pool = nullptr;   // this context's own stream-ordered pool (see ctx_alloc)
-  // Freed blocks kept for the next request of (about) the same size: see ctx_alloc
-  struct CachedBlock { void* p; unsigned long long stamp; };
-  std::multimap<size_t, CachedBlock> cache;        // size -> free block
-  std::unordered_map<void*, size_t> live;           // blocks handed out -> their true size
-  size_t cached_bytes = 0, cache_limit = (size_t)16 << 30;   // one 64-view multiband job parks ~8 GB; an H100 has 80
-  unsigned long long cache_stamp = 0;
-  std::string err;
-  bool profiling = false;
-  std::vector<ProfEvent> prof_pending;
-  std::vector<cudaEvent_t> event_pool;
-  std::map<std::string, std::pair<int, double>> prof_acc;  // name -> (launches, ms)
-  long long launches = 0;
-  int last_match_exact_rows = 0;   // rows the last match call had to decide exactly (gathered pass)
-  int last_match_nominated_rows = 0;   // columns on demand: rows of the larger sets nominated on request
-  int last_match_full_rescans = 0; // of those, rows that needed a scan of every target
-  int num_sms = 132;
-  // cudaFuncSetAttribute is per device: remembered per context, never per process
-  bool attr_tc = false, attr_match = false;
-  int sift_cap = 0;                // per-image list capacity SIFT batches start with (grows on overflow, sticky)
-  // The last SIFT batch's shape-dependent setup (sift.cu), one entry; its device bytes count against
-  // cache_limit, so PANO_CACHE_MB=0 keeps none.  pano_trim, pano_destroy and ctx_alloc's
-  // out-of-memory retry release it.
-  SiftPlan* sift_plan = nullptr;
-  size_t sift_plan_bytes = 0;
-  void* tma_encode = nullptr;      // cuTensorMapEncodeTiled, resolved through the runtime (no -lcuda)
-  // pinned host staging (grown on demand)
-  void* pinned = nullptr;
-  size_t pinned_bytes = 0;
-  void* pinned2 = nullptr;
-  size_t pinned2_bytes = 0;
-  // pinned + device-mapped ring for small host<->device moves done by SM kernels
-  char* ring = nullptr;
-  size_t ring_cap = 0, ring_off = 0;
-  // recycled pinned blocks for per-featureset count read-backs (cudaHostAlloc / cudaFreeHost
-  // are slow and cudaFreeHost synchronises the whole device)
-  std::vector<std::pair<void*, size_t>> small_pinned;
-  // completion markers: a word in pinned host memory the stream writes sequence numbers to
-  volatile unsigned* flag = nullptr;
-  unsigned flag_seq = 0;
-  // planet(): per-pixel d / center and theta / 2π (planet.cu), uploaded on the first call, freed by pano_destroy
-  double2* planet_tab = nullptr;
-};
-
-// Every entry point makes its context's device current first: host threads other than the
-// creating one start on device 0 (a stitch lane's thread on rank 1 would otherwise issue
-// its copies against the wrong device).
-static inline void ctx_enter(const pano_ctx* ctx) { if (ctx) cudaSetDevice(ctx->device); }
-
-int  ctx_fail(pano_ctx* ctx, int code, const char* fmt, ...);
-int  ctx_cuda(pano_ctx* ctx, cudaError_t e, const char* what);
 // Stream-ordered device memory from the CONTEXT'S OWN pool.  Contexts sharing the device's
 // default pool hand each other freed blocks, and the allocator then makes the taking
 // stream wait for the giving stream ("internal dependencies"): concurrent stitch lanes
@@ -135,7 +75,113 @@ class DevBuf {
   pano_ctx* ctx_ = nullptr;
   T* p_ = nullptr;
 };
-void ctx_sift_plan_release(pano_ctx* ctx);   // frees the kept SIFT plan's blocks (into the cache)
+
+// Owners of pinned host blocks, CUDA events, streams and memory pools.
+struct CudaDestroy {
+  void operator()(void* host) const { cudaFreeHost(host); }
+  void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+  void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }
+  void operator()(cudaMemPool_t p) const { cudaMemPoolDestroy(p); }
+};
+// One page-locked host block from cudaHostAlloc (cudaFreeHost synchronises the whole device: see
+// pano_ctx::small_pinned).  Move-only.
+class PinnedBuf {
+ public:
+  // Holds at least `bytes` afterwards: a smaller block is freed and `alloc` (>= bytes) bytes are taken
+  // with `flags`.  On failure the buffer is empty.
+  cudaError_t grow(size_t bytes, size_t alloc, unsigned flags) {
+    if (bytes <= cap()) return cudaSuccess;
+    p_.reset();
+    void* p = nullptr;
+    const cudaError_t e = cudaHostAlloc(&p, alloc, flags);
+    if (e == cudaSuccess) { p_.reset(p); cap_ = alloc; }
+    return e;
+  }
+  void* get() const { return p_.get(); }
+  size_t cap() const { return p_ ? cap_ : 0; }
+
+ private:
+  std::unique_ptr<void, CudaDestroy> p_;
+  size_t cap_ = 0;   // of the block p_ holds
+};
+using EventPtr = std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, CudaDestroy>;
+using StreamPtr = std::unique_ptr<std::remove_pointer_t<cudaStream_t>, CudaDestroy>;
+using PoolPtr = std::unique_ptr<std::remove_pointer_t<cudaMemPool_t>, CudaDestroy>;
+static inline cudaError_t make_event(EventPtr* ev, unsigned flags) {
+  cudaEvent_t e = nullptr;
+  const cudaError_t err = cudaEventCreateWithFlags(&e, flags);
+  ev->reset(err == cudaSuccess ? e : nullptr);
+  return err;
+}
+static inline cudaError_t make_stream(StreamPtr* s) {
+  cudaStream_t h = nullptr;
+  const cudaError_t err = cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking);
+  s->reset(err == cudaSuccess ? h : nullptr);
+  return err;
+}
+
+// ------------------------------------------------------------------ context
+
+struct ProfEvent {
+  const char* name;
+  EventPtr start, stop;
+};
+
+struct SiftPlan;   // sift.cuh
+
+struct pano_ctx {
+  ~pano_ctx();
+  // declared first, destroyed last: the other members may free into the pool or queue on the stream
+  StreamPtr own_stream;           // the stream pano_create made; empty when it was given one (borrowed)
+  cudaStream_t stream = nullptr;  // what every call of this context is queued on
+  PoolPtr pool;                   // this context's own stream-ordered pool (see ctx_alloc)
+  int device = 0;
+  // Freed blocks kept for the next request of (about) the same size: see ctx_alloc
+  struct CachedBlock { void* p; unsigned long long stamp; };
+  std::multimap<size_t, CachedBlock> cache;        // size -> free block
+  std::unordered_map<void*, size_t> live;           // blocks handed out -> their true size
+  size_t cached_bytes = 0, cache_limit = (size_t)16 << 30;   // one 64-view multiband job parks ~8 GB; an H100 has 80
+  unsigned long long cache_stamp = 0;
+  std::string err;
+  bool profiling = false;
+  std::vector<ProfEvent> prof_pending;
+  std::vector<EventPtr> event_pool;
+  std::map<std::string, std::pair<int, double>> prof_acc;  // name -> (launches, ms)
+  long long launches = 0;
+  int last_match_exact_rows = 0;   // rows the last match call had to decide exactly (gathered pass)
+  int last_match_nominated_rows = 0;   // columns on demand: rows of the larger sets nominated on request
+  int last_match_full_rescans = 0; // of those, rows that needed a scan of every target
+  int num_sms = 132;
+  // cudaFuncSetAttribute is per device: remembered per context, never per process
+  bool attr_tc = false, attr_match = false;
+  int sift_cap = 0;                // per-image list capacity SIFT batches start with (grows on overflow, sticky)
+  // The last SIFT batch's shape-dependent setup (sift.cu), one entry; its device bytes count against
+  // cache_limit, so PANO_CACHE_MB=0 keeps none.  pano_trim, pano_destroy and ctx_alloc's
+  // out-of-memory retry release it.
+  std::unique_ptr<SiftPlan> sift_plan;
+  void* tma_encode = nullptr;      // cuTensorMapEncodeTiled, resolved through the runtime (no -lcuda)
+  // pinned host staging (grown on demand)
+  PinnedBuf pinned, pinned2;
+  // pinned + device-mapped ring for small host<->device moves done by SM kernels
+  PinnedBuf ring;
+  size_t ring_off = 0;
+  // recycled pinned blocks for per-featureset count read-backs (cudaHostAlloc / cudaFreeHost
+  // are slow and cudaFreeHost synchronises the whole device)
+  std::vector<PinnedBuf> small_pinned;
+  // completion markers: a word in pinned host memory the stream writes sequence numbers to
+  PinnedBuf flag;
+  unsigned flag_seq = 0;
+  // planet(): per-pixel d / center and theta / 2π (planet.cu), uploaded on the first call, freed by pano_destroy
+  DevBuf<double2> planet_tab;
+};
+
+// Every entry point makes its context's device current first: host threads other than the
+// creating one start on device 0 (a stitch lane's thread on rank 1 would otherwise issue
+// its copies against the wrong device).
+static inline void ctx_enter(const pano_ctx* ctx) { if (ctx) cudaSetDevice(ctx->device); }
+
+int  ctx_fail(pano_ctx* ctx, int code, const char* fmt, ...);
+int  ctx_cuda(pano_ctx* ctx, cudaError_t e, const char* what);
 void* ctx_pinned(pano_ctx* ctx, size_t bytes);   // staging buffer A (inputs)
 void* ctx_pinned2(pano_ctx* ctx, size_t bytes);  // staging buffer B (results)
 extern "C" bool host_is_pinned(const void* p);   // page-locked (cudaHostAlloc / pano_host_alloc) host memory
@@ -160,8 +206,9 @@ cudaError_t ctx_spin_stream(pano_ctx* ctx);
 cudaError_t ctx_signal(pano_ctx* ctx, unsigned* token);
 cudaError_t ctx_wait_signal(pano_ctx* ctx, unsigned token);
 void* ctx_ring(pano_ctx* ctx, size_t bytes);
-void* ctx_small_pinned_get(pano_ctx* ctx, size_t bytes, size_t* cap);
-void ctx_small_pinned_put(pano_ctx* ctx, void* p, size_t cap);
+// a mapped block of at least `bytes` from ctx->small_pinned (empty on failure); put gives one back to it
+PinnedBuf ctx_small_pinned_get(pano_ctx* ctx, size_t bytes);
+void ctx_small_pinned_put(pano_ctx* ctx, PinnedBuf&& b);
 int  ctx_fetch(pano_ctx* ctx, void* d_dst, const void* h_pinned_src, size_t bytes);
 int  ctx_store(pano_ctx* ctx, void* h_pinned_dst, const void* d_src, size_t bytes);
 int  ctx_put(pano_ctx* ctx, void* d_dst, const void* h_src, size_t bytes);

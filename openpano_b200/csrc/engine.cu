@@ -51,12 +51,12 @@ int ctx_alloc(pano_ctx* ctx, void** p, size_t bytes) {
       return PANO_OK;
     }
   }
-  cudaError_t e = ctx->pool ? cudaMallocFromPoolAsync(p, bytes, ctx->pool, ctx->stream) : cudaMallocAsync(p, bytes, ctx->stream);
+  cudaError_t e = cudaMallocFromPoolAsync(p, bytes, ctx->pool.get(), ctx->stream);
   if (e != cudaSuccess && (ctx->cached_bytes || ctx->sift_plan)) {   // out of memory with blocks parked here: give them back, retry
     cudaGetLastError();
-    ctx_sift_plan_release(ctx);
+    ctx->sift_plan.reset();
     ctx_cache_release(ctx, 0);
-    e = ctx->pool ? cudaMallocFromPoolAsync(p, bytes, ctx->pool, ctx->stream) : cudaMallocAsync(p, bytes, ctx->stream);
+    e = cudaMallocFromPoolAsync(p, bytes, ctx->pool.get(), ctx->stream);
   }
   if (e != cudaSuccess) return ctx_cuda(ctx, e, "cudaMallocAsync");
   if (ctx->cache_limit) ctx->live[*p] = bytes;
@@ -85,32 +85,18 @@ void ctx_free(pano_ctx* ctx, void* p) {
   if (!ctx->cache_limit || size > ctx->cache_limit) { cudaFreeAsync(p, ctx->stream); return; }
   ctx->cache.emplace(size, pano_ctx::CachedBlock{p, ++ctx->cache_stamp});
   ctx->cached_bytes += size;
-  if (ctx->cached_bytes + ctx->sift_plan_bytes > ctx->cache_limit)   // the kept SIFT plan shares the budget
-    ctx_cache_release(ctx, ctx->cache_limit - std::min(ctx->sift_plan_bytes, ctx->cache_limit));
+  const size_t plan_bytes = ctx->sift_plan ? ctx->sift_plan->bytes : 0;   // the kept SIFT plan shares the budget
+  if (ctx->cached_bytes + plan_bytes > ctx->cache_limit) ctx_cache_release(ctx, ctx->cache_limit - std::min(plan_bytes, ctx->cache_limit));
 }
 
-void ctx_sift_plan_release(pano_ctx* ctx) {
-  SiftPlan* plan = ctx->sift_plan;
-  ctx->sift_plan = nullptr;
-  ctx->sift_plan_bytes = 0;
-  delete plan;
+static void* staging(PinnedBuf& b, size_t bytes) {
+  return b.grow(bytes, std::max(bytes, (size_t)1 << 20), cudaHostAllocDefault) == cudaSuccess ? b.get() : nullptr;
 }
-
-static void* grow_pinned(void** buf, size_t* cap, size_t bytes) {
-  if (bytes <= *cap) return *buf;
-  if (*buf) cudaFreeHost(*buf);
-  *buf = nullptr; *cap = 0;
-  size_t want = std::max(bytes, (size_t)1 << 20);
-  if (cudaMallocHost(buf, want) != cudaSuccess) { *buf = nullptr; return nullptr; }
-  *cap = want;
-  return *buf;
-}
-
-void* ctx_pinned(pano_ctx* ctx, size_t bytes) { return grow_pinned(&ctx->pinned, &ctx->pinned_bytes, bytes); }
+void* ctx_pinned(pano_ctx* ctx, size_t bytes) { return staging(ctx->pinned, bytes); }
 void* ctx_pinned2(pano_ctx* ctx, size_t bytes) {
   // metadata staging is reused across calls: wait for earlier async copies
-  if (ctx->pinned2) cudaStreamSynchronize(ctx->stream);
-  return grow_pinned(&ctx->pinned2, &ctx->pinned2_bytes, bytes);
+  if (ctx->pinned2.get()) cudaStreamSynchronize(ctx->stream);
+  return staging(ctx->pinned2, bytes);
 }
 
 static inline void cpu_relax(int n) {
@@ -137,25 +123,24 @@ __global__ void k_set_flag(volatile unsigned* flag, unsigned seq) {
 
 cudaError_t ctx_signal(pano_ctx* ctx, unsigned* token) {
   SlowCall sc("ctx_signal");
-  if (!ctx->flag) {
-    void* p = nullptr;
-    cudaError_t e = cudaHostAlloc(&p, 64, cudaHostAllocMapped | cudaHostAllocPortable);
+  if (!ctx->flag.get()) {
+    cudaError_t e = ctx->flag.grow(64, 64, cudaHostAllocMapped | cudaHostAllocPortable);
     if (e != cudaSuccess) return e;
-    memset(p, 0, 64);
-    ctx->flag = (volatile unsigned*)p;
+    memset(ctx->flag.get(), 0, 64);
   }
   const unsigned seq = ++ctx->flag_seq;
   ctx->launches++;
-  k_set_flag<<<1, 1, 0, ctx->stream>>>(ctx->flag, seq);
+  k_set_flag<<<1, 1, 0, ctx->stream>>>((volatile unsigned*)ctx->flag.get(), seq);
   *token = seq;
   return cudaGetLastError();
 }
 
 cudaError_t ctx_wait_signal(pano_ctx* ctx, unsigned token) {
   SlowCall sc("ctx_wait_signal(gpu)");
-  if (!ctx->flag) return cudaStreamSynchronize(ctx->stream);
+  const volatile unsigned* flag = (const volatile unsigned*)ctx->flag.get();
+  if (!flag) return cudaStreamSynchronize(ctx->stream);
   for (long long spins = 0;; ++spins) {
-    if ((int)(*ctx->flag - token) >= 0) return cudaSuccess;
+    if ((int)(*flag - token) >= 0) return cudaSuccess;
     cpu_relax(4);
     if (spins > (1LL << 28)) return cudaStreamSynchronize(ctx->stream);   // seconds: let a device fault surface
   }
@@ -179,35 +164,33 @@ __global__ void k_zero_u32(uint32_t* __restrict__ dst, size_t n) {
 void* ctx_ring(pano_ctx* ctx, size_t bytes) {
   SlowCall sc("ctx_ring");
   bytes = (bytes + 63) / 64 * 64;
-  if (!ctx->ring || bytes > ctx->ring_cap) {
-    if (ctx->ring) { cudaStreamSynchronize(ctx->stream); cudaFreeHost(ctx->ring); ctx->ring = nullptr; }
-    size_t cap = std::max(bytes * 2, (size_t)8 << 20);
-    if (cudaHostAlloc((void**)&ctx->ring, cap, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) { ctx->ring = nullptr; ctx->ring_cap = 0; return nullptr; }
-    ctx->ring_cap = cap; ctx->ring_off = 0;
+  if (bytes > ctx->ring.cap()) {
+    if (ctx->ring.get()) cudaStreamSynchronize(ctx->stream);   // queued kernels may still read the old ring
+    if (ctx->ring.grow(bytes, std::max(bytes * 2, (size_t)8 << 20), cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) return nullptr;
+    ctx->ring_off = 0;
   }
-  if (ctx->ring_off + bytes > ctx->ring_cap) {   // wrap: everything queued so far must have consumed its slice
+  if (ctx->ring_off + bytes > ctx->ring.cap()) {   // wrap: everything queued so far must have consumed its slice
     cudaStreamSynchronize(ctx->stream);
     ctx->ring_off = 0;
   }
-  void* p = ctx->ring + ctx->ring_off;
+  void* p = (char*)ctx->ring.get() + ctx->ring_off;
   ctx->ring_off += bytes;
   return p;
 }
 
-void* ctx_small_pinned_get(pano_ctx* ctx, size_t bytes, size_t* cap) {
-  for (size_t i = 0; i < ctx->small_pinned.size(); ++i)
-    if (ctx->small_pinned[i].second >= bytes) {
-      void* p = ctx->small_pinned[i].first; *cap = ctx->small_pinned[i].second;
-      ctx->small_pinned.erase(ctx->small_pinned.begin() + i);
-      return p;
+PinnedBuf ctx_small_pinned_get(pano_ctx* ctx, size_t bytes) {
+  for (auto it = ctx->small_pinned.begin(); it != ctx->small_pinned.end(); ++it)
+    if (it->cap() >= bytes) {
+      PinnedBuf b = std::move(*it);
+      ctx->small_pinned.erase(it);
+      return b;
     }
-  void* p = nullptr;
-  size_t want = std::max<size_t>((bytes + 255) / 256 * 256, 1024);
-  if (cudaHostAlloc(&p, want, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) return nullptr;
-  *cap = want;
-  return p;
+  PinnedBuf b;
+  const size_t want = std::max<size_t>((bytes + 255) / 256 * 256, 1024);
+  b.grow(want, want, cudaHostAllocMapped | cudaHostAllocPortable);
+  return b;
 }
-void ctx_small_pinned_put(pano_ctx* ctx, void* p, size_t cap) { if (p) ctx->small_pinned.emplace_back(p, cap); }
+void ctx_small_pinned_put(pano_ctx* ctx, PinnedBuf&& b) { if (b.get()) ctx->small_pinned.push_back(std::move(b)); }
 
 static unsigned small_grid(size_t words) { return (unsigned)std::min<size_t>(std::max<size_t>((words + 255) / 256, 1), 256); }
 
@@ -395,36 +378,42 @@ int ctx_copy_blocks(pano_ctx* ctx, int n, void* const* dst, const void* const* s
   return PANO_OK;
 }
 
-static cudaEvent_t get_event(pano_ctx* ctx) {
-  if (!ctx->event_pool.empty()) { cudaEvent_t e = ctx->event_pool.back(); ctx->event_pool.pop_back(); return e; }
-  cudaEvent_t e;
-  cudaEventCreate(&e);
+static EventPtr get_event(pano_ctx* ctx) {
+  EventPtr e;
+  if (!ctx->event_pool.empty()) { e = std::move(ctx->event_pool.back()); ctx->event_pool.pop_back(); }
+  else make_event(&e, cudaEventDefault);
   return e;
 }
 
 void ctx_prof_begin(pano_ctx* ctx, const char* name) {
-  ProfEvent pe;
-  pe.name = name;
-  pe.start = get_event(ctx);
-  pe.stop = get_event(ctx);
-  cudaEventRecord(pe.start, ctx->stream);
-  ctx->prof_pending.push_back(pe);
+  ProfEvent pe{name, get_event(ctx), get_event(ctx)};
+  cudaEventRecord(pe.start.get(), ctx->stream);
+  ctx->prof_pending.push_back(std::move(pe));
 }
 
-void ctx_prof_end(pano_ctx* ctx) { cudaEventRecord(ctx->prof_pending.back().stop, ctx->stream); }
+void ctx_prof_end(pano_ctx* ctx) { cudaEventRecord(ctx->prof_pending.back().stop.get(), ctx->stream); }
 
 static void prof_drain(pano_ctx* ctx) {
   if (ctx->prof_pending.empty()) return;
   cudaStreamSynchronize(ctx->stream);
   for (auto& pe : ctx->prof_pending) {
     float ms = 0;
-    cudaEventElapsedTime(&ms, pe.start, pe.stop);
+    cudaEventElapsedTime(&ms, pe.start.get(), pe.stop.get());
     auto& acc = ctx->prof_acc[pe.name];
     acc.first += 1; acc.second += ms;
-    ctx->event_pool.push_back(pe.start);
-    ctx->event_pool.push_back(pe.stop);
+    ctx->event_pool.push_back(std::move(pe.start));
+    ctx->event_pool.push_back(std::move(pe.stop));
   }
   ctx->prof_pending.clear();
+}
+
+// the DevBuf owners first (ctx_free uses the cache); the other members go after the body, pool and stream last
+pano_ctx::~pano_ctx() {
+  sift_plan.reset();
+  planet_tab.reset();
+  ctx_cache_release(this, 0);
+  cudaStreamSynchronize(stream);
+  prof_drain(this);
 }
 
 extern "C" {
@@ -450,21 +439,14 @@ int pano_create(pano_ctx** out, int device, void* cuda_stream) {
                     e != cudaSuccess ? cudaGetErrorString(e) : "device count 0");
   if (device < 0 || device >= ndev) return ctx_fail(nullptr, PANO_ERR_INVALID, "device %d out of range [0,%d)", device, ndev);
   if ((e = cudaSetDevice(device)) != cudaSuccess) return ctx_cuda(nullptr, e, "cudaSetDevice");
-  pano_ctx* ctx = new pano_ctx;
-  ctx->device = device;
   cudaDeviceProp prop;
-  if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) { delete ctx; return ctx_cuda(nullptr, e, "cudaGetDeviceProperties"); }
-  if (prop.major != 9 || prop.minor != 0) {   // sm_90a code runs on compute capability 9.0 only
-    int rc = ctx_fail(nullptr, PANO_ERR_NO_DEVICE, "device %d is sm_%d%d; libpano_b200 is built for sm_90a only", device, prop.major, prop.minor);
-    delete ctx; return rc;
-  }
-  ctx->num_sms = prop.multiProcessorCount;
-  if (cuda_stream) { ctx->stream = (cudaStream_t)cuda_stream; ctx->owns_stream = false; }
-  else {
-    if ((e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking)) != cudaSuccess) { delete ctx; return ctx_cuda(nullptr, e, "cudaStreamCreate"); }
-    ctx->owns_stream = true;
-  }
+  if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return ctx_cuda(nullptr, e, "cudaGetDeviceProperties");
+  if (prop.major != 9 || prop.minor != 0)   // sm_90a code runs on compute capability 9.0 only
+    return ctx_fail(nullptr, PANO_ERR_NO_DEVICE, "device %d is sm_%d%d; libpano_b200 is built for sm_90a only", device, prop.major, prop.minor);
+  StreamPtr own_stream;   // a caller's stream is borrowed: never destroyed here
+  if (!cuda_stream && (e = make_stream(&own_stream)) != cudaSuccess) return ctx_cuda(nullptr, e, "cudaStreamCreate");
   // a private pool that keeps its freed blocks: the same sizes recur every batch
+  PoolPtr pool;
   {
     cudaMemPoolProps props;
     memset(&props, 0, sizeof(props));
@@ -472,14 +454,18 @@ int pano_create(pano_ctx** out, int device, void* cuda_stream) {
     props.handleTypes = cudaMemHandleTypeNone;
     props.location.type = cudaMemLocationTypeDevice;
     props.location.id = device;
-    if ((e = cudaMemPoolCreate(&ctx->pool, &props)) != cudaSuccess) {
-      if (ctx->owns_stream) cudaStreamDestroy(ctx->stream);
-      delete ctx;
-      return ctx_cuda(nullptr, e, "cudaMemPoolCreate");
-    }
+    cudaMemPool_t p = nullptr;
+    if ((e = cudaMemPoolCreate(&p, &props)) != cudaSuccess) return ctx_cuda(nullptr, e, "cudaMemPoolCreate");
+    pool.reset(p);
     uint64_t thr = UINT64_MAX;
-    cudaMemPoolSetAttribute(ctx->pool, cudaMemPoolAttrReleaseThreshold, &thr);
+    cudaMemPoolSetAttribute(p, cudaMemPoolAttrReleaseThreshold, &thr);
   }
+  pano_ctx* ctx = new pano_ctx;
+  ctx->device = device;
+  ctx->num_sms = prop.multiProcessorCount;
+  ctx->stream = cuda_stream ? (cudaStream_t)cuda_stream : own_stream.get();
+  ctx->own_stream = std::move(own_stream);
+  ctx->pool = std::move(pool);
   if (const char* e = getenv("PANO_CACHE_MB")) ctx->cache_limit = (size_t)std::max(0LL, atoll(e)) << 20;
   *out = ctx;
   return PANO_OK;
@@ -488,7 +474,7 @@ int pano_create(pano_ctx** out, int device, void* cuda_stream) {
 int pano_trim(pano_ctx* ctx) {
   if (!ctx) return PANO_ERR_INVALID;
   ctx_enter(ctx);
-  ctx_sift_plan_release(ctx);
+  ctx->sift_plan.reset();
   ctx_cache_release(ctx, 0);
   return PANO_OK;
 }
@@ -497,31 +483,17 @@ int pano_mem_high_water(pano_ctx* ctx, size_t* bytes, int reset) {
   if (!ctx || !bytes) return PANO_ERR_INVALID;
   ctx_enter(ctx);
   unsigned long long v = 0;   // cuuint64_t
-  PANO_CUDA(ctx, cudaMemPoolGetAttribute(ctx->pool, cudaMemPoolAttrUsedMemHigh, &v));
+  PANO_CUDA(ctx, cudaMemPoolGetAttribute(ctx->pool.get(), cudaMemPoolAttrUsedMemHigh, &v));
   *bytes = (size_t)v;
   if (reset) {
     unsigned long long zero = 0;   // the mark restarts at what is in use now
-    PANO_CUDA(ctx, cudaMemPoolSetAttribute(ctx->pool, cudaMemPoolAttrUsedMemHigh, &zero));
+    PANO_CUDA(ctx, cudaMemPoolSetAttribute(ctx->pool.get(), cudaMemPoolAttrUsedMemHigh, &zero));
   }
   return PANO_OK;
 }
 
 void pano_destroy(pano_ctx* ctx) {
-  if (!ctx) return;
-  cudaSetDevice(ctx->device);
-  ctx_sift_plan_release(ctx);
-  ctx_cache_release(ctx, 0);
-  if (ctx->planet_tab) cudaFreeAsync(ctx->planet_tab, ctx->stream);
-  cudaStreamSynchronize(ctx->stream);
-  prof_drain(ctx);
-  for (auto e : ctx->event_pool) cudaEventDestroy(e);
-  if (ctx->pinned) cudaFreeHost(ctx->pinned);
-  if (ctx->pinned2) cudaFreeHost(ctx->pinned2);
-  if (ctx->ring) cudaFreeHost(ctx->ring);
-  if (ctx->flag) cudaFreeHost((void*)ctx->flag);
-  for (auto& sp : ctx->small_pinned) cudaFreeHost(sp.first);
-  if (ctx->pool) cudaMemPoolDestroy(ctx->pool);   // released once the last block has been freed
-  if (ctx->owns_stream) cudaStreamDestroy(ctx->stream);
+  ctx_enter(ctx);
   delete ctx;
 }
 
@@ -609,56 +581,46 @@ int pano_host_alloc(size_t bytes, void** h_ptr) {
 }
 int pano_host_free(void* h_ptr) { return cudaFreeHost(h_ptr) == cudaSuccess ? PANO_OK : PANO_ERR_CUDA; }
 
-struct pano_event { cudaEvent_t ev; int device; };
+struct pano_event { EventPtr ev; int device; };
 
 int pano_event_create(pano_ctx* ctx, pano_event** out) {
   ctx_enter(ctx);
   if (!ctx || !out) return PANO_ERR_INVALID;
-  pano_event* e = new pano_event;
+  std::unique_ptr<pano_event> e(new pano_event);
   e->device = ctx->device;
-  cudaError_t err = cudaEventCreateWithFlags(&e->ev, cudaEventDisableTiming);
-  if (err != cudaSuccess) { delete e; return ctx_cuda(ctx, err, "cudaEventCreate"); }
-  *out = e;
+  cudaError_t err = make_event(&e->ev, cudaEventDisableTiming);
+  if (err != cudaSuccess) return ctx_cuda(ctx, err, "cudaEventCreate");
+  *out = e.release();
   return PANO_OK;
 }
 int pano_event_record(pano_ctx* ctx, pano_event* ev) {
   ctx_enter(ctx);
   if (!ctx || !ev) return PANO_ERR_INVALID;
-  PANO_CUDA(ctx, cudaEventRecord(ev->ev, ctx->stream));
+  PANO_CUDA(ctx, cudaEventRecord(ev->ev.get(), ctx->stream));
   return PANO_OK;
 }
 int pano_event_wait(pano_ctx* ctx, pano_event* ev) {
   ctx_enter(ctx);
   if (!ctx || !ev) return PANO_ERR_INVALID;
-  PANO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev->ev, 0));
+  PANO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev->ev.get(), 0));
   return PANO_OK;
 }
 int pano_event_sync(pano_event* ev) {
   if (ev) cudaSetDevice(ev->device);
   if (!ev) return PANO_ERR_INVALID;
-  return ctx_spin_event(ev->ev) == cudaSuccess ? PANO_OK : PANO_ERR_CUDA;
+  return ctx_spin_event(ev->ev.get()) == cudaSuccess ? PANO_OK : PANO_ERR_CUDA;
 }
 void pano_event_destroy(pano_event* ev) {
   if (ev) cudaSetDevice(ev->device);
-  if (!ev) return;
-  cudaEventDestroy(ev->ev);
   delete ev;
 }
 
 // ---------------------------------------------------------------- features
 
-// the device blocks go with the featureset's owners
-static void featureset_release(pano_featureset* fs) {
-  if (!fs) return;
-  pano_ctx* ctx = fs->ctx;
-  if (fs->h_count_pinned) { if (ctx) ctx_small_pinned_put(ctx, fs->h_count_pinned, fs->h_count_cap); else cudaFreeHost(fs->h_count_pinned); }
-  delete fs;
-}
-
 // channels == nullptr: h×w×3 f32 device images; otherwise h×w×channels[i] u8 device images
 static int sift_detect_dev(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w,
                            const int* h, const pano_params* p, pano_featureset** out) {
-  pano_featureset* fs = new pano_featureset;
+  std::unique_ptr<pano_featureset> fs(new pano_featureset);
   fs->ctx = ctx;
   // kept for the capacity retry of featureset_sync_counts
   fs->src.assign(d_src, d_src + n); fs->src_w.assign(w, w + n); fs->src_h.assign(h, h + n); fs->src_params = *p;
@@ -667,9 +629,9 @@ static int sift_detect_dev(pano_ctx* ctx, int n, const void* const* d_src, const
     const char* e = getenv("PANO_SIFT_CAP");            // test hook: start small to exercise the growth path
     ctx->sift_cap = e ? std::max(256, atoi(e)) : SIFT_CAP_DEFAULT;
   }
-  int rc = sift_run_batch(ctx, n, d_src, channels, w, h, p, fs, nullptr, ctx->sift_cap);
-  if (rc != 0) { featureset_release(fs); return rc; }
-  *out = fs;
+  int rc = sift_run_batch(ctx, n, d_src, channels, w, h, p, fs.get(), nullptr, ctx->sift_cap);
+  if (rc != 0) return rc;
+  *out = fs.release();
   return PANO_OK;
 }
 
@@ -786,7 +748,7 @@ static int featureset_build(pano_ctx* ctx, int n_images, const int* n_kp, const 
   *out = nullptr;
   if (n_images > PANO_MAX_IMAGES)   // the matcher prepares its operands with images on gridDim.y
     return ctx_fail(ctx, PANO_ERR_INVALID, "featureset: %d images (limit %d)", n_images, PANO_MAX_IMAGES);
-  std::unique_ptr<pano_featureset> fs(new pano_featureset);   // no pinned count block: a plain delete releases it
+  std::unique_ptr<pano_featureset> fs(new pano_featureset);
   fs->ctx = ctx; fs->n_images = n_images;
   fs->base.resize(n_images); fs->h_count.resize(n_images);
   long long total = 0;
@@ -928,14 +890,14 @@ int pano_featureset_download_real(pano_featureset* fs, int image, double* real_x
 }
 
 void pano_featureset_free(pano_featureset* fs) {
-  if (fs) ctx_enter(fs->ctx); featureset_release(fs); }
+  if (fs) ctx_enter(fs->ctx); delete fs; }
 
 // ---------------------------------------------------------------- stage inspection
 
 struct pano_sift_trace {
   pano_ctx* ctx;
   std::unique_ptr<SiftWork> wk;
-  pano_featureset* fs;
+  std::unique_ptr<pano_featureset> fs;
   DevBuf<unsigned char> d_img;
 };
 
@@ -948,14 +910,14 @@ int pano_sift_trace_run(pano_ctx* ctx, const float* rgb, int w, int h, const pan
   const void* src = rgb;
   int rc = upload_images(ctx, 1, &src, nullptr, &w, &h, d_imgs, d_block);
   if (rc) return rc;
-  pano_featureset* fs = new pano_featureset;
+  std::unique_ptr<pano_featureset> fs(new pano_featureset);
   fs->ctx = ctx;
   std::unique_ptr<SiftWork> wk;
   // the trace keeps the work buffers of ONE run, so it grows the lists itself
   for (int cap = SIFT_CAP_DEFAULT;; cap *= 2) {
-    rc = sift_run_batch(ctx, 1, d_imgs.data(), nullptr, &w, &h, p, fs, &wk, cap);
+    rc = sift_run_batch(ctx, 1, d_imgs.data(), nullptr, &w, &h, p, fs.get(), &wk, cap);
     if (rc) break;
-    rc = featureset_sync_counts(fs);
+    rc = featureset_sync_counts(fs.get());
     if (rc == PANO_ERR_CAPACITY && cap < SIFT_CAP_MAX) {
       wk.reset();
       fs->d_desc.reset(); fs->d_coor.reset(); fs->d_count.reset();
@@ -964,8 +926,8 @@ int pano_sift_trace_run(pano_ctx* ctx, const float* rgb, int w, int h, const pan
     }
     break;
   }
-  if (rc) { featureset_release(fs); return rc; }
-  *out = new pano_sift_trace{ctx, std::move(wk), fs, std::move(d_block)};
+  if (rc) return rc;
+  *out = new pano_sift_trace{ctx, std::move(wk), std::move(fs), std::move(d_block)};
   return PANO_OK;
 }
 
@@ -1062,7 +1024,7 @@ int pano_sift_trace_descriptors(pano_sift_trace* t, int cap, double* coor_xy, fl
   if (t) ctx_enter(t->ctx);
   int n = t->fs->h_count[0];
   if (n <= cap && n > 0) {
-    int rc = pano_featureset_download(t->fs, 0, coor_xy, desc);
+    int rc = pano_featureset_download(t->fs.get(), 0, coor_xy, desc);
     if (rc) return rc;
   }
   return n;
@@ -1070,8 +1032,6 @@ int pano_sift_trace_descriptors(pano_sift_trace* t, int cap, double* coor_xy, fl
 
 void pano_sift_trace_free(pano_sift_trace* t) {
   if (t) ctx_enter(t->ctx);
-  if (!t) return;
-  featureset_release(t->fs);
   delete t;
 }
 

@@ -47,12 +47,11 @@ const std::vector<double2>& planet_table() {
 
 int planet_table_dev(pano_ctx* ctx, const double2** out) {
   if (!ctx->planet_tab) {
-    const std::vector<double2>& tab = planet_table();
-    void* p = nullptr;
-    PANO_CUDA(ctx, cudaMallocFromPoolAsync(&p, kPixels * sizeof(double2), ctx->pool, ctx->stream));
-    cudaError_t e = cudaMemcpyAsync(p, tab.data(), kPixels * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) { cudaFreeAsync(p, ctx->stream); return ctx_cuda(ctx, e, "planet table upload"); }
-    ctx->planet_tab = (double2*)p;
+    DevBuf<double2> tab;
+    if (int rc = tab.alloc(ctx, kPixels)) return rc;
+    cudaError_t e = cudaMemcpyAsync(tab, planet_table().data(), kPixels * sizeof(double2), cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess) return ctx_cuda(ctx, e, "planet table upload");
+    ctx->planet_tab = std::move(tab);
   }
   *out = ctx->planet_tab;
   return PANO_OK;

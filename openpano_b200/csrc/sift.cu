@@ -1221,9 +1221,7 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
   std::vector<int> key = sift_plan_key(n, channels, w, h, p, cap);
   std::unique_ptr<SiftPlan> plan;
   if (!keep) {
-    plan.reset(ctx->sift_plan);
-    ctx->sift_plan = nullptr;
-    ctx->sift_plan_bytes = 0;
+    plan = std::move(ctx->sift_plan);
     if (plan && plan->key != key) plan.reset();
   }
   const bool fresh = plan == nullptr;
@@ -1421,12 +1419,13 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
   wk->n_desc = fs->d_count;
 
   // counts to the host (pinned, async); consumers wait on the completion marker queued behind them
-  if (!fs->h_count_pinned) {
-    fs->h_count_pinned = (int*)ctx_small_pinned_get(ctx, (size_t)2 * n * sizeof(int) + 16, &fs->h_count_cap);
-    if (!fs->h_count_pinned) return ctx_fail(ctx, PANO_ERR_CUDA, "pinned allocation failed");
+  if (!fs->h_count_pinned.get()) {
+    fs->h_count_pinned = ctx_small_pinned_get(ctx, (size_t)2 * n * sizeof(int) + 16);
+    if (!fs->h_count_pinned.get()) return ctx_fail(ctx, PANO_ERR_CUDA, "pinned allocation failed");
   }
   {
-    void* dsts[2] = {fs->h_count_pinned, fs->h_count_pinned + n};
+    int* h_counts = (int*)fs->h_count_pinned.get();
+    void* dsts[2] = {h_counts, h_counts + n};
     const void* srcs[2] = {fs->d_count, wk->cand_count};
     size_t sizes[2] = {n * sizeof(int), n * sizeof(int)};
     if (int rc = ctx_store_many(ctx, 2, dsts, srcs, sizes)) return rc;
@@ -1438,9 +1437,8 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
   if (keep) {
     *keep = std::move(plan->wk);
   } else if (ctx->cache_limit && plan->bytes <= ctx->cache_limit) {
-    ctx->sift_plan_bytes = plan->bytes;
-    ctx->sift_plan = plan.release();
-    if (ctx->cached_bytes + ctx->sift_plan_bytes > ctx->cache_limit) ctx_cache_release(ctx, ctx->cache_limit - ctx->sift_plan_bytes);
+    ctx->sift_plan = std::move(plan);
+    if (ctx->cached_bytes + ctx->sift_plan->bytes > ctx->cache_limit) ctx_cache_release(ctx, ctx->cache_limit - ctx->sift_plan->bytes);
   }
   return PANO_OK;   // a plan nobody took is freed here
 }
@@ -1460,10 +1458,11 @@ int featureset_sync_counts(pano_featureset* fs) {
     if (e != cudaSuccess) return fs->error = ctx_cuda(ctx, e, "feature count read-back");
     fs->counts_pending = false;
     const int n = fs->n_images;
+    const int* h_counts = (const int*)fs->h_count_pinned.get();
     int worst = 0;
-    for (int i = 0; i < n; ++i) worst = std::max(worst, std::max(fs->h_count_pinned[i], fs->h_count_pinned[n + i]));
+    for (int i = 0; i < n; ++i) worst = std::max(worst, std::max(h_counts[i], h_counts[n + i]));
     if (worst <= fs->cap) {
-      fs->h_count.assign(fs->h_count_pinned, fs->h_count_pinned + n);
+      fs->h_count.assign(h_counts, h_counts + n);
       break;
     }
     int cap = fs->cap;

@@ -86,6 +86,7 @@ struct SiftPlan {
 };
 
 struct pano_featureset {
+  ~pano_featureset() { ctx_small_pinned_put(ctx, std::move(h_count_pinned)); }
   pano_ctx* ctx = nullptr;
   int n_images = 0;
   DevBuf<float> d_desc;       // rows of 128 f32
@@ -97,8 +98,7 @@ struct pano_featureset {
   bool counts_on_host = false;
   unsigned counts_token = 0;            // completion marker of the count read-back (ctx_signal)
   bool counts_pending = false;
-  int* h_count_pinned = nullptr;
-  size_t h_count_cap = 0;
+  PinnedBuf h_count_pinned;            // mapped [2n] ints: the counts, then the candidate counts
   TcOperands tc;              // fp16 tensor-core operands of the descriptors (lazy)
   bool tc_ready = false;
   int error = 0;              // sticky failure of the count read-back (returned by every later use)

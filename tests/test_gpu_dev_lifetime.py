@@ -1,6 +1,6 @@
 """GPU: with PANO_CACHE_MB=0 (no block cache, no kept SIFT plan) every entry point gives back every pool block it
 took, on success and on a failure after its inputs were validated: after each call the pool holds only the
-caller's buffers again."""
+caller's buffers again.  And a context gives back its pinned host memory, events and streams when it closes."""
 import ctypes
 
 import numpy as np
@@ -185,3 +185,66 @@ def test_every_entry_point_gives_its_blocks_back(eng):
 
     for d in d_img + d_pix + d_warp + [d_out, d_planet, d_rect, d_rgb8, d_desc, d_coor]:
         eng.dev_free(d)
+
+
+def _rss_bytes():
+    with open("/proc/self/status") as f:
+        for line in f:
+            if line.startswith("VmRSS:"):
+                return int(line.split()[1]) * 1024
+    raise AssertionError("no VmRSS in /proc/self/status")
+
+
+def test_closed_contexts_give_their_host_resources_back():
+    """Each cycle opens a context, takes every pinned-memory and event path once and closes it.  Pinned pages count
+    in the process's resident set, and one context holds at least its 8 MB ring, so contexts that kept their pinned
+    memory would grow it by that much per cycle."""
+    from openpano_b200.capi import Engine
+    p = default_params()
+    imgs, org = synth.make_stack(N, W, H, 120, 3)
+    items, geom = synth.translation_blend_setup(org, W, H)
+    shapes = [(H, W)] * N
+    pairs = [(0, 1), (1, 2), (0, 2)]
+    rcases = [ransac_case(200, 64, 5), ransac_case(80, 16, 6)]
+    cams, bpairs, bpts = ba_case(5, 40, 5, extra_pairs=3)
+    hto = np.tile(np.eye(3).reshape(-1), (len(bpairs), 1))
+
+    def cycle():
+        e = Engine(0)
+        try:
+            fs = e.sift_detect_batch(imgs, p)              # pageable sources: staging buffer A
+            try:
+                e.match_pairs(fs, pairs, p)                # the mapped ring and the completion-marker word
+            finally:
+                fs.free()
+            e.ransac_score_pairs(rcases)                   # staging buffers A and B
+            s = e.ba_session(5, bpairs, bpts)              # a recycled mapped block; B for the residuals
+            try:
+                s.error(hto, want_residuals=True)
+            finally:
+                s.close()
+            bs = e.blend_stream(shapes, items, geom, 0, p)  # its copy stream, events and pinned staging
+            try:
+                bs.add(imgs[:2])
+                bs.add(imgs[2:])
+                bs.finish()
+            finally:
+                bs.close()
+            e.profile(True)                                # pooled timing events
+            e.ransac_score_pairs(rcases)
+            e.profile(False)
+            ev = e.event_create()
+            e.event_record(ev)
+            Engine.event_sync(ev)
+            Engine.event_destroy(ev)
+        finally:
+            e.close()
+
+    cycles, ring_bytes = 20, 8 << 20
+    for _ in range(2):          # first-use costs of the driver, the library and the allocator
+        cycle()
+    rss0 = _rss_bytes()
+    for _ in range(cycles):
+        cycle()
+    grown = _rss_bytes() - rss0
+    assert grown < cycles * ring_bytes // 4, f"resident set grew by {grown / 2**20:.1f} MB over {cycles} contexts"
