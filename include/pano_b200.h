@@ -477,6 +477,50 @@ int  pano_blend_stream_finish_dev(pano_blend_stream* s, float* d_out_hwc);
 int  pano_blend_stream_finish(pano_blend_stream* s, float* out_hwc);
 void pano_blend_stream_free(pano_blend_stream* s);
 
+/* SIFT whose sources arrive in windows: LAZY_READ's feature stage (config.cfg:10-11, calc_feature in
+ * stitcherbase.cc:9-27 loads, detects and releases one image at a time) on the device.  For every
+ * partition of the images into windows and every source kind, the featureset from pano_sift_stream_finish
+ * equals pano_sift_detect_batch's (pano_sift_detect_batch_rgb8's for 8-bit sources) on the same images, bit
+ * for bit: counts, coordinates, real coordinates and descriptors, and so the match lists on it.  A stream
+ * takes up to PANO_MAX_IMAGES images, PANO_MAX_SIFT_BATCH at most in one add, so one featureset can hold
+ * more images than one SIFT batch.
+ *
+ * Device memory: a stream never holds more than two windows of sources.  Besides them it holds
+ *   - the SIFT work buffers and per-image keypoint lists of ONE window, what pano_sift_detect_batch_dev
+ *     takes for the images of that window (a list overflow re-runs the window with doubled lists, as the
+ *     batch does; the larger lists are the context's starting point from then on);
+ *   - the packed rows of finished windows: 544 B per descriptor (128 f32, 2 f64 coordinates, 2 f64 real
+ *     coordinates), each image's rows rounded up to 32, and no per-image list capacity;
+ *   - in pano_sift_stream_finish only, the featureset's own block of the same packed rows, filled from the
+ *     finished windows before they are freed.
+ * Host sources go through a two-slot device ring, each slot as large as the largest window uploaded through
+ * it; device sources are read in place and take no ring memory.  The work buffers stay with the context for
+ * the next window of the same shape, as between batches (PANO_CACHE_MB bounds what it keeps).
+ *
+ * Calls on a stream are calls on its ctx (same threading rule); the ctx must outlive it.  A misuse (null
+ * pointers, an unknown kind, channels other than 1 or 3 for 8-bit or 3 for f32 sources, out-of-order,
+ * overlapping or excess adds, more than PANO_MAX_SIFT_BATCH images in one add, finish before the last image
+ * or twice) returns PANO_ERR_INVALID, and every failure is sticky: later adds and finishes return it again.
+ * pano_sift_stream_free is always valid, and the ctx stays usable. */
+typedef struct pano_sift_stream pano_sift_stream;
+/* w[i] × h[i]: image i's shape (at least 2×2); p: the SIFT parameters of every window. */
+int  pano_sift_stream_create(pano_ctx* ctx, int n, const int* w, const int* h, const pano_params* p,
+                             pano_sift_stream** out);
+/* Adds images [first, first + count): first must be the number of images added so far.  srcs[i] is image
+ * first + i, h×w×3 f32 (Mat32f layout) for the f32 kinds and h×w×channels u8 (read_img's input) for the 8-bit
+ * kinds, with pano_src_kind as for pano_blend_stream_add.  The add first queues the upload of host sources on
+ * the stream's copy stream, then reads the previous window's counts (waiting for its SIFT, and running it again
+ * with doubled lists if it overflowed them), packs its rows and queues this window's SIFT.
+ * PAGEABLE host buffers are staged and may be reused as soon as the call returns.  PINNED host buffers
+ * (pano_host_alloc / cudaHostAlloc) and device sources are read asynchronously, and read again by a re-run:
+ * they must stay valid and untouched until the following add or the finish has returned. */
+int  pano_sift_stream_add(pano_sift_stream* s, int first, int count, const void* const* srcs, int kind,
+                          int channels);
+/* Valid once all n images have been added, once per stream.  Resolves the last window and returns an ordinary
+ * featureset (counts already on the host) that outlives the stream; free it with pano_featureset_free. */
+int  pano_sift_stream_finish(pano_sift_stream* s, pano_featureset** out);
+void pano_sift_stream_free(pano_sift_stream* s);
+
 /* ---------------------------------------------------------- little planet
  * Replaces planet() (main.cc:294-331, the `planet` sub-command) without the file I/O: the
  * stereographic "little planet" view of a mosaic.  The input is any h×w×3 f32 image (the blenders'

@@ -109,6 +109,10 @@ def _load():
         "pano_blend_stream_finish_dev": (C.c_int, [C.c_void_p, C.c_void_p]),
         "pano_blend_stream_finish": (C.c_int, [C.c_void_p, _fp]),
         "pano_blend_stream_free": (None, [C.c_void_p]),
+        "pano_sift_stream_create": (C.c_int, [C.c_void_p, C.c_int, _ip, _ip, P, _vpp]),
+        "pano_sift_stream_add": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _vpp, C.c_int, C.c_int]),
+        "pano_sift_stream_finish": (C.c_int, [C.c_void_p, _vpp]),
+        "pano_sift_stream_free": (None, [C.c_void_p]),
         "pano_mem_high_water": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t), C.c_int]),
         "pano_planet": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, _fp]),
         "pano_planet_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
@@ -312,14 +316,17 @@ class BaSession:
 SRC_F32_DEV, SRC_F32_HOST, SRC_RGB8_DEV, SRC_RGB8_HOST = 0, 1, 2, 3
 
 
-class BlendStream:
-    """A pano_blend_stream: the mosaic of pano_blend, fed window by window (LAZY_READ's memory contract).
-    add() takes numpy arrays (host; uint8 H×W / H×W×1 / H×W×3 or float32 H×W×3, the kind from the dtype) or
-    raw pointers with an explicit kind (SRC_*).  Every failure is sticky, as in the C ABI."""
+class _SourceStream:
+    """What the windowed streams share: add() takes numpy arrays (host; uint8 H×W / H×W×1 / H×W×3 or float32
+    H×W×3, the kind from the dtype) or raw pointers with an explicit kind (SRC_*).  Every failure is sticky, as
+    in the C ABI."""
+    _NAME = ""
+    _ADD = None
+    _FREE = None
 
-    def __init__(self, eng, handle, shapes, out_w, out_h):
+    def __init__(self, eng, handle, shapes):
         self.eng, self._h = eng, handle
-        self.shapes, self.out_w, self.out_h = list(shapes), out_w, out_h
+        self.shapes = list(shapes)
         self.added = 0
         self._err = None
 
@@ -341,7 +348,7 @@ class BlendStream:
             arrs = list(srcs)
             dts = {a.dtype for a in arrs}
             if len(dts) != 1 or dts.pop() not in (np.uint8, np.float32):
-                self._fail("blend stream: sources must all be uint8 or all float32 numpy arrays")
+                self._fail(f"{self._NAME}: sources must all be uint8 or all float32 numpy arrays")
             u8 = arrs[0].dtype == np.uint8
             kind = SRC_RGB8_HOST if u8 else SRC_F32_HOST
             channels = None
@@ -350,7 +357,7 @@ class BlendStream:
                 ch = 1 if a.ndim == 2 else (a.shape[2] if a.ndim == 3 else -1)
                 if want is None or a.shape[:2] != tuple(want) or (ch not in (1, 3) if u8 else ch != 3) or \
                         (channels is not None and ch != channels):
-                    self._fail(f"blend stream: source {self.added + k} has shape {a.shape}, the stream expects "
+                    self._fail(f"{self._NAME}: source {self.added + k} has shape {a.shape}, the stream expects "
                                f"{want} with {'1 or 3 channels' if u8 else '3 channels'}, the same for the window")
                 channels = ch
                 keep.append(np.ascontiguousarray(a))
@@ -360,8 +367,30 @@ class BlendStream:
             channels = 3 if channels is None else channels
         n = len(ptrs)
         arr = (C.c_void_p * max(n, 1))(*ptrs)
-        self._call(LIB.pano_blend_stream_add(self._h, self.added, n, arr, kind, channels))
+        self._call(type(self)._ADD(self._h, self.added, n, arr, kind, channels))
         self.added += n
+
+    def close(self):
+        if self._h:
+            type(self)._FREE(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class BlendStream(_SourceStream):
+    """A pano_blend_stream: the mosaic of pano_blend, fed window by window (LAZY_READ's memory contract)."""
+    _NAME = "blend stream"
+    _ADD = LIB.pano_blend_stream_add
+    _FREE = LIB.pano_blend_stream_free
+
+    def __init__(self, eng, handle, shapes, out_w, out_h):
+        super().__init__(eng, handle, shapes)
+        self.out_w, self.out_h = out_w, out_h
 
     def finish(self):
         out = np.empty((self.out_h, self.out_w, 3), np.float32)
@@ -371,16 +400,18 @@ class BlendStream:
     def finish_dev(self, d_out):
         self._call(LIB.pano_blend_stream_finish_dev(self._h, C.c_void_p(d_out or 0)))
 
-    def close(self):
-        if self._h:
-            LIB.pano_blend_stream_free(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+class SiftStream(_SourceStream):
+    """A pano_sift_stream: the featureset of sift_detect_batch (sift_detect_batch_rgb8 for uint8 sources), fed
+    window by window (LAZY_READ's feature stage).  At most PANO_MAX_SIFT_BATCH images per add."""
+    _NAME = "sift stream"
+    _ADD = LIB.pano_sift_stream_add
+    _FREE = LIB.pano_sift_stream_free
+
+    def finish(self) -> FeatureSet:
+        out = C.c_void_p()
+        self._call(LIB.pano_sift_stream_finish(self._h, C.byref(out)))
+        return FeatureSet(self.eng, out)
 
 
 class Engine:
@@ -568,6 +599,33 @@ class Engine:
             return fs.download(0)
         finally:
             fs.free()
+
+    def sift_stream(self, shapes, params=None) -> SiftStream:
+        """shapes: (h, w) per image.  Detects with `params` window by window; finish() returns the featureset."""
+        params = params or default_params()
+        n = len(shapes)
+        ws = (C.c_int * max(n, 1))(*[int(s[1]) for s in shapes])
+        hs = (C.c_int * max(n, 1))(*[int(s[0]) for s in shapes])
+        h = C.c_void_p()
+        self._check(LIB.pano_sift_stream_create(self._h, n, ws, hs, C.byref(params), C.byref(h)))
+        return SiftStream(self, h, [tuple(s[:2]) for s in shapes])
+
+    def sift_lazy(self, imgs, window=1, params=None) -> FeatureSet:
+        """sift_detect_batch (uint8 sources: sift_detect_batch_rgb8) with the sources added `window` images at a
+        time (an int, or a list of window sizes): numpy uint8 (H×W, H×W×1 or H×W×3) or float32 H×W×3 images.
+        The images of one window share one channel count."""
+        sizes = window if isinstance(window, (list, tuple)) else None
+        s = self.sift_stream([im.shape[:2] for im in imgs], params)
+        try:
+            k = 0
+            for q in (sizes if sizes is not None else iter(lambda: window, None)):
+                if k >= len(imgs):
+                    break
+                s.add(imgs[k:k + q])
+                k += q
+            return s.finish()
+        finally:
+            s.close()
 
     def sift_trace(self, img, params=None) -> GpuSiftTrace:
         params = params or default_params()

@@ -706,26 +706,18 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
 // ------------------------------------------------------------------ blend stream
 // LAZY_READ's memory contract (blender.cc:38-64, multiband.cc:27,49): sources arrive window by
 // window and are dropped after their window.  State: the canvas (linear: sums + weight plane;
-// multiband: BlendDev's level buffers and masks) plus at most two windows of host sources in a
-// two-slot device ring.  Window k's upload runs on the stream's copy stream into slot k & 1 while
-// window k-1's kernels run on the context's stream; events order the slot's reuse.
+// multiband: BlendDev's level buffers and masks) plus at most two windows of host sources in the
+// upload ring (common.cuh): window k's upload runs while window k-1's kernels run.
 struct pano_blend_stream {
-  // the copy stream drains before the staging and slot memory go
-  ~pano_blend_stream() { if (copy) cudaStreamSynchronize(copy.get()); }
   pano_ctx* ctx = nullptr;
   int n = 0, bands = 0, lazy = 0, ordered = 0;
   BlendJob job;
   BlendDev dev;
   DevBuf<float> d_sum;         // linear: tw×th×3 Σ c·w
   DevBuf<float> d_wsum;        // linear: tw×th Σ w
-  int added = 0, windows = 0, err = 0;
+  int added = 0, err = 0;
   bool finished = false;
-  StreamPtr copy;
-  EventPtr ev_copied[2];   // slot's upload done (copy stream)
-  EventPtr ev_done[2];     // slot's last reader done (context stream)
-  DevBuf<unsigned char> slot[2];
-  size_t slot_cap[2] = {0, 0};
-  PinnedBuf stage[2];      // pinned staging of pageable sources
+  UploadRing ring;
 };
 
 // every failure is sticky: the canvas state is undefined after it
@@ -737,46 +729,17 @@ static int stream_fail(pano_blend_stream* s, int rc) { s->err = rc; return rc; }
     if (_e != cudaSuccess) return stream_fail((s), ctx_cuda((s)->ctx, _e, #call)); \
   } while (0)
 
-// Uploads host window `win` (count images from srcs) into ring slot windows & 1; points win[] at it.
+// Uploads host window `win` (count images from srcs) into the ring; points win[] at it.
 static int stream_upload(pano_blend_stream* s, int first, int count, const void* const* srcs, bool u8, int channels,
                          BlendImg* win, int* slot_out) {
-  pano_ctx* ctx = s->ctx;
-  const int b = s->windows & 1;
-  std::vector<size_t> bytes(count), off(count);
-  size_t total = 0;
-  bool all_pinned = true;
+  std::vector<size_t> bytes(count);
+  std::vector<const void*> d_src(count);
   for (int k = 0; k < count; ++k) {
     const BlendImg& im = s->job.imgs[first + k];
     bytes[k] = (size_t)im.w * im.h * (u8 ? channels : 3 * sizeof(float));
-    off[k] = total;
-    total += align_up(bytes[k], 256);
-    all_pinned = all_pinned && host_is_pinned(srcs[k]);
   }
-  // slot b and its staging were last used by window - 2: its upload must be over before the host
-  // refills the staging buffer (an event never recorded counts as complete)
-  STREAM_CUDA(s, cudaEventSynchronize(s->ev_copied[b].get()));
-  if (s->slot_cap[b] < total) {
-    s->slot[b].reset(); s->slot_cap[b] = 0;
-    if (int rc = s->slot[b].alloc(ctx, total)) return stream_fail(s, rc);
-    s->slot_cap[b] = total;
-    STREAM_CUDA(s, cudaEventRecord(s->ev_done[b].get(), ctx->stream));   // the block is ours from here on the context stream
-  }
-  if (!all_pinned) STREAM_CUDA(s, s->stage[b].grow(total, total, cudaHostAllocDefault));
-  // the copy must not overwrite the slot before window - 2's kernels have read it
-  STREAM_CUDA(s, cudaStreamWaitEvent(s->copy.get(), s->ev_done[b].get(), 0));
-  unsigned char* stage = (unsigned char*)s->stage[b].get();
-  for (int k = 0; k < count; ++k) {
-    const void* src = srcs[k];
-    if (!host_is_pinned(src)) {               // pageable: staged, the caller may reuse it on return
-      memcpy(stage + off[k], src, bytes[k]);
-      src = stage + off[k];
-    }
-    STREAM_CUDA(s, cudaMemcpyAsync(s->slot[b] + off[k], src, bytes[k], cudaMemcpyHostToDevice, s->copy.get()));
-    win[k].pix = s->slot[b] + off[k];
-  }
-  STREAM_CUDA(s, cudaEventRecord(s->ev_copied[b].get(), s->copy.get()));
-  STREAM_CUDA(s, cudaStreamWaitEvent(ctx->stream, s->ev_copied[b].get(), 0));
-  *slot_out = b;
+  if (int rc = s->ring.upload(s->ctx, count, srcs, bytes.data(), d_src.data(), slot_out)) return stream_fail(s, rc);
+  for (int k = 0; k < count; ++k) win[k].pix = (const unsigned char*)d_src[k];
   return PANO_OK;
 }
 
@@ -883,11 +846,7 @@ int pano_blend_stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs,
     PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx * 3 + 255) / 256), 256, 0, s->d_sum, npx * 3, 0.f);
     PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx + 255) / 256), 256, 0, s->d_wsum, npx, 0.f);
   }
-  cudaError_t e = make_stream(&s->copy);
-  for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
-    e = make_event(&s->ev_copied[b], cudaEventDisableTiming);
-    if (e == cudaSuccess) e = make_event(&s->ev_done[b], cudaEventDisableTiming);
-  }
+  cudaError_t e = s->ring.init();
   if (e != cudaSuccess) return ctx_cuda(ctx, e, "blend stream: copy stream / events");
   *out = s.release();
   return PANO_OK;
@@ -920,10 +879,7 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
   if ((rc = ctx_put(ctx, d_win, win.data(), count * sizeof(BlendImg)))) return stream_fail(s, rc);
   rc = u8 ? stream_launch<SrcRgb8>(s, d_win, win.data(), count) : stream_launch<SrcF32>(s, d_win, win.data(), count);
   if (rc) return stream_fail(s, rc);
-  if (slot >= 0) {
-    STREAM_CUDA(s, cudaEventRecord(s->ev_done[slot].get(), ctx->stream));
-    ++s->windows;
-  }
+  if (slot >= 0) STREAM_CUDA(s, s->ring.release(ctx, slot));
   s->added += count;
   return PANO_OK;
 }

@@ -221,6 +221,29 @@ int  ctx_copy_blocks(pano_ctx* ctx, int n, void* const* dst, const void* const* 
 void ctx_prof_begin(pano_ctx* ctx, const char* name);
 void ctx_prof_end(pano_ctx* ctx);
 
+// Two-slot device ring for windows of host sources (pano_blend_stream, pano_sift_stream): window k's upload runs
+// on the ring's own copy stream into slot k & 1 while earlier windows' kernels run on the context's stream;
+// events order each slot's reuse, so at most two windows of sources are resident.  Each slot is as large as the
+// largest window uploaded through it; pageable sources go through a pinned staging buffer per slot.
+struct UploadRing {
+  // the copy stream drains before the staging and slot memory go
+  ~UploadRing() { if (copy) cudaStreamSynchronize(copy.get()); }
+  cudaError_t init();
+  // Uploads count host sources of bytes[k] each into the next slot and points d_src[k] at their device copies;
+  // the context's stream waits for the upload.  *slot_out: the slot, to hand to release().
+  int upload(pano_ctx* ctx, int count, const void* const* srcs, const size_t* bytes, const void** d_src, int* slot_out);
+  // The slot's last reader has been queued on the context's stream: the upload two windows on may overwrite it.
+  cudaError_t release(pano_ctx* ctx, int slot);
+
+  StreamPtr copy;
+  EventPtr ev_copied[2];   // slot's upload done (copy stream)
+  EventPtr ev_done[2];     // slot's last reader done (context stream)
+  DevBuf<unsigned char> slot[2];
+  size_t slot_cap[2] = {0, 0};
+  PinnedBuf stage[2];      // pinned staging of pageable sources
+  int windows = 0;         // windows uploaded so far
+};
+
 // Diagnostics (PANO_TRACE_SLOW_MS=<ms>): report every wrapped driver-facing call that blocks the host
 // longer than the threshold — which call a stall sits in, not how long the GPU takes.
 double pano_now_ms();

@@ -378,6 +378,57 @@ int ctx_copy_blocks(pano_ctx* ctx, int n, void* const* dst, const void* const* s
   return PANO_OK;
 }
 
+cudaError_t UploadRing::init() {
+  cudaError_t e = make_stream(&copy);
+  for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
+    e = make_event(&ev_copied[b], cudaEventDisableTiming);
+    if (e == cudaSuccess) e = make_event(&ev_done[b], cudaEventDisableTiming);
+  }
+  return e;
+}
+
+int UploadRing::upload(pano_ctx* ctx, int count, const void* const* srcs, const size_t* bytes, const void** d_src,
+                       int* slot_out) {
+  const int b = windows & 1;
+  std::vector<size_t> off(count);
+  size_t total = 0;
+  bool all_pinned = true;
+  for (int k = 0; k < count; ++k) {
+    off[k] = total;
+    total += align_up(bytes[k], 256);
+    all_pinned = all_pinned && host_is_pinned(srcs[k]);
+  }
+  // slot b and its staging were last used by window - 2: its upload must be over before the host
+  // refills the staging buffer (an event never recorded counts as complete)
+  PANO_CUDA(ctx, cudaEventSynchronize(ev_copied[b].get()));
+  if (slot_cap[b] < total) {
+    slot[b].reset(); slot_cap[b] = 0;
+    if (int rc = slot[b].alloc(ctx, total)) return rc;
+    slot_cap[b] = total;
+    PANO_CUDA(ctx, cudaEventRecord(ev_done[b].get(), ctx->stream));   // the block is ours from here on the context stream
+  }
+  if (!all_pinned) PANO_CUDA(ctx, stage[b].grow(total, total, cudaHostAllocDefault));
+  // the copy must not overwrite the slot before window - 2's kernels have read it
+  PANO_CUDA(ctx, cudaStreamWaitEvent(copy.get(), ev_done[b].get(), 0));
+  unsigned char* st = (unsigned char*)stage[b].get();
+  for (int k = 0; k < count; ++k) {
+    const void* src = srcs[k];
+    if (!host_is_pinned(src)) {               // pageable: staged, the caller may reuse it on return
+      memcpy(st + off[k], src, bytes[k]);
+      src = st + off[k];
+    }
+    PANO_CUDA(ctx, cudaMemcpyAsync(slot[b] + off[k], src, bytes[k], cudaMemcpyHostToDevice, copy.get()));
+    d_src[k] = slot[b] + off[k];
+  }
+  PANO_CUDA(ctx, cudaEventRecord(ev_copied[b].get(), copy.get()));
+  PANO_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev_copied[b].get(), 0));
+  ++windows;
+  *slot_out = b;
+  return PANO_OK;
+}
+
+cudaError_t UploadRing::release(pano_ctx* ctx, int b) { return cudaEventRecord(ev_done[b].get(), ctx->stream); }
+
 static EventPtr get_event(pano_ctx* ctx) {
   EventPtr e;
   if (!ctx->event_pool.empty()) { e = std::move(ctx->event_pool.back()); ctx->event_pool.pop_back(); }
@@ -617,6 +668,14 @@ void pano_event_destroy(pano_event* ev) {
 
 // ---------------------------------------------------------------- features
 
+int ctx_sift_cap(pano_ctx* ctx) {
+  if (ctx->sift_cap <= 0) {
+    const char* e = getenv("PANO_SIFT_CAP");            // test hook: start small to exercise the growth path
+    ctx->sift_cap = e ? std::max(256, atoi(e)) : SIFT_CAP_DEFAULT;
+  }
+  return ctx->sift_cap;
+}
+
 // channels == nullptr: h×w×3 f32 device images; otherwise h×w×channels[i] u8 device images
 static int sift_detect_dev(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w,
                            const int* h, const pano_params* p, pano_featureset** out) {
@@ -625,11 +684,7 @@ static int sift_detect_dev(pano_ctx* ctx, int n, const void* const* d_src, const
   // kept for the capacity retry of featureset_sync_counts
   fs->src.assign(d_src, d_src + n); fs->src_w.assign(w, w + n); fs->src_h.assign(h, h + n); fs->src_params = *p;
   if (channels) fs->src_channels.assign(channels, channels + n);
-  if (ctx->sift_cap <= 0) {
-    const char* e = getenv("PANO_SIFT_CAP");            // test hook: start small to exercise the growth path
-    ctx->sift_cap = e ? std::max(256, atoi(e)) : SIFT_CAP_DEFAULT;
-  }
-  int rc = sift_run_batch(ctx, n, d_src, channels, w, h, p, fs.get(), nullptr, ctx->sift_cap);
+  int rc = sift_run_batch(ctx, n, d_src, channels, w, h, p, fs.get(), nullptr, ctx_sift_cap(ctx));
   if (rc != 0) return rc;
   *out = fs.release();
   return PANO_OK;

@@ -116,3 +116,5 @@ struct pano_featureset {
 int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w, const int* h,
                    const pano_params* p, pano_featureset* fs, std::unique_ptr<SiftWork>* keep, int cap);
 int featureset_sync_counts(pano_featureset* fs);
+// the per-image list capacity the context's SIFT runs start with (PANO_SIFT_CAP on first use, then grown)
+extern "C" int ctx_sift_cap(pano_ctx* ctx);

@@ -109,6 +109,41 @@ class B200SIFTDetector : public pano::FeatureDetector {
     c_.check(pano_sift_detect_batch_rgb8(c_.get(), n, pix.data(), w.data(), h.data(), channels.data(), &p, &fs));
     return unpack_batch(fs, n, keep);
   }
+  // calc_feature()'s LAZY_READ branch (stitcherbase.cc:14-19): the images are loaded `window` at a time, handed to a
+  // pano_sift_stream and released before the next window is loaded, so at most one window of Mat32f is resident on
+  // the host and two on the device.  Returns detect_batch's descriptors on the same images, bit for bit, and every
+  // image is released afterwards.  The stream takes every shape up front and an ImageRef knows its shape only once
+  // loaded, so an image that is not loaded yet is first loaded and released once on its own.
+  std::vector<std::vector<pano::Descriptor>> detect_lazy(std::vector<pano::ImageRef>& imgs, int window,
+                                                         pano_featureset** keep = nullptr) const {
+    const int n = (int)imgs.size();
+    if (window < 1) window = 1;
+    std::vector<int> w(n), h(n);
+    for (int k = 0; k < n; ++k) {
+      const bool resident = imgs[k].img != nullptr;
+      imgs[k].load();
+      w[k] = imgs[k].width(); h[k] = imgs[k].height();
+      if (!resident) imgs[k].release();
+    }
+    pano_params p = snapshot_params();
+    pano_sift_stream* s = nullptr;
+    c_.check(pano_sift_stream_create(c_.get(), n, w.data(), h.data(), &p, &s));
+    for (int k0 = 0; k0 < n; k0 += window) {
+      const int k1 = std::min(n, k0 + window);
+      std::vector<const void*> src;
+      for (int k = k0; k < k1; ++k) {
+        imgs[k].load();
+        src.push_back(imgs[k].img->ptr());
+      }
+      // Mat32f storage is pageable: the stream stages it before returning
+      c_.check(pano_sift_stream_add(s, k0, k1 - k0, src.data(), PANO_SRC_F32_HOST, 3));
+      for (int k = k0; k < k1; ++k) imgs[k].release();
+    }
+    pano_featureset* fs = nullptr;
+    c_.check(pano_sift_stream_finish(s, &fs));
+    pano_sift_stream_free(s);
+    return unpack_batch(fs, n, keep);
+  }
  private:
   std::vector<std::vector<pano::Descriptor>> unpack_batch(pano_featureset* fs, int n, pano_featureset** keep) const {
     std::vector<std::vector<pano::Descriptor>> feats(n);
