@@ -123,6 +123,8 @@ def _load():
         "pano_rgb8_to_mat32f_batch_dev": (C.c_int, [C.c_void_p, C.c_int, _vpp, _ip, _ip, _ip, _vpp]),
         "pano_crop_rect_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
         "pano_mat32f_to_rgb8_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+        "pano_mat32f_to_pix8_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                              C.c_void_p]),
         "pano_dev_alloc": (C.c_int, [C.c_void_p, C.c_size_t, _vpp]),
         "pano_dev_free": (C.c_int, [C.c_void_p, C.c_void_p]),
         "pano_dev_upload": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
@@ -315,6 +317,38 @@ class BaSession:
 # pano_src_kind
 SRC_F32_DEV, SRC_F32_HOST, SRC_RGB8_DEV, SRC_RGB8_HOST = 0, 1, 2, 3
 
+# PANO_PIX_*: the pixel formats of decoded 8-bit images, passed where the 8-bit entry points take `channels`
+PIX_GREY, PIX_RGB, PIX_RGBA, PIX_RGB_PLANAR = 1, 3, 0x104, 0x203
+# the `fmt` keyword of the numpy methods: "rgba" selects lodepng's H×W×4 buffers, "planar" CImg's 3×H×W planes;
+# None keeps the inference from the shape (H×W or H×W×1 grey, H×W×3 interleaved RGB)
+PIX_FORMATS = {"grey": PIX_GREY, "rgb": PIX_RGB, "rgba": PIX_RGBA, "planar": PIX_RGB_PLANAR}
+
+
+def pix_format(a, fmt=None):
+    """(PANO_PIX_* code, h, w) of a uint8 array read in layout `fmt`; raises PanoError if the shape does not fit."""
+    if fmt is None:
+        if a.ndim == 2 or (a.ndim == 3 and a.shape[2] == 1):
+            return PIX_GREY, a.shape[0], a.shape[1]
+        if a.ndim == 3 and a.shape[2] == 3:
+            return PIX_RGB, a.shape[0], a.shape[1]
+    elif fmt not in PIX_FORMATS:
+        raise PanoError(-2, f"unknown pixel format {fmt!r} (one of {sorted(PIX_FORMATS)})")
+    elif fmt == "planar":
+        if a.ndim == 3 and a.shape[0] == 3:
+            return PIX_RGB_PLANAR, a.shape[1], a.shape[2]
+    else:
+        code = PIX_FORMATS[fmt]
+        if code == PIX_GREY and a.ndim == 2:
+            return code, a.shape[0], a.shape[1]
+        if a.ndim == 3 and a.shape[2] == {PIX_GREY: 1, PIX_RGB: 3, PIX_RGBA: 4}[code]:
+            return code, a.shape[0], a.shape[1]
+    raise PanoError(-2, f"8-bit source of shape {a.shape} does not fit format {fmt or 'grey / rgb'}: expected H×W or "
+                        "H×W×{1,3}, H×W×4 with fmt='rgba', 3×H×W with fmt='planar'")
+
+
+def _fmt_list(fmt, n):
+    return list(fmt) if isinstance(fmt, (list, tuple)) else [fmt] * n
+
 
 class _SourceStream:
     """What the windowed streams share: add() takes numpy arrays (host; uint8 H×W / H×W×1 / H×W×3 or float32
@@ -339,8 +373,9 @@ class _SourceStream:
             self._err = PanoError(rc, LIB.pano_last_error(self.eng._h).decode())
             raise self._err
 
-    def add(self, srcs, kind=None, channels=None):
-        """Adds the next len(srcs) images."""
+    def add(self, srcs, kind=None, channels=None, fmt=None):
+        """Adds the next len(srcs) images.  fmt ("rgba" or "planar", see pix_format) reads uint8 arrays in that
+        layout; raw pointers take a PANO_PIX_* code as `channels`."""
         if self._err is not None:
             raise self._err
         keep = []
@@ -354,8 +389,17 @@ class _SourceStream:
             channels = None
             for k, a in enumerate(arrs):
                 want = self.shapes[self.added + k] if self.added + k < len(self.shapes) else None
-                ch = 1 if a.ndim == 2 else (a.shape[2] if a.ndim == 3 else -1)
-                if want is None or a.shape[:2] != tuple(want) or (ch not in (1, 3) if u8 else ch != 3) or \
+                if u8 and fmt is not None:
+                    try:
+                        ch, ah, aw = pix_format(a, fmt)
+                    except PanoError as e:
+                        self._fail(f"{self._NAME}: source {self.added + k}: {e}")
+                    a_hw = (ah, aw)
+                else:
+                    ch = 1 if a.ndim == 2 else (a.shape[2] if a.ndim == 3 else -1)
+                    a_hw = a.shape[:2]
+                if want is None or a_hw != tuple(want) or (ch not in (1, 3) if u8 and fmt is None else
+                                                           (not u8 and ch != 3)) or \
                         (channels is not None and ch != channels):
                     self._fail(f"{self._NAME}: source {self.added + k} has shape {a.shape}, the stream expects "
                                f"{want} with {'1 or 3 channels' if u8 else '3 channels'}, the same for the window")
@@ -412,6 +456,24 @@ class SiftStream(_SourceStream):
         out = C.c_void_p()
         self._call(LIB.pano_sift_stream_finish(self._h, C.byref(out)))
         return FeatureSet(self.eng, out)
+
+
+def _lazy_windows(imgs, window, fmt):
+    """The windows of sift_lazy / blend_lazy as (first, count, fmt), and every image's (h, w): window is an int or
+    a list of sizes, fmt one value or a list with one per window (see pix_format)."""
+    sizes = window if isinstance(window, (list, tuple)) else None
+    wins, k = [], 0
+    for q, n in enumerate(sizes if sizes is not None else iter(lambda: window, None)):
+        if k >= len(imgs):
+            break
+        wins.append((k, n, fmt[q] if isinstance(fmt, (list, tuple)) else fmt))
+        k += n
+    shapes = [im.shape[:2] for im in imgs]
+    for k0, n, f in wins:
+        for i in range(k0, min(k0 + n, len(imgs))):
+            if f is not None and imgs[i].dtype == np.uint8:
+                shapes[i] = pix_format(imgs[i], f)[1:]
+    return wins, shapes
 
 
 class Engine:
@@ -568,20 +630,19 @@ class Engine:
         self._check(fn(self._h, n, cp, cw, ch, C.byref(params), C.byref(out)))
         return FeatureSet(self, out)
 
-    def sift_detect_batch_rgb8(self, pix, params=None) -> FeatureSet:
-        """SIFT straight from decoded 8-bit pixels (numpy uint8 H×W, H×W×1 or H×W×3, read_img's input):
-        the features of sift_detect_batch on read_img's f32 images, without those images."""
+    def sift_detect_batch_rgb8(self, pix, params=None, fmt=None) -> FeatureSet:
+        """SIFT straight from decoded 8-bit pixels (numpy uint8 H×W, H×W×1 or H×W×3, read_img's input; with
+        fmt="rgba" lodepng's H×W×4, with fmt="planar" CImg's 3×H×W; fmt may be a list, one per image): the
+        features of sift_detect_batch on read_img's f32 images, without those images."""
         pix = [np.ascontiguousarray(x, np.uint8) for x in pix]
-        for x in pix:
-            if not (x.ndim == 2 or (x.ndim == 3 and x.shape[2] in (1, 3))):
-                raise PanoError(-2, f"sift rgb8: expected H×W or H×W×{{1,3}} uint8, got shape {x.shape}")
-        return self.sift_detect_batch_rgb8_ptr([x.ctypes.data for x in pix], [x.shape[1] for x in pix],
-                                               [x.shape[0] for x in pix], [1 if x.ndim == 2 else x.shape[2] for x in pix],
-                                               params)
+        fm = [pix_format(x, f) for x, f in zip(pix, _fmt_list(fmt, len(pix)))]
+        return self.sift_detect_batch_rgb8_ptr([x.ctypes.data for x in pix], [f[2] for f in fm], [f[1] for f in fm],
+                                               [f[0] for f in fm], params)
 
     def sift_detect_batch_rgb8_ptr(self, ptrs, ws, hs, channels, params=None, device=False) -> FeatureSet:
-        """Raw-pointer variant: h×w×channels u8 images in host memory (pageable or pinned) or, with device=True,
-        in device memory (valid until the first count query / download / match of the featureset)."""
+        """Raw-pointer variant: 8-bit images in host memory (pageable or pinned) or, with device=True, in device
+        memory (valid until the first count query / download / match of the featureset); channels: one PANO_PIX_*
+        code per image (1 or 3 for H×W×channels)."""
         params = params or default_params()
         n = len(ptrs)
         cp = (C.c_void_p * max(n, 1))(*ptrs)
@@ -610,19 +671,15 @@ class Engine:
         self._check(LIB.pano_sift_stream_create(self._h, n, ws, hs, C.byref(params), C.byref(h)))
         return SiftStream(self, h, [tuple(s[:2]) for s in shapes])
 
-    def sift_lazy(self, imgs, window=1, params=None) -> FeatureSet:
+    def sift_lazy(self, imgs, window=1, params=None, fmt=None) -> FeatureSet:
         """sift_detect_batch (uint8 sources: sift_detect_batch_rgb8) with the sources added `window` images at a
         time (an int, or a list of window sizes): numpy uint8 (H×W, H×W×1 or H×W×3) or float32 H×W×3 images.
-        The images of one window share one channel count."""
-        sizes = window if isinstance(window, (list, tuple)) else None
-        s = self.sift_stream([im.shape[:2] for im in imgs], params)
+        The images of one window share one channel count.  fmt: see pix_format; a list gives one per window."""
+        wins, shapes = _lazy_windows(imgs, window, fmt)
+        s = self.sift_stream(shapes, params)
         try:
-            k = 0
-            for q in (sizes if sizes is not None else iter(lambda: window, None)):
-                if k >= len(imgs):
-                    break
-                s.add(imgs[k:k + q])
-                k += q
+            for k, q, f in wins:
+                s.add(imgs[k:k + q], fmt=f)
             return s.finish()
         finally:
             s.close()
@@ -874,18 +931,15 @@ class Engine:
                                                  oh.value, C.byref(h)))
         return BlendStream(self, h, shapes, ow.value, oh.value)
 
-    def blend_lazy(self, imgs, items, geom, bands=0, params=None, window=1):
+    def blend_lazy(self, imgs, items, geom, bands=0, params=None, window=1, fmt=None):
         """blend() with the sources added `window` images at a time (an int, or a list of window sizes):
-        numpy uint8 (read_img's input: H×W, H×W×1 or H×W×3) or float32 H×W×3 images."""
-        sizes = window if isinstance(window, (list, tuple)) else None
-        s = self.blend_stream([im.shape[:2] for im in imgs], items, geom, bands, params)
+        numpy uint8 (read_img's input: H×W, H×W×1 or H×W×3) or float32 H×W×3 images.  fmt: see pix_format; a
+        list gives one per window."""
+        wins, shapes = _lazy_windows(imgs, window, fmt)
+        s = self.blend_stream(shapes, items, geom, bands, params)
         try:
-            k = 0
-            for q in (sizes if sizes is not None else iter(lambda: window, None)):
-                if k >= len(imgs):
-                    break
-                s.add(imgs[k:k + q])
-                k += q
+            for k, q, f in wins:
+                s.add(imgs[k:k + q], fmt=f)
             return s.finish()
         finally:
             s.close()
@@ -927,11 +981,17 @@ class Engine:
         self._check(LIB.pano_mat32f_to_rgb8_dev(self._h, C.c_void_p(d_mat), w, h, C.c_void_p(d_rect or 0),
                                                 C.c_void_p(d_out)))
 
+    def mat32f_to_pix8_dev(self, d_mat, w, h, d_rect, fmt, d_out):
+        """The same conversion in an encoder's layout: fmt is a PANO_PIX_* code or "rgb" / "rgba" (write_png's
+        buffer, alpha 255) / "planar" (write_rgb's CImg planes), packed to the rectangle's size."""
+        code = PIX_FORMATS.get(fmt, fmt) if isinstance(fmt, str) else fmt
+        self._check(LIB.pano_mat32f_to_pix8_dev(self._h, C.c_void_p(d_mat), w, h, C.c_void_p(d_rect or 0), int(code),
+                                                C.c_void_p(d_out)))
+
     # numpy conveniences for tests
-    def read_img_rgb8(self, pix):
+    def read_img_rgb8(self, pix, fmt=None):
         pix = np.ascontiguousarray(pix, np.uint8)
-        h, w = pix.shape[:2]
-        ch = 1 if pix.ndim == 2 else pix.shape[2]
+        ch, h, w = pix_format(pix, fmt)
         d_in = self.dev_alloc(max(pix.nbytes, 256))
         d_out = self.dev_alloc(h * w * 12)
         out = np.empty((h, w, 3), np.float32)
@@ -968,3 +1028,31 @@ class Engine:
             return None, out.reshape(h, w, 3)
         cw, ch = int(rect[2]), int(rect[3])
         return rect, out[:cw * ch * 3].reshape(ch, cw, 3).copy()
+
+    def crop_write_pix8(self, mat, crop=True, fmt="rgb"):
+        """crop_write_rgb8 with the pixels in layout fmt: "rgb" (ch×cw×3), "rgba" (ch×cw×4, alpha 255) or
+        "planar" (3×ch×cw)."""
+        mat = np.ascontiguousarray(mat, np.float32)
+        h, w = mat.shape[:2]
+        code = PIX_FORMATS[fmt]
+        bpp = 4 if code == PIX_RGBA else 3
+        d_mat = self.dev_alloc(mat.nbytes)
+        d_rect = self.dev_alloc(256)
+        d_out = self.dev_alloc(max(h * w * bpp, 256))
+        rect = np.zeros(4, np.int32)
+        out = np.empty(h * w * bpp, np.uint8)
+        try:
+            self.dev_upload(d_mat, mat)
+            if crop:
+                self.crop_rect_dev(d_mat, w, h, d_rect)
+            self.mat32f_to_pix8_dev(d_mat, w, h, d_rect if crop else 0, code, d_out)
+            self.dev_download(out, d_out)
+            if crop:
+                self.dev_download(rect, d_rect)
+        finally:
+            for p_ in (d_mat, d_rect, d_out):
+                self.dev_free(p_)
+        cw, ch = (int(rect[2]), int(rect[3])) if crop else (w, h)
+        px = out[:cw * ch * bpp]
+        px = px.reshape(3, ch, cw) if code == PIX_RGB_PLANAR else px.reshape(ch, cw, bpp)
+        return (rect if crop else None), px.copy()

@@ -20,7 +20,7 @@
 struct BlendImg {
   union {
     const float* rgb;           // device, h×w×3 f32 (SrcF32)
-    const unsigned char* pix;   // device, h×w×channels u8 (SrcRgb8)
+    const unsigned char* pix;   // device, 8-bit pixels in format `channels` (SrcRgb8 / SrcPix8)
   };
   int w, h;
   int x0, y0, x1, y1;
@@ -32,13 +32,16 @@ struct BlendImg {
   long long plane;        // floats per plane (pitch * rh)
   long long mask_off;     // first byte of the validity mask (same pitch)
   int rw, rh, pitch;
-  int channels;           // SrcRgb8 only: 1 or 3
+  int channels;           // 8-bit sources only: the PANO_PIX_* format
 };
 
 template <class Src> __device__ __forceinline__ Src blend_src(const BlendImg& im, const float* lut);
 template <> __device__ __forceinline__ SrcF32 blend_src<SrcF32>(const BlendImg& im, const float*) { return SrcF32{im.rgb}; }
 template <> __device__ __forceinline__ SrcRgb8 blend_src<SrcRgb8>(const BlendImg& im, const float* lut) {
   return SrcRgb8{im.pix, lut, im.channels};
+}
+template <> __device__ __forceinline__ SrcPix8 blend_src<SrcPix8>(const BlendImg& im, const float* lut) {
+  return SrcPix8{im.pix, lut, im.channels, (size_t)im.w * im.h};
 }
 
 struct BlendGeom {
@@ -510,8 +513,9 @@ static int blend_plan(pano_ctx* ctx, int n, const pano_blend_image* imgs, const 
     const pano_blend_image& s = imgs[k];
     if ((need_src && !s.rgb_hwc) || s.w < 2 || s.h < 2 || s.x1 < s.x0 || s.y1 < s.y0 || s.x0 < 0 || s.y0 < 0)
       return ctx_fail(ctx, PANO_ERR_INVALID, "blend: image %d has an invalid shape or range", k);
-    if (pix && (!pix[k] || (channels[k] != 1 && channels[k] != 3)))
-      return ctx_fail(ctx, PANO_ERR_INVALID, "blend: image %d has no pixels or %d channels (1 or 3)", k, channels[k]);
+    if (pix && !pix[k]) return ctx_fail(ctx, PANO_ERR_INVALID, "blend: image %d has no pixels", k);
+    if (pix)
+      if (int rc = pix8_check(ctx, "blend", k, channels[k], pix[k])) return rc;
     job->tw = std::max(job->tw, s.x1); job->th = std::max(job->th, s.y1);
     BlendImg d;
     memset(&d, 0, sizeof(d));
@@ -667,14 +671,16 @@ static int blend_run(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands,
                      int row0, int row1) {
   const int n = (int)job.imgs.size(), tw = job.tw;
   const dim3 b(32, 8);   // 256 threads: the 8-bit kernels' conversion table
+  constexpr bool pix8 = std::is_same<Src, SrcPix8>::value;
   if (bands == 0) {
     dim3 gs(ceil_div(tw, 32), ceil_div(row1 - row0, 8));
-    PANO_LAUNCH(ctx, Src::kLut ? "k_linear_blend_rgb8" : "k_linear_blend", k_linear_blend<Src>, gs, b, 0, d->d_imgs, n,
-              job.g, p->lazy_read, p->ordered_input, d_out, tw, row0, row1);
+    PANO_LAUNCH(ctx, pix8 ? "k_linear_blend_pix8" : Src::kLut ? "k_linear_blend_rgb8" : "k_linear_blend",
+                k_linear_blend<Src>, gs, b, 0, d->d_imgs, n, job.g, p->lazy_read, p->ordered_input, d_out, tw, row0, row1);
     return PANO_OK;
   }
   dim3 gr(ceil_div(job.max_rw, 32), ceil_div(job.max_rh, 8), n);
-  PANO_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<Src>, gr, b, 0, d->d_imgs, job.g, d->d_cur, d->d_mask);
+  PANO_LAUNCH(ctx, pix8 ? "k_mb_first_level_pix8" : "k_mb_first_level", k_mb_first_level<Src>, gr, b, 0, d->d_imgs, job.g,
+              d->d_cur, d->d_mask);
   return mb_levels(ctx, job, d, bands, d_out, row0, row1);
 }
 
@@ -699,6 +705,8 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
   }
   BlendDev dev;
   if ((rc = blend_dev_setup(ctx, &job, bands, row0, row1, &dev))) return rc;
+  if (pix && std::any_of(channels, channels + n, pix8_layout))
+    return blend_run<SrcPix8>(ctx, job, &dev, bands, p, d_out, row0, row1);
   return pix ? blend_run<SrcRgb8>(ctx, job, &dev, bands, p, d_out, row0, row1)
              : blend_run<SrcF32>(ctx, job, &dev, bands, p, d_out, row0, row1);
 }
@@ -736,7 +744,7 @@ static int stream_upload(pano_blend_stream* s, int first, int count, const void*
   std::vector<const void*> d_src(count);
   for (int k = 0; k < count; ++k) {
     const BlendImg& im = s->job.imgs[first + k];
-    bytes[k] = (size_t)im.w * im.h * (u8 ? channels : 3 * sizeof(float));
+    bytes[k] = (size_t)im.w * im.h * (u8 ? (size_t)pix8_bytes(channels) : 3 * sizeof(float));
   }
   if (int rc = s->ring.upload(s->ctx, count, srcs, bytes.data(), d_src.data(), slot_out)) return stream_fail(s, rc);
   for (int k = 0; k < count; ++k) win[k].pix = (const unsigned char*)d_src[k];
@@ -748,6 +756,7 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
   pano_ctx* ctx = s->ctx;
   const BlendJob& job = s->job;
   const dim3 b(32, 8);
+  constexpr bool pix8 = std::is_same<Src, SrcPix8>::value;
   if (s->bands == 0) {
     // bounding rectangle of the window on the canvas (inclusive ranges: a superset of both range rules)
     int x0 = INT_MAX, y0 = INT_MAX, x1 = 0, y1 = 0;
@@ -758,13 +767,14 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
     x1 = std::min(x1, job.tw); y1 = std::min(y1, job.th);
     if (x0 >= x1 || y0 >= y1) return PANO_OK;
     dim3 g(ceil_div(x1 - x0, 32), ceil_div(y1 - y0, 8));
-    PANO_LAUNCH(ctx, "k_linear_accumulate", k_linear_accumulate<Src>, g, b, 0, d_win, count, job.g, s->lazy, s->ordered,
-              s->d_sum, s->d_wsum, job.tw, x0, y0, x1, y1);
+    PANO_LAUNCH(ctx, pix8 ? "k_linear_accumulate_pix8" : "k_linear_accumulate", k_linear_accumulate<Src>, g, b, 0, d_win,
+                count, job.g, s->lazy, s->ordered, s->d_sum, s->d_wsum, job.tw, x0, y0, x1, y1);
   } else {
     int rw = 0, rh = 0;
     for (int k = 0; k < count; ++k) { rw = std::max(rw, win[k].rw); rh = std::max(rh, win[k].rh); }
     dim3 g(ceil_div(rw, 32), ceil_div(rh, 8), count);
-    PANO_LAUNCH(ctx, "k_mb_first_level", k_mb_first_level<Src>, g, b, 0, d_win, job.g, s->dev.d_cur, s->dev.d_mask);
+    PANO_LAUNCH(ctx, pix8 ? "k_mb_first_level_pix8" : "k_mb_first_level", k_mb_first_level<Src>, g, b, 0, d_win, job.g,
+                s->dev.d_cur, s->dev.d_mask);
   }
   return PANO_OK;
 }
@@ -866,8 +876,11 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
   const bool u8 = kind == PANO_SRC_RGB8_DEV || kind == PANO_SRC_RGB8_HOST;
   const bool host = kind == PANO_SRC_F32_HOST || kind == PANO_SRC_RGB8_HOST;
   if (!u8 && kind != PANO_SRC_F32_DEV && kind != PANO_SRC_F32_HOST) return STREAM_MISUSE(s, "blend stream: unknown source kind %d", kind);
-  if (u8 ? (channels != 1 && channels != 3) : channels != 3)
-    return STREAM_MISUSE(s, "blend stream: %d channels for source kind %d", channels, kind);
+  if (u8 ? !pix8_bytes(channels) : channels != 3)
+    return STREAM_MISUSE(s, "blend stream: format %#x for source kind %d", channels, kind);
+  if (kind == PANO_SRC_RGB8_DEV && channels == PANO_PIX_RGBA)
+    for (int k = 0; k < count; ++k)
+      if (int rc = pix8_check(ctx, "blend stream", first + k, channels, srcs[k])) return stream_fail(s, rc);
   std::vector<BlendImg> win(s->job.imgs.begin() + first, s->job.imgs.begin() + first + count);
   for (int k = 0; k < count; ++k) {
     win[k].pix = (const unsigned char*)srcs[k];
@@ -877,7 +890,9 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
   if (host && (rc = stream_upload(s, first, count, srcs, u8, channels, win.data(), &slot))) return rc;
   BlendImg* d_win = s->dev.d_imgs + first;
   if ((rc = ctx_put(ctx, d_win, win.data(), count * sizeof(BlendImg)))) return stream_fail(s, rc);
-  rc = u8 ? stream_launch<SrcRgb8>(s, d_win, win.data(), count) : stream_launch<SrcF32>(s, d_win, win.data(), count);
+  rc = !u8 ? stream_launch<SrcF32>(s, d_win, win.data(), count)
+     : pix8_layout(channels) ? stream_launch<SrcPix8>(s, d_win, win.data(), count)
+                             : stream_launch<SrcRgb8>(s, d_win, win.data(), count);
   if (rc) return stream_fail(s, rc);
   if (slot >= 0) STREAM_CUDA(s, s->ring.release(ctx, slot));
   s->added += count;

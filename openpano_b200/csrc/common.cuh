@@ -281,6 +281,23 @@ struct __align__(64) TmaDesc { unsigned long long opaque[16]; };
 int ctx_tma_encode(pano_ctx* ctx, TmaDesc* out, void* base, int rank, const unsigned long long* dims,
                    const unsigned long long* strides_bytes, const unsigned* box);
 
+// The 8-bit source formats (PANO_PIX_*, pano_b200.h): bytes per pixel, 0 for a value no 8-bit entry point
+// takes.  Every 8-bit entry point, stream and staging size goes through these.
+static inline int pix8_bytes(int fmt) {
+  switch (fmt) {
+    case PANO_PIX_GREY: return 1;
+    case PANO_PIX_RGB: return 3;
+    case PANO_PIX_RGBA: return 4;
+    case PANO_PIX_RGB_PLANAR: return 3;
+    default: return 0;
+  }
+}
+// RGBA and planar images are read through SrcPix8; grey and interleaved RGB through SrcRgb8
+static inline bool pix8_layout(int fmt) { return fmt == PANO_PIX_RGBA || fmt == PANO_PIX_RGB_PLANAR; }
+// Checks image i's format and, for device sources (d_pix non-null), the 4-byte alignment an RGBA tap load
+// needs; fails the context with `what` in the message.
+int pix8_check(pano_ctx* ctx, const char* what, int i, int fmt, const void* d_pix);
+
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 // gridDim.y for `count` items (at least 1 block).  CUDA refuses a grid.y above 65,535, so kernels whose
 // y index is an input count (pairs, sides, segments) loop: item = blockIdx.y; item < count; item += gridDim.y.
@@ -456,6 +473,38 @@ struct SrcRgb8 {
       const unsigned char* p10 = p00 + (size_t)w * 3;
 #pragma unroll
       for (int k = 0; k < 6; ++k) { q[k] = lut[__ldg(p00 + k)]; q[6 + k] = lut[__ldg(p10 + k)]; }
+    }
+  }
+};
+// 8-bit pixels in any PANO_PIX_* layout (pano_b200.h), one format per image: what a batch that holds an
+// RGBA or planar image reads through (a batch of grey and interleaved RGB images keeps SrcRgb8).  RGBA is
+// what lodepng::decode returns (read_png, lib/imgio.cc:43-61): every colour sample through the table, the
+// fourth byte ignored, one 32-bit load per tap (the caller guarantees 4-byte alignment).  Planar is
+// CImg<unsigned char>'s layout (imgio.cc:72-88): three w×h planes R, G, B, `plane` bytes apart.
+struct SrcPix8 {
+  const unsigned char* pix;
+  const float* lut;
+  int fmt;
+  size_t plane;   // w * h: the planar layout's plane stride
+  static constexpr bool kMayBeNo = false, kLut = true;
+  __device__ __forceinline__ void fetch(int w, int fr, int fc, float* q) const {
+    if (fmt == PANO_PIX_RGBA) {
+      const unsigned* p00 = reinterpret_cast<const unsigned*>(pix) + (size_t)fr * w + fc;
+      const unsigned t[4] = {__ldg(p00), __ldg(p00 + 1), __ldg(p00 + w), __ldg(p00 + w + 1)};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        q[3 * k] = lut[t[k] & 0xff]; q[3 * k + 1] = lut[(t[k] >> 8) & 0xff]; q[3 * k + 2] = lut[(t[k] >> 16) & 0xff];
+      }
+    } else if (fmt == PANO_PIX_RGB_PLANAR) {
+      const unsigned char* p00 = pix + (size_t)fr * w + fc;
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const unsigned char* p = p00 + ch * plane;
+        q[ch] = lut[__ldg(p)]; q[3 + ch] = lut[__ldg(p + 1)];
+        q[6 + ch] = lut[__ldg(p + w)]; q[9 + ch] = lut[__ldg(p + w + 1)];
+      }
+    } else {
+      SrcRgb8{pix, lut, fmt}.fetch(w, fr, fc, q);
     }
   }
 };

@@ -22,6 +22,15 @@ int ctx_fail(pano_ctx* ctx, int code, const char* fmt, ...) {
   return code;
 }
 
+int pix8_check(pano_ctx* ctx, const char* what, int i, int fmt, const void* d_pix) {
+  if (!pix8_bytes(fmt))
+    return ctx_fail(ctx, PANO_ERR_INVALID, "%s: image %d has format %#x (PANO_PIX_GREY, _RGB, _RGBA or _RGB_PLANAR)",
+                    what, i, fmt);
+  if (d_pix && fmt == PANO_PIX_RGBA && (reinterpret_cast<uintptr_t>(d_pix) & 3))
+    return ctx_fail(ctx, PANO_ERR_INVALID, "%s: image %d: an RGBA source must be 4-byte aligned", what, i);
+  return PANO_OK;
+}
+
 int ctx_cuda(pano_ctx* ctx, cudaError_t e, const char* what) {
   return ctx_fail(ctx, PANO_ERR_CUDA, "CUDA error %s (%s) at %s", cudaGetErrorName(e), cudaGetErrorString(e), what);
 }
@@ -676,7 +685,7 @@ int ctx_sift_cap(pano_ctx* ctx) {
   return ctx->sift_cap;
 }
 
-// channels == nullptr: h×w×3 f32 device images; otherwise h×w×channels[i] u8 device images
+// channels == nullptr: h×w×3 f32 device images; otherwise 8-bit device images in PANO_PIX_* format channels[i]
 static int sift_detect_dev(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w,
                            const int* h, const pano_params* p, pano_featureset** out) {
   std::unique_ptr<pano_featureset> fs(new pano_featureset);
@@ -707,7 +716,8 @@ bool host_is_pinned(const void* p) {
 
 // Uploads host images through one pinned staging buffer (async H2D on the ctx
 // stream), then runs the device path.  channels == nullptr: h×w×3 f32 images; otherwise
-// h×w×channels[i] u8 images.  Every image starts on a 256-byte boundary of d_block.
+// 8-bit images in format channels[i].  Every image starts on a 256-byte boundary of d_block (so RGBA taps
+// are aligned).
 static int upload_images(pano_ctx* ctx, int n, const void* const* src, const int* channels, const int* w, const int* h,
                          std::vector<const void*>& d_imgs, DevBuf<unsigned char>& d_block) {
   size_t total = 0;
@@ -715,7 +725,7 @@ static int upload_images(pano_ctx* ctx, int n, const void* const* src, const int
   for (int i = 0; i < n; ++i) {
     if (!src[i] || w[i] <= 0 || h[i] <= 0) return ctx_fail(ctx, PANO_ERR_INVALID, "image %d: null or empty", i);
     offs[i] = total;
-    bytes[i] = (size_t)w[i] * h[i] * (channels ? (size_t)channels[i] : 3 * sizeof(float));
+    bytes[i] = (size_t)w[i] * h[i] * (channels ? (size_t)pix8_bytes(channels[i]) : 3 * sizeof(float));
     total += align_up(bytes[i], 256);
   }
   if (int rc = d_block.alloc(ctx, total)) return rc;
@@ -760,13 +770,13 @@ int pano_sift_detect_batch(pano_ctx* ctx, int n, const float* const* rgb, const 
 }
 
 // Checks of the 8-bit entry points: the f32 ones take any pointer, these reject what they cannot read.
+// device: pix are device pointers (an RGBA source must be 4-byte aligned); host sources are staged aligned.
 static int rgb8_args_ok(pano_ctx* ctx, int n, const unsigned char* const* pix, const int* w, const int* h,
-                        const int* channels, const pano_params* p) {
+                        const int* channels, const pano_params* p, bool device) {
   if (n <= 0 || !pix || !w || !h || !channels || !p) return ctx_fail(ctx, PANO_ERR_INVALID, "sift rgb8: bad argument");
   for (int i = 0; i < n; ++i) {
     if (!pix[i]) return ctx_fail(ctx, PANO_ERR_INVALID, "sift rgb8: image %d is null", i);
-    if (channels[i] != 1 && channels[i] != 3)
-      return ctx_fail(ctx, PANO_ERR_INVALID, "sift rgb8: image %d has %d channels (1 or 3)", i, channels[i]);
+    if (int rc = pix8_check(ctx, "sift rgb8", i, channels[i], device ? pix[i] : nullptr)) return rc;
     if (w[i] < 2 || h[i] < 2) return ctx_fail(ctx, PANO_ERR_INVALID, "sift rgb8: image %d is %dx%d (at least 2x2)", i, w[i], h[i]);
   }
   return PANO_OK;
@@ -777,7 +787,7 @@ int pano_sift_detect_batch_rgb8_dev(pano_ctx* ctx, int n, const unsigned char* c
   ctx_enter(ctx);
   if (!ctx || !out) return PANO_ERR_INVALID;
   *out = nullptr;
-  int rc = rgb8_args_ok(ctx, n, d_pix, w, h, channels, p);
+  int rc = rgb8_args_ok(ctx, n, d_pix, w, h, channels, p, true);
   if (rc) return rc;
   return sift_detect_dev(ctx, n, (const void* const*)d_pix, channels, w, h, p, out);
 }
@@ -787,7 +797,7 @@ int pano_sift_detect_batch_rgb8(pano_ctx* ctx, int n, const unsigned char* const
   ctx_enter(ctx);
   if (!ctx || !out) return PANO_ERR_INVALID;
   *out = nullptr;
-  int rc = rgb8_args_ok(ctx, n, pix, w, h, channels, p);
+  int rc = rgb8_args_ok(ctx, n, pix, w, h, channels, p, false);
   if (rc) return rc;
   return sift_detect_host(ctx, n, (const void* const*)pix, channels, w, h, p, out);
 }

@@ -10,7 +10,7 @@ struct Rgb8Job {
   const unsigned char* src;
   float* dst;
   long long n_px;
-  int channels;
+  int channels;   // the PANO_PIX_* format
   int pad;
 };
 
@@ -45,6 +45,33 @@ __global__ void __launch_bounds__(256) k_rgb8_to_f32(const Rgb8Job* __restrict__
       job.dst[i * 3 + 1] = v;
       job.dst[i * 3 + 2] = v;
     }
+  }
+}
+
+// The same for a batch that holds RGBA or planar images (any format per image), one pixel per thread and
+// trip: RGBA (read_png, imgio.cc:43-61) is one 32-bit load whose fourth byte is ignored, planar (CImg,
+// imgio.cc:72-88) reads the pixel's byte of each plane.  Every colour sample goes through the table except
+// grey's, which is replicated undivided.
+__global__ void __launch_bounds__(256) k_pix8_to_f32(const Rgb8Job* __restrict__ jobs) {
+  __shared__ float lut[256];
+  const Rgb8Job job = jobs[blockIdx.y];
+  lut[threadIdx.x] = (float)((double)threadIdx.x / 255.0);
+  __syncthreads();
+  const unsigned char* src = job.src;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < job.n_px; i += (long long)gridDim.x * blockDim.x) {
+    float r, g, b;
+    if (job.channels == PANO_PIX_RGBA) {
+      const unsigned t = __ldg(reinterpret_cast<const unsigned*>(src) + i);
+      r = lut[t & 0xff]; g = lut[(t >> 8) & 0xff]; b = lut[(t >> 16) & 0xff];
+    } else if (job.channels == PANO_PIX_RGB_PLANAR) {
+      r = lut[__ldg(src + i)]; g = lut[__ldg(src + job.n_px + i)]; b = lut[__ldg(src + 2 * job.n_px + i)];
+    } else if (job.channels == PANO_PIX_RGB) {
+      r = lut[__ldg(src + 3 * i)]; g = lut[__ldg(src + 3 * i + 1)]; b = lut[__ldg(src + 3 * i + 2)];
+    } else {
+      r = g = b = (float)__ldg(src + i);
+    }
+    float* d = job.dst + i * 3;
+    d[0] = r; d[1] = g; d[2] = b;
   }
 }
 
@@ -313,6 +340,34 @@ __global__ void __launch_bounds__(256) k_f32_to_rgb8(const float* __restrict__ m
   }
 }
 
+// k_f32_to_rgb8's samples in an encoder's layout: PANO_PIX_RGBA rows of 4 bytes per pixel with alpha 255
+// (write_png, imgio.cc:25-41), or PANO_PIX_RGB_PLANAR, three planes of the rectangle's size (write_rgb's
+// CImg<unsigned char>, imgio.cc:98-113).
+template <int FMT>
+__global__ void __launch_bounds__(256) k_f32_to_pix8(const float* __restrict__ mat, int w, int h,
+                                                     const int* __restrict__ rect, unsigned char* __restrict__ out) {
+  int x0 = 0, y0 = 0, cw = w, ch = h;
+  if (rect) { x0 = rect[0]; y0 = rect[1]; cw = rect[2]; ch = rect[3]; }
+  const long long n = (long long)cw * ch;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int r = (int)(i / cw), c = (int)(i - (long long)r * cw);
+    const float* p = mat + ((size_t)(r + y0) * w + (c + x0)) * 3;
+    unsigned char o[3];
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      float v = p[q];
+      v = (v < 0 ? 1.0f : v) * 255.0f;
+      o[q] = (unsigned char)(int)v;
+    }
+    if (FMT == PANO_PIX_RGBA) {
+      unsigned char* d = out + i * 4;
+      d[0] = o[0]; d[1] = o[1]; d[2] = o[2]; d[3] = 255;
+    } else {
+      out[i] = o[0]; out[n + i] = o[1]; out[2 * n + i] = o[2];
+    }
+  }
+}
+
 // ------------------------------------------------------------------ C API
 extern "C" {
 
@@ -327,10 +382,12 @@ int pano_rgb8_to_mat32f_batch_dev(pano_ctx* ctx, int n, const unsigned char* con
   if (n == 0) return PANO_OK;
   std::vector<Rgb8Job> jobs(n);
   long long max_px = 0;
+  bool layouts = false;   // an RGBA or planar image: k_pix8_to_f32
   for (int i = 0; i < n; ++i) {
-    if (w[i] <= 0 || h[i] <= 0 || (channels[i] != 1 && channels[i] != 3) || !d_pix[i] || !d_out_hwc[i])
-      return ctx_fail(ctx, PANO_ERR_INVALID, "pano_rgb8_to_mat32f_batch_dev: image %d: w=%d h=%d channels=%d", i, w[i], h[i],
-                      channels[i]);
+    if (w[i] <= 0 || h[i] <= 0 || !d_pix[i] || !d_out_hwc[i])
+      return ctx_fail(ctx, PANO_ERR_INVALID, "pano_rgb8_to_mat32f_batch_dev: image %d: w=%d h=%d", i, w[i], h[i]);
+    if (int rc = pix8_check(ctx, "pano_rgb8_to_mat32f_batch_dev", i, channels[i], d_pix[i])) return rc;
+    layouts = layouts || pix8_layout(channels[i]);
     if ((reinterpret_cast<uintptr_t>(d_pix[i]) & 3) || (reinterpret_cast<uintptr_t>(d_out_hwc[i]) & 15))
       return ctx_fail(ctx, PANO_ERR_INVALID, "pano_rgb8_to_mat32f_batch_dev: image %d: source must be 4-byte and "
                       "destination 16-byte aligned", i);
@@ -340,9 +397,10 @@ int pano_rgb8_to_mat32f_batch_dev(pano_ctx* ctx, int n, const unsigned char* con
   DevBuf<Rgb8Job> d_jobs;
   if (int rc = d_jobs.alloc(ctx, n)) return rc;
   if (int rc = ctx_put(ctx, d_jobs, jobs.data(), sizeof(Rgb8Job) * n)) return rc;
-  long long per_img = (max_px * 3 / 4 + 255) / 256;
+  long long per_img = ((layouts ? max_px : max_px * 3 / 4) + 255) / 256;
   int gx = (int)std::min<long long>(std::max<long long>(per_img, 1), std::max(1, ctx->num_sms * 8 / n));
-  PANO_LAUNCH(ctx, "k_rgb8_to_f32", k_rgb8_to_f32, dim3(gx, n), 256, 0, d_jobs);
+  if (layouts) PANO_LAUNCH(ctx, "k_pix8_to_f32", k_pix8_to_f32, dim3(gx, n), 256, 0, d_jobs);
+  else PANO_LAUNCH(ctx, "k_rgb8_to_f32", k_rgb8_to_f32, dim3(gx, n), 256, 0, d_jobs);
   return PANO_OK;
 }
 
@@ -380,6 +438,23 @@ int pano_mat32f_to_rgb8_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h,
   long long blocks = ((long long)w * h + 255) / 256;
   int grid = (int)std::min<long long>(blocks, (long long)ctx->num_sms * 16);
   PANO_LAUNCH(ctx, "k_f32_to_rgb8", k_f32_to_rgb8, grid, 256, 0, d_mat_hwc, w, h, d_rect, d_out);
+  return PANO_OK;
+}
+
+int pano_mat32f_to_pix8_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h, const int* d_rect, int format,
+                            unsigned char* d_out) {
+  ctx_enter(ctx);
+  if (!ctx || !d_mat_hwc || !d_out || w <= 0 || h <= 0)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "pano_mat32f_to_pix8_dev: bad argument");
+  if (format == PANO_PIX_RGB) return pano_mat32f_to_rgb8_dev(ctx, d_mat_hwc, w, h, d_rect, d_out);
+  if (format != PANO_PIX_RGBA && format != PANO_PIX_RGB_PLANAR)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "pano_mat32f_to_pix8_dev: format %#x (PANO_PIX_RGB, _RGBA or _RGB_PLANAR)", format);
+  long long blocks = ((long long)w * h + 255) / 256;
+  int grid = (int)std::min<long long>(blocks, (long long)ctx->num_sms * 16);
+  if (format == PANO_PIX_RGBA)
+    PANO_LAUNCH(ctx, "k_f32_to_rgba8", k_f32_to_pix8<PANO_PIX_RGBA>, grid, 256, 0, d_mat_hwc, w, h, d_rect, d_out);
+  else
+    PANO_LAUNCH(ctx, "k_f32_to_planar8", k_f32_to_pix8<PANO_PIX_RGB_PLANAR>, grid, 256, 0, d_mat_hwc, w, h, d_rect, d_out);
   return PANO_OK;
 }
 

@@ -53,7 +53,7 @@ __device__ __forceinline__ int first_tap_at_least(int t, float inv, int src_n, i
 //     (first_tap_at_least).  Its upper tap, at most h0-1 / w0-1, is the halo at the latest.
 // Every stored value comes from the same float operations on the same operands as the reference's
 // resize and rgb2grey (no FMA contraction, --fmad=false), so every plane is bit-identical to them.
-// Src = SrcRgb8: every tap is the f32 value read_img would have stored (common.cuh), so the
+// Src = SrcRgb8 / SrcPix8: every tap is the f32 value read_img would have stored (common.cuh), so the
 // bilinear sample of those taps is the sample of read_img's image.
 // work: null, or the arena when a trace keeps the working RGB image (at im.work_off).
 template <class Src>
@@ -72,7 +72,8 @@ __global__ void __launch_bounds__(PG_THREADS) k_pyramid_grey(const ImgMeta* __re
   if constexpr (Src::kLut) {
     build_rgb8_lut(lut, threadIdx.x);
     __syncthreads();
-    src = Src{im.pix, lut, im.channels};
+    if constexpr (std::is_same<Src, SrcPix8>::value) src = Src{im.pix, lut, im.channels, (size_t)im.in_w * im.in_h};
+    else src = Src{im.pix, lut, im.channels};
   } else {
     src = Src{im.src};
   }
@@ -1242,8 +1243,8 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
     tilespan.resize((size_t)n * n_oct);
     for (int i = 0; i < n; ++i) {
       if (w[i] < 2 || h[i] < 2) return ctx_fail(ctx, PANO_ERR_INVALID, "sift: image too small");
-      if (channels && (channels[i] != 1 && channels[i] != 3))
-        return ctx_fail(ctx, PANO_ERR_INVALID, "sift: image %d has %d channels (1 or 3)", i, channels[i]);
+      if (channels)
+        if (int rc = pix8_check(ctx, "sift", i, channels[i], nullptr)) return rc;
       ImgMeta& im = wk->h_img[i];
       im.channels = channels ? channels[i] : 3;
       im.in_w = w[i]; im.in_h = h[i];
@@ -1365,7 +1366,9 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
   {
     dim3 g(ceil_div(plan->max_w0, PG_TW), ceil_div(plan->max_h0, PG_TH), n);
     float* work = keep ? wk->arena.get() : nullptr;
-    if (channels)
+    if (channels && std::any_of(channels, channels + n, pix8_layout))
+      PANO_LAUNCH(ctx, "k_pyramid_grey_pix8", k_pyramid_grey<SrcPix8>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);
+    else if (channels)
       PANO_LAUNCH(ctx, "k_pyramid_grey_rgb8", k_pyramid_grey<SrcRgb8>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);
     else
       PANO_LAUNCH(ctx, "k_pyramid_grey", k_pyramid_grey<SrcF32>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);

@@ -16,13 +16,13 @@
 struct ImgMeta {
   union {
     const float* src;           // input, h×w×3 f32 (device)
-    const unsigned char* pix;   // input, h×w×channels u8 (device), read as SrcRgb8 reads it
+    const unsigned char* pix;   // input, 8-bit pixels in format `channels` (device), read as SrcRgb8 / SrcPix8 read them
   };
   int in_w, in_h;
   int w0, h0;         // working size
   float ifx, ify;     // 1/fx (rows), 1/fy (cols) of the working resize
   long long work_off; // working RGB offset in the arena (floats); a trace's arena only holds it
-  int channels;       // u8 sources only: 1 or 3
+  int channels;       // u8 sources only: the PANO_PIX_* format
 };
 
 struct OctMeta {
@@ -106,13 +106,13 @@ struct pano_featureset {
   // the sources must stay valid until the counts have been read once (pano_b200.h).
   int cap = 0;                          // per-image row capacity of d_desc / d_coor (0: not a SIFT set)
   std::vector<const void*> src;         // device images
-  std::vector<int> src_channels;        // u8 sources: channels per image; empty: f32 sources
+  std::vector<int> src_channels;        // u8 sources: PANO_PIX_* format per image; empty: f32 sources
   std::vector<int> src_w, src_h;
   pano_params src_params;
   DevBuf<unsigned char> owned_block;    // staged upload of the host entry points, freed after the count sync
 };
 
-// d_src: h×w×3 f32 device images when channels is null, else h×w×channels[i] u8 device images
+// d_src: h×w×3 f32 device images when channels is null, else 8-bit device images in format channels[i]
 int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* channels, const int* w, const int* h,
                    const pano_params* p, pano_featureset* fs, std::unique_ptr<SiftWork>* keep, int cap);
 int featureset_sync_counts(pano_featureset* fs);

@@ -101,16 +101,16 @@ __global__ void k_cyl_warp(const float* __restrict__ src, int w, int h, float* _
 
 // The same for a batch of device-resident images: blockIdx.z = image; per-image parameters and the
 // two per-column tables (concatenated) sit in device memory.  Src = SrcF32 reads h×w×3 f32 images,
-// Src = SrcRgb8 reads h×w×channels u8 pixels and converts every tap as read_img converts it, so the
-// warp of the pixels is the warp of read_img's f32 image, bit for bit.
+// Src = SrcRgb8 (SrcPix8 when a batch holds RGBA or planar images) reads 8-bit pixels and converts every
+// tap as read_img converts it, so the warp of the pixels is the warp of read_img's f32 image, bit for bit.
 struct CylJobDev {
   union {
     const float* src;           // SrcF32
-    const unsigned char* pix;   // SrcRgb8
+    const unsigned char* pix;   // SrcRgb8 / SrcPix8
   };
   float* dst;
   int w, h, ow, oh;
-  int channels;                 // SrcRgb8 only: 1 or 3
+  int channels;                 // 8-bit sources only: the PANO_PIX_* format
   long long tab_off;            // first entry of this image's col_x[ow] followed by col_cos[ow]
   double r, cy, offy, sizefactor_inv;
 };
@@ -119,6 +119,9 @@ template <class Src> __device__ __forceinline__ Src cyl_src(const CylJobDev& jb,
 template <> __device__ __forceinline__ SrcF32 cyl_src<SrcF32>(const CylJobDev& jb, const float*) { return SrcF32{jb.src}; }
 template <> __device__ __forceinline__ SrcRgb8 cyl_src<SrcRgb8>(const CylJobDev& jb, const float* lut) {
   return SrcRgb8{jb.pix, lut, jb.channels};
+}
+template <> __device__ __forceinline__ SrcPix8 cyl_src<SrcPix8>(const CylJobDev& jb, const float* lut) {
+  return SrcPix8{jb.pix, lut, jb.channels, (size_t)jb.w * jb.h};
 }
 
 template <class Src>
@@ -162,9 +165,9 @@ static int cyl_warp_batch(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double
     const pano_cyl_job& jb = jobs[k];
     if ((!pix && !jb.d_rgb_hwc) || !jb.d_out_hwc || jb.w <= 1 || jb.h <= 1 || jb.n_kpts < 0 || (jb.n_kpts && !jb.kpts_xy))
       return ctx_fail(ctx, PANO_ERR_INVALID, "cyl_warp_batch: job %d has a null pointer or an empty image", k);
-    if (pix && (!pix[k] || (channels[k] != 1 && channels[k] != 3)))
-      return ctx_fail(ctx, PANO_ERR_INVALID, "cyl_warp_batch rgb8: job %d has no pixels or %d channels (1 or 3)", k,
-                      channels[k]);
+    if (pix && !pix[k]) return ctx_fail(ctx, PANO_ERR_INVALID, "cyl_warp_batch rgb8: job %d has no pixels", k);
+    if (pix)
+      if (int rc = pix8_check(ctx, "cyl_warp_batch rgb8", k, channels[k], pix[k])) return rc;
     CylProj c = get_projector(jb.w, jb.h, h_factor, p);
     if (c.r <= 0) return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder radius <= 0");
     int sw = jb.w, sh = jb.h;
@@ -198,7 +201,9 @@ static int cyl_warp_batch(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double
   if ((rc = ctx_put(ctx, d_jobs, dj.data(), dj.size() * sizeof(CylJobDev)))) return rc;
   if ((rc = ctx_put(ctx, d_tabs, tabs.data(), tabs.size() * sizeof(double)))) return rc;
   dim3 b(32, 8), g(ceil_div(max_ow, 32), ceil_div(max_oh, 8), n);   // 256 threads: the 8-bit conversion table
-  if (pix) PANO_LAUNCH(ctx, "k_cyl_warp_rgb8", k_cyl_warp_batch<SrcRgb8>, g, b, 0, d_jobs, d_tabs);
+  if (pix && std::any_of(channels, channels + n, pix8_layout))
+    PANO_LAUNCH(ctx, "k_cyl_warp_pix8", k_cyl_warp_batch<SrcPix8>, g, b, 0, d_jobs, d_tabs);
+  else if (pix) PANO_LAUNCH(ctx, "k_cyl_warp_rgb8", k_cyl_warp_batch<SrcRgb8>, g, b, 0, d_jobs, d_tabs);
   else PANO_LAUNCH(ctx, "k_cyl_warp", k_cyl_warp_batch<SrcF32>, g, b, 0, d_jobs, d_tabs);
   return PANO_OK;   // stream-ordered: the blocks are released after the kernel
 }

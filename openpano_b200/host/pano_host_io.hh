@@ -1,0 +1,145 @@
+// pano_host_io.hh — the drop-in's file boundary in the reference's own codecs (lib/imgio.cc), apart from
+// pano_host.hh so that CImg and lodepng only enter the translation units that read or write files.
+//   load_pixels       read_img's decode (imgio.cc:67-90) without its f32 conversion: the decoder's own buffer
+//                     and format, lodepng's RGBA for a .png, CImg's planes (or grey) otherwise
+//   B200PixelBlender  B200LazyBlender's blend (LinearBlender / MultiBandBlender, bit for bit) from such buffers
+//   write_mosaic      crop + write_rgb of main.cc:226-234 from a device mosaic: the 8-bit conversion on the
+//                     device, lodepng::encode for a .png, CImg::save otherwise
+// The buffers go to B200SIFTDetector::detect_batch_rgb8, B200PixelBlender or the streams (pano_b200.h) with
+// their format as the `channels` argument; no Mat32f of a source is built.  Include after the reference's
+// headers are on the include path (-I <reference>/src -isystem <reference>/src/third-party), as pano_host.hh.
+#pragma once
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "pano_host.hh"
+
+#ifndef cimg_display
+#define cimg_display 0
+#endif
+#if !defined(DISABLE_JPEG) && !defined(cimg_use_jpeg)
+#define cimg_use_jpeg   // read_img's CImg reads JPEG unless the reference is built with -DDISABLE_JPEG
+#endif
+// lib/debugutils.hh's one-letter macros (P, PP, PA) collide with CImg's identifiers; imgio.cc includes CImg first
+#pragma push_macro("P")
+#pragma push_macro("PP")
+#pragma push_macro("PA")
+#undef P
+#undef PP
+#undef PA
+#include "CImg.h"
+#pragma pop_macro("PA")
+#pragma pop_macro("PP")
+#pragma pop_macro("P")
+#include "lodepng/lodepng.h"
+#include "lib/utils.hh"
+
+namespace pano_b200 {
+
+// One decoded image as the reference's decoder left it: h×w×4 (PANO_PIX_RGBA), three h×w planes
+// (PANO_PIX_RGB_PLANAR) or h×w (PANO_PIX_GREY).
+struct Pixels {
+  std::vector<unsigned char> data;
+  int w = 0, h = 0;
+  int format = PANO_PIX_RGB;
+  const unsigned char* ptr() const { return data.data(); }
+};
+
+// read_img's file handling (imgio.cc:67-90), same checks and messages, without building the Mat32f.
+inline Pixels load_pixels(const char* fname) {
+  if (!exists_file(fname)) error_exit(ssprintf("File \"%s\" not exists!", fname));
+  Pixels px;
+  if (endswith(fname, ".png")) {
+    unsigned w = 0, h = 0;
+    const unsigned error = lodepng::decode(px.data, w, h, fname);
+    if (error) error_exit(ssprintf("png encoder error %u: %s", error, lodepng_error_text(error)));
+    px.w = (int)w; px.h = (int)h; px.format = PANO_PIX_RGBA;
+  } else {
+    cimg_library::CImg<unsigned char> img(fname);
+    m_assert(img.spectrum() == 3 || img.spectrum() == 1);
+    px.w = img.width(); px.h = img.height();
+    px.format = img.spectrum() == 3 ? PANO_PIX_RGB_PLANAR : PANO_PIX_GREY;
+    px.data.assign(img.data(), img.data() + img.size());
+  }
+  m_assert(px.h > 1 && px.w > 1);
+  return px;
+}
+
+// Blends decoded buffers through a pano_blend_stream: the mosaic of LinearBlender / MultiBandBlender (and of
+// B200Blender) on read_img's images of the same files, bit for bit.  Consecutive images of one format go in
+// windows of up to `window`; the caller keeps the buffers until run() returns.
+class B200PixelBlender {
+ public:
+  B200PixelBlender(const Context& c, int bands, int projection, Vec2D resolution, Vec2D proj_min, int window = 1)
+      : c_(c), bands_(bands), window_(window < 1 ? 1 : window) {
+    g_.projection = projection; g_.res_x = resolution.x; g_.res_y = resolution.y;
+    g_.proj_min_x = proj_min.x; g_.proj_min_y = proj_min.y;
+  }
+  void add_image(const Coor& upper_left, const Coor& bottom_right, const Pixels& px, const pano::Homography& homo_inv) {
+    pano_blend_image b;
+    b.rgb_hwc = nullptr; b.w = px.w; b.h = px.h;
+    b.x0 = upper_left.x; b.y0 = upper_left.y; b.x1 = bottom_right.x; b.y1 = bottom_right.y;
+    memcpy(b.homo_inv, homo_inv.data, sizeof(double) * 9);
+    imgs_.push_back(b);
+    px_.push_back(&px);
+  }
+  Mat32f run() {
+    const int n = (int)imgs_.size();
+    int ow = 0, oh = 0;
+    c_.check(pano_blend_target_size(n, imgs_.data(), &ow, &oh));
+    pano_params p = snapshot_params();
+    pano_blend_stream* s = nullptr;
+    c_.check(pano_blend_stream_create(c_.get(), n, imgs_.data(), &g_, bands_, &p, ow, oh, &s));
+    for (int k0 = 0; k0 < n;) {
+      int k1 = k0 + 1;
+      while (k1 < n && k1 - k0 < window_ && px_[k1]->format == px_[k0]->format) ++k1;
+      std::vector<const void*> src;
+      for (int k = k0; k < k1; ++k) src.push_back(px_[k]->ptr());
+      c_.check(pano_blend_stream_add(s, k0, k1 - k0, src.data(), PANO_SRC_RGB8_HOST, px_[k0]->format));
+      k0 = k1;
+    }
+    Mat32f out(oh, ow, 3);
+    c_.check(pano_blend_stream_finish(s, out.ptr()));
+    pano_blend_stream_free(s);
+    return out;
+  }
+ private:
+  const Context& c_;
+  int bands_, window_;
+  pano_blend_geom g_;
+  std::vector<pano_blend_image> imgs_;
+  std::vector<const Pixels*> px_;
+};
+
+// main.cc:226-234 on a device mosaic (h×w×3 f32, Color::NO < 0): crop() when `crop`, then write_rgb(fname).
+// The conversion runs on the device into the encoder's layout; the file is what write_rgb writes, byte for byte.
+inline void write_mosaic(const Context& c, const float* d_mosaic, int w, int h, bool crop, const char* fname) {
+  const bool png = endswith(fname, ".png");
+  const int format = png ? PANO_PIX_RGBA : PANO_PIX_RGB_PLANAR;
+  void* d_rect = nullptr;
+  void* d_out = nullptr;
+  int rect[4] = {0, 0, w, h};
+  c.check(pano_dev_alloc(c.get(), (size_t)w * h * (png ? 4 : 3), &d_out));
+  if (crop) {
+    c.check(pano_dev_alloc(c.get(), sizeof(rect), &d_rect));
+    c.check(pano_crop_rect_dev(c.get(), d_mosaic, w, h, (int*)d_rect));
+  }
+  c.check(pano_mat32f_to_pix8_dev(c.get(), d_mosaic, w, h, (const int*)d_rect, format, (unsigned char*)d_out));
+  if (crop) c.check(pano_dev_download(c.get(), rect, d_rect, sizeof(rect)));
+  const int cw = rect[2], ch = rect[3];
+  std::vector<unsigned char> buf((size_t)cw * ch * (png ? 4 : 3));
+  c.check(pano_dev_download(c.get(), buf.data(), d_out, buf.size()));
+  c.check(pano_dev_free(c.get(), d_out));
+  if (d_rect) c.check(pano_dev_free(c.get(), d_rect));
+  if (png) {
+    const unsigned error = lodepng::encode(fname, buf, (unsigned)cw, (unsigned)ch);
+    if (error) error_exit(ssprintf("png encoder error %u: %s", error, lodepng_error_text(error)));
+  } else {
+    cimg_library::CImg<unsigned char> img(cw, ch, 1, 3);
+    memcpy(img.data(), buf.data(), buf.size());
+    img.save(fname);
+  }
+}
+
+}  // namespace pano_b200

@@ -17,7 +17,7 @@ from __future__ import annotations
 import numpy as np
 
 from ._abi import default_params
-from .capi import Engine
+from .capi import PIX_FORMATS, PIX_RGB, PIX_RGBA, PIX_RGB_PLANAR, Engine
 
 
 from .synth import all_pairs, ordered_pairs  # noqa: F401  (task lists live with the workload generator)
@@ -154,7 +154,8 @@ class PipelinedStitcher:
     host while the match lists come back, and that is when the next upload flies.
     """
 
-    def __init__(self, device: int, params=None, depth: int = 2, rgb8: bool = False, crop: bool = True):
+    def __init__(self, device: int, params=None, depth: int = 2, rgb8: bool = False, crop: bool = True,
+                 in_format: str = "rgb", out_format: str = "rgb"):
         """rgb8: the host side speaks the reference's FILE formats instead of Mat32f —
         decoded 8-bit pixels in (what read_img starts from, imgio.cc:72) and the 8-bit
         mosaic out (what write_rgb saves, imgio.cc:98-113, after crop() when `crop`,
@@ -163,7 +164,17 @@ class PipelinedStitcher:
         f32 copy of an image exists on the device; the output conversion runs there with
         the reference's arithmetic.  The output buffer then
         holds a 256-byte header (int32 x0, y0, width, height of the crop rectangle)
-        followed by height*width*3 packed bytes."""
+        followed by height*width*3 packed bytes.
+
+        in_format / out_format (rgb8 only) select the layouts of the reference's codecs
+        instead of interleaved RGB: "rgba" is lodepng's (read_png's input, imgio.cc:43-61;
+        write_png's output with alpha 255, h*w*4 bytes), "planar" is CImg<unsigned char>'s
+        (three h×w planes R, G, B: read_img's other path and write_rgb's image).  The mosaic
+        is the interleaved path's, re-laid out (unpack_rgb8_mosaic reads it back)."""
+        if in_format not in ("rgb", "rgba", "planar") or out_format not in ("rgb", "rgba", "planar"):
+            raise ValueError(f"in_format / out_format: 'rgb', 'rgba' or 'planar', not {in_format!r} / {out_format!r}")
+        if not rgb8 and (in_format, out_format) != ("rgb", "rgb"):
+            raise ValueError("in_format / out_format need rgb8=True")
         self.params = params or default_params()
         self.up = Engine(device)
         self.cmp = Engine(device)
@@ -171,6 +182,9 @@ class PipelinedStitcher:
         self.depth = depth
         self.rgb8 = rgb8
         self.crop = crop
+        self.in_code, self.out_code = PIX_FORMATS[in_format], PIX_FORMATS[out_format]
+        self.in_bpp = 4 if self.in_code == PIX_RGBA else 3
+        self.out_bpp = 4 if self.out_code == PIX_RGBA else 3
         self.slots = [dict(imgs=None, out=None, shapes=None, offs=None, out_wh=None, pix=None, pix_offs=None, out8=None,
                            ev_up=self.up.event_create(), ev_cmp=self.cmp.event_create(),
                            ev_dn=self.dn.event_create(), busy=False) for _ in range(depth)]
@@ -182,7 +196,7 @@ class PipelinedStitcher:
             realloc = True
             # one device block per slot: the f32 images, or with rgb8 the 8-bit pixels that SIFT and the
             # blend read directly
-            key, offs_key, px = ("pix", "pix_offs", 3) if self.rgb8 else ("imgs", "offs", 12)
+            key, offs_key, px = ("pix", "pix_offs", self.in_bpp) if self.rgb8 else ("imgs", "offs", 12)
             if s[key]:
                 self.cmp.dev_free(s[key])
             offs, total = [], 0
@@ -213,11 +227,11 @@ class PipelinedStitcher:
     def out_bytes(self, out_wh) -> int:
         """Size of the host buffer run() fills for a canvas of out_wh."""
         if self.rgb8:
-            return self.RGB8_HEADER + out_wh[0] * out_wh[1] * 3
+            return self.RGB8_HEADER + out_wh[0] * out_wh[1] * self.out_bpp
         return out_wh[0] * out_wh[1] * 3 * 4
 
     def in_bytes(self, shapes) -> int:
-        return sum(h * w * 3 * (1 if self.rgb8 else 4) for (h, w) in shapes)
+        return sum(h * w * (self.in_bpp if self.rgb8 else 12) for (h, w) in shapes)
 
     def stage(self, host_ptrs, shapes, out_wh) -> int:
         k = self._next
@@ -230,7 +244,7 @@ class PipelinedStitcher:
         self.up.event_wait(s["ev_cmp"])            # its previous compute no longer reads these images
         if self.rgb8:
             for p, o, (h, w) in zip(host_ptrs, s["pix_offs"], shapes):
-                self.up.dev_upload_async(s["pix"] + o, p, h * w * 3)
+                self.up.dev_upload_async(s["pix"] + o, p, h * w * self.in_bpp)
         else:
             for p, o, (h, w) in zip(host_ptrs, s["offs"], shapes):
                 self.up.dev_upload_async(s["imgs"] + o, p, h * w * 3 * 4)
@@ -243,7 +257,7 @@ class PipelinedStitcher:
         ws, hs = [q[1] for q in shapes], [q[0] for q in shapes]
         self.cmp.event_wait(s["ev_up"])
         if self.rgb8:
-            ptrs, chans = [s["pix"] + o for o in s["pix_offs"]], [3] * len(shapes)
+            ptrs, chans = [s["pix"] + o for o in s["pix_offs"]], [self.in_code] * len(shapes)
             fs = self.cmp.sift_detect_batch_rgb8_ptr(ptrs, ws, hs, chans, self.params, device=True)
         else:
             ptrs = [s["imgs"] + o for o in s["offs"]]
@@ -258,7 +272,11 @@ class PipelinedStitcher:
         if self.rgb8:
             if self.crop:
                 self.cmp.crop_rect_dev(s["out"], ow, oh, s["out8"])
-            self.cmp.mat32f_to_rgb8_dev(s["out"], ow, oh, s["out8"] if self.crop else 0, s["out8"] + self.RGB8_HEADER)
+            rect = s["out8"] if self.crop else 0
+            if self.out_code == PIX_RGB:
+                self.cmp.mat32f_to_rgb8_dev(s["out"], ow, oh, rect, s["out8"] + self.RGB8_HEADER)
+            else:
+                self.cmp.mat32f_to_pix8_dev(s["out"], ow, oh, rect, self.out_code, s["out8"] + self.RGB8_HEADER)
         self.cmp.event_record(s["ev_cmp"])
         fs.free()
         self.dn.event_wait(s["ev_cmp"])
@@ -297,15 +315,20 @@ class PipelinedStitcher:
             e.close()
 
 
-def unpack_rgb8_mosaic(buf: np.ndarray, out_wh, cropped: bool = True):
+def unpack_rgb8_mosaic(buf: np.ndarray, out_wh, cropped: bool = True, out_format: str = "rgb"):
     """View of the 8-bit mosaic PipelinedStitcher(rgb8=True).run() wrote into `buf`
-    (uint8, out_bytes long).  Returns (rect (x0, y0, w, h), H×W×3 uint8 view)."""
+    (uint8, out_bytes long).  Returns (rect (x0, y0, w, h), uint8 view): H×W×3, or H×W×4 for
+    out_format "rgba", or 3×H×W for "planar"."""
     hdr = PipelinedStitcher.RGB8_HEADER
     if cropped:
         x0, y0, w, h = (int(v) for v in buf[:16].view(np.int32))
     else:
         x0, y0, w, h = 0, 0, out_wh[0], out_wh[1]
-    return (x0, y0, w, h), buf[hdr:hdr + w * h * 3].reshape(h, w, 3)
+    code = PIX_FORMATS[out_format]
+    if code == PIX_RGB_PLANAR:
+        return (x0, y0, w, h), buf[hdr:hdr + w * h * 3].reshape(3, h, w)
+    bpp = 4 if code == PIX_RGBA else 3
+    return (x0, y0, w, h), buf[hdr:hdr + w * h * bpp].reshape(h, w, bpp)
 
 
 class StitchLanes:
@@ -321,8 +344,10 @@ class StitchLanes:
         results = lanes.map(jobs)     # jobs[i] = (host_ptrs, shapes, out_wh, pairs, items, geom, out_host_ptr, bands)
     """
 
-    def __init__(self, device: int, params=None, lanes: int = 2, depth: int = 2, rgb8: bool = False, crop: bool = True):
-        self.lanes = [PipelinedStitcher(device, params, depth=depth, rgb8=rgb8, crop=crop) for _ in range(lanes)]
+    def __init__(self, device: int, params=None, lanes: int = 2, depth: int = 2, rgb8: bool = False, crop: bool = True,
+                 in_format: str = "rgb", out_format: str = "rgb"):
+        self.lanes = [PipelinedStitcher(device, params, depth=depth, rgb8=rgb8, crop=crop, in_format=in_format,
+                                        out_format=out_format) for _ in range(lanes)]
         self.done_times = []       # perf_counter() at which each job of the last map() came back (diagnostics)
 
     def out_bytes(self, out_wh):
