@@ -501,6 +501,25 @@ int  pano_blend_stream_add(pano_blend_stream* s, int first, int count, const voi
 int  pano_blend_stream_finish_dev(pano_blend_stream* s, float* d_out_hwc);
 int  pano_blend_stream_finish(pano_blend_stream* s, float* out_hwc);
 void pano_blend_stream_free(pano_blend_stream* s);
+/* A blend stream of rows [row0, row1) of the canvas only (0 <= row0 < row1 <= out_h): the strip form of
+ * pano_blend_rows_dev with LAZY_READ's windows.  add and free are as above; finish writes
+ * (row1 - row0)×out_w×3 f32, and the strips of any partition of the canvas, concatenated, are
+ * pano_blend's mosaic bit for bit (every window partition, source kind and PANO_PIX_* format, linear and
+ * multiband).  Its canvas state covers the rows only:
+ *   bands == 0: 16 B per strip pixel;
+ *   bands > 0:  33 B per pixel of each ROI clipped to [row0 - H, row1 + H) (H as for pano_blend_rows_dev)
+ *               plus 1 B per strip pixel; finish adds the 12 B per strip pixel of the output.
+ * The strip needs only the images pano_blend_rows_rgb8_dev reads for it (see pano_blend_stream_needs).  An
+ * add may pass NULL for the others; their sources are never read and take no ring memory, and a window
+ * without a needed image queues nothing.  A NULL source for a needed image is a misuse.  A strip that no
+ * image reaches finishes as all -1. */
+int  pano_blend_stream_create_rows(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g,
+                                   int bands, const pano_params* p, int out_w, int out_h, int row0, int row1,
+                                   pano_blend_stream** out);
+/* flags[k] (k < n) = 1 if the stream reads image k, else 0.  bands > 0: the images whose ROI, clipped to
+ * [row0 - H, row1 + H) on a strip with rows above or below it, keeps a row; bands == 0: the images whose
+ * rows [y0, y1] meet [row0, row1).  A stream of the whole canvas needs every image. */
+int  pano_blend_stream_needs(const pano_blend_stream* s, unsigned char* flags);
 
 /* SIFT whose sources arrive in windows: LAZY_READ's feature stage (config.cfg:10-11, calc_feature in
  * stitcherbase.cc:9-27 loads, detects and releases one image at a time) on the device.  For every
@@ -609,6 +628,18 @@ int pano_rgb8_to_mat32f_batch_dev(pano_ctx* ctx, int n, const unsigned char* con
  * rectangle of pixels whose max(r,g,b) >= 0, first maximum in (line, column)
  * order.  d_rect receives {x0, y0, width, height} (device int[4]). */
 int pano_crop_rect_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h, int* d_rect);
+/* The same rectangle from a mosaic that arrives in row strips, top to bottom, for widths up to 80,000 (the
+ * reference's limit on a mosaic's edge; pano_crop_rect_dev takes 40,000).  Between adds the scan keeps
+ * O(w) ints and the best rectangle so far on the device.  add: d_strip_hwc is the next `rows` lines of the
+ * w-wide f32 mosaic, read by work queued on the ctx stream.  rect: valid once all h lines have been added;
+ * waits for the scan and writes {x0, y0, width, height} to the host array, pano_crop_rect_dev's rectangle for
+ * every strip partition.  A misuse (bad sizes, more than h lines, rect before the last line) returns
+ * PANO_ERR_INVALID and is sticky, as on a blend stream; pano_crop_scan_free is always valid. */
+typedef struct pano_crop_scan pano_crop_scan;
+int  pano_crop_scan_create(pano_ctx* ctx, int w, int h, pano_crop_scan** out);
+int  pano_crop_scan_add_dev(pano_crop_scan* c, const float* d_strip_hwc, int rows);
+int  pano_crop_scan_rect(pano_crop_scan* c, int rect[4]);
+void pano_crop_scan_free(pano_crop_scan* c);
 /* write_rgb's conversion loop (lib/imgio.cc:98-113) applied to the sub-rectangle
  * d_rect = {x0,y0,cw,ch} (device int[4]; NULL = whole image): every sample is
  * (unsigned char)((v < 0 ? 1 : v) * 255), i.e. Color::NO turns white.  Output
@@ -622,6 +653,12 @@ int pano_mat32f_to_rgb8_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h,
  * (RGBA) or h*w*3; any other format returns PANO_ERR_INVALID. */
 int pano_mat32f_to_pix8_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h, const int* d_rect, int format,
                             unsigned char* d_out);
+/* pano_mat32f_to_pix8_dev's bytes from the mosaic already converted to 8 bits: d_rgb8 is h×w×3 u8 as
+ * pano_mat32f_to_rgb8_dev writes it without a rect (the conversion works sample by sample, so converting
+ * before cropping changes no byte), d_rect the crop rectangle (device int[4]; NULL = whole image) and
+ * format PANO_PIX_RGB, _RGBA or _RGB_PLANAR as above.  d_out must not overlap d_rgb8. */
+int pano_rgb8_crop_to_pix8_dev(pano_ctx* ctx, const unsigned char* d_rgb8, int w, int h, const int* d_rect,
+                               int format, unsigned char* d_out);
 
 /* ------------------------------------------------------- device utilities */
 int pano_dev_alloc(pano_ctx* ctx, size_t bytes, void** d_ptr);

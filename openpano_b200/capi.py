@@ -109,6 +109,10 @@ def _load():
         "pano_blend_stream_finish_dev": (C.c_int, [C.c_void_p, C.c_void_p]),
         "pano_blend_stream_finish": (C.c_int, [C.c_void_p, _fp]),
         "pano_blend_stream_free": (None, [C.c_void_p]),
+        "pano_blend_stream_create_rows": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage),
+                                                    C.POINTER(PanoBlendGeom), C.c_int, P, C.c_int, C.c_int, C.c_int,
+                                                    C.c_int, _vpp]),
+        "pano_blend_stream_needs": (C.c_int, [C.c_void_p, C.c_void_p]),
         "pano_sift_stream_create": (C.c_int, [C.c_void_p, C.c_int, _ip, _ip, P, _vpp]),
         "pano_sift_stream_add": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _vpp, C.c_int, C.c_int]),
         "pano_sift_stream_finish": (C.c_int, [C.c_void_p, _vpp]),
@@ -122,6 +126,12 @@ def _load():
         "pano_rgb8_to_mat32f_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
         "pano_rgb8_to_mat32f_batch_dev": (C.c_int, [C.c_void_p, C.c_int, _vpp, _ip, _ip, _ip, _vpp]),
         "pano_crop_rect_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+        "pano_crop_scan_create": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _vpp]),
+        "pano_crop_scan_add_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
+        "pano_crop_scan_rect": (C.c_int, [C.c_void_p, _ip]),
+        "pano_crop_scan_free": (None, [C.c_void_p]),
+        "pano_rgb8_crop_to_pix8_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                                 C.c_void_p]),
         "pano_mat32f_to_rgb8_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
         "pano_mat32f_to_pix8_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                               C.c_void_p]),
@@ -357,6 +367,7 @@ class _SourceStream:
     _NAME = ""
     _ADD = None
     _FREE = None
+    _NULL_OK = False     # None in a numpy window: an image the stream does not read (row-strip blend streams)
 
     def __init__(self, eng, handle, shapes):
         self.eng, self._h = eng, handle
@@ -380,14 +391,18 @@ class _SourceStream:
             raise self._err
         keep = []
         if kind is None:
-            arrs = list(srcs)
+            all_srcs = list(srcs)
+            arrs = [a for a in all_srcs if a is not None] if self._NULL_OK else all_srcs
             dts = {a.dtype for a in arrs}
-            if len(dts) != 1 or dts.pop() not in (np.uint8, np.float32):
+            if len(dts) > 1 or (not dts and not all_srcs) or (dts and dts.pop() not in (np.uint8, np.float32)):
                 self._fail(f"{self._NAME}: sources must all be uint8 or all float32 numpy arrays")
-            u8 = arrs[0].dtype == np.uint8
+            u8 = bool(arrs) and arrs[0].dtype == np.uint8
             kind = SRC_RGB8_HOST if u8 else SRC_F32_HOST
             channels = None
-            for k, a in enumerate(arrs):
+            for k, a in enumerate(all_srcs):
+                if a is None:
+                    keep.append(None)
+                    continue
                 want = self.shapes[self.added + k] if self.added + k < len(self.shapes) else None
                 if u8 and fmt is not None:
                     try:
@@ -405,7 +420,8 @@ class _SourceStream:
                                f"{want} with {'1 or 3 channels' if u8 else '3 channels'}, the same for the window")
                 channels = ch
                 keep.append(np.ascontiguousarray(a))
-            ptrs = [a.ctypes.data for a in keep]
+            ptrs = [a.ctypes.data if a is not None else 0 for a in keep]
+            channels = 3 if channels is None else channels
         else:
             ptrs = [int(p or 0) for p in srcs]
             channels = 3 if channels is None else channels
@@ -427,17 +443,26 @@ class _SourceStream:
 
 
 class BlendStream(_SourceStream):
-    """A pano_blend_stream: the mosaic of pano_blend, fed window by window (LAZY_READ's memory contract)."""
+    """A pano_blend_stream: the mosaic of pano_blend, fed window by window (LAZY_READ's memory contract).  A stream
+    of rows (row0, row1) gives those rows of it and reads only the images needs() reports."""
     _NAME = "blend stream"
     _ADD = LIB.pano_blend_stream_add
     _FREE = LIB.pano_blend_stream_free
+    _NULL_OK = True      # add() takes None for an image needs() reports False: passed as a null source
 
-    def __init__(self, eng, handle, shapes, out_w, out_h):
+    def __init__(self, eng, handle, shapes, out_w, out_h, rows=None):
         super().__init__(eng, handle, shapes)
         self.out_w, self.out_h = out_w, out_h
+        self.rows = tuple(rows) if rows is not None else (0, out_h)
+
+    def needs(self):
+        """bool per image: whether the stream reads its source (pano_blend_stream_needs)."""
+        flags = np.zeros(max(len(self.shapes), 1), np.uint8)
+        self._call(LIB.pano_blend_stream_needs(self._h, flags.ctypes.data))
+        return flags[:len(self.shapes)].astype(bool)
 
     def finish(self):
-        out = np.empty((self.out_h, self.out_w, 3), np.float32)
+        out = np.empty((self.rows[1] - self.rows[0], self.out_w, 3), np.float32)
         self._call(LIB.pano_blend_stream_finish(self._h, _f(out)))
         return out
 
@@ -456,6 +481,34 @@ class SiftStream(_SourceStream):
         out = C.c_void_p()
         self._call(LIB.pano_sift_stream_finish(self._h, C.byref(out)))
         return FeatureSet(self.eng, out)
+
+
+class CropScan:
+    """A pano_crop_scan: crop()'s rectangle of a mosaic that arrives in row strips (widths up to 80,000)."""
+
+    def __init__(self, eng, handle, w, h):
+        self.eng, self._h, self.w, self.h = eng, handle, w, h
+
+    def add_dev(self, d_strip, rows):
+        """The next `rows` lines of the mosaic: a rows×w×3 f32 device buffer."""
+        self.eng._check(LIB.pano_crop_scan_add_dev(self._h, C.c_void_p(d_strip or 0), rows))
+
+    def rect(self):
+        """{x0, y0, width, height} once every line has been added."""
+        r = np.zeros(4, np.int32)
+        self.eng._check(LIB.pano_crop_scan_rect(self._h, _i(r)))
+        return r
+
+    def close(self):
+        if self._h:
+            LIB.pano_crop_scan_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def _lazy_windows(imgs, window, fmt):
@@ -931,6 +984,17 @@ class Engine:
                                                  oh.value, C.byref(h)))
         return BlendStream(self, h, shapes, ow.value, oh.value)
 
+    def blend_stream_rows(self, shapes, items, geom, row0, row1, bands=0, params=None) -> BlendStream:
+        """blend_stream for rows [row0, row1) of the canvas only: finish() gives those rows of the mosaic."""
+        params = params or default_params()
+        arr, g = self._blend_args([None] * len(items), shapes, items, geom)
+        ow, oh = C.c_int(), C.c_int()
+        self._check(LIB.pano_blend_target_size(len(items), arr, C.byref(ow), C.byref(oh)))
+        h = C.c_void_p()
+        self._check(LIB.pano_blend_stream_create_rows(self._h, len(items), arr, C.byref(g), bands, C.byref(params),
+                                                      ow.value, oh.value, row0, row1, C.byref(h)))
+        return BlendStream(self, h, shapes, ow.value, oh.value, (row0, row1))
+
     def blend_lazy(self, imgs, items, geom, bands=0, params=None, window=1, fmt=None):
         """blend() with the sources added `window` images at a time (an int, or a list of window sizes):
         numpy uint8 (read_img's input: H×W, H×W×1 or H×W×3) or float32 H×W×3 images.  fmt: see pix_format; a
@@ -980,6 +1044,17 @@ class Engine:
         """write_rgb's conversion (imgio.cc:98-113) of the rectangle d_rect (0/None = whole image)."""
         self._check(LIB.pano_mat32f_to_rgb8_dev(self._h, C.c_void_p(d_mat), w, h, C.c_void_p(d_rect or 0),
                                                 C.c_void_p(d_out)))
+
+    def crop_scan(self, w, h) -> CropScan:
+        h_ = C.c_void_p()
+        self._check(LIB.pano_crop_scan_create(self._h, w, h, C.byref(h_)))
+        return CropScan(self, h_, w, h)
+
+    def rgb8_crop_to_pix8_dev(self, d_rgb8, w, h, d_rect, fmt, d_out):
+        """mat32f_to_pix8_dev's bytes from the h×w×3 u8 mosaic mat32f_to_rgb8_dev wrote without a rect."""
+        code = PIX_FORMATS.get(fmt, fmt) if isinstance(fmt, str) else fmt
+        self._check(LIB.pano_rgb8_crop_to_pix8_dev(self._h, C.c_void_p(d_rgb8), w, h, C.c_void_p(d_rect or 0),
+                                                   int(code), C.c_void_p(d_out)))
 
     def mat32f_to_pix8_dev(self, d_mat, w, h, d_rect, fmt, d_out):
         """The same conversion in an encoder's layout: fmt is a PANO_PIX_* code or "rgb" / "rgba" (write_png's

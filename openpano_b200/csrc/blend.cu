@@ -164,14 +164,15 @@ __global__ void k_linear_blend(const BlendImg* __restrict__ imgs, int n, BlendGe
   linear_resolve_px(lazy, s0, s1, s2, wsum, out + ((size_t)(i - row0) * tw + j) * 3);
 }
 
-// One window of a blend stream: adds imgs[0, n) into the persistent sums (sum: tw×th×3, wsum:
-// tw×th, both zero at the start), one thread per pixel of the window's bounding rectangle
-// [rx0, rx1) × [ry0, ry1).  Windows run in image order, so every pixel sees the float additions
-// of k_linear_blend in the same order.
+// One window of a blend stream: adds imgs[0, n) into the persistent sums of the stream's rows
+// (sum: tw×rows×3, wsum: tw×rows, both zero at the start; canvas row row0 is their first row), one
+// thread per pixel of the window's bounding rectangle [rx0, rx1) × [ry0, ry1), which lies in those
+// rows.  Windows run in image order, so every pixel sees the float additions of k_linear_blend in
+// the same order.
 template <class Src>
 __global__ void k_linear_accumulate(const BlendImg* __restrict__ imgs, int n, BlendGeom g, int lazy, int ordered,
-                                    float* __restrict__ sum, float* __restrict__ wsum, int tw, int rx0, int ry0, int rx1,
-                                    int ry1) {
+                                    float* __restrict__ sum, float* __restrict__ wsum, int tw, int row0, int rx0, int ry0,
+                                    int rx1, int ry1) {
   __shared__ TileList tl;
   __shared__ float lut[Src::kLut ? 256 : 1];
   if constexpr (Src::kLut) build_rgb8_lut(lut, threadIdx.y * blockDim.x + threadIdx.x);   // ordered by the list's barrier
@@ -179,7 +180,7 @@ __global__ void k_linear_accumulate(const BlendImg* __restrict__ imgs, int n, Bl
   build_tile_list(imgs, n, tj0, ti0, tj0 + blockDim.x - 1, ti0 + blockDim.y - 1, &tl);
   const int j = tj0 + threadIdx.x, i = ti0 + threadIdx.y;
   if (tl.n == 0 || j >= rx1 || i >= ry1) return;
-  const size_t t = (size_t)i * tw + j;
+  const size_t t = (size_t)(i - row0) * tw + j;
   float* p = sum + t * 3;
   float s0 = p[0], s1 = p[1], s2 = p[2], ws = wsum[t];
   linear_add_px<Src>(imgs, n, tl, g, lazy, ordered, lut, i, j, s0, s1, s2, ws);
@@ -446,6 +447,7 @@ __global__ void k_fill(float* __restrict__ p, size_t n, float v) {
 // Everything a blend derives from its arguments on the host, before any device work.
 struct BlendJob {
   std::vector<BlendImg> imgs;
+  std::vector<int> src;       // the caller's index of each entry of imgs (images that reach no row are left out)
   BlendGeom g;
   int tw = 0, th = 0;
   long long roi_floats = 0;   // floats of one level buffer (4 planes per image)
@@ -535,6 +537,7 @@ static int blend_plan(pano_ctx* ctx, int n, const pano_blend_image* imgs, const 
     job->mask_bytes += d.plane;
     job->max_rw = std::max(job->max_rw, d.rw); job->max_rh = std::max(job->max_rh, d.rh);
     job->imgs.push_back(d);
+    job->src.push_back(k);
   }
   if (job->tw != ow || job->th != oh || ow <= 0 || oh <= 0)
     return ctx_fail(ctx, PANO_ERR_INVALID, "blend: output is %dx%d but target_size is %dx%d", ow, oh, job->tw, job->th);
@@ -716,13 +719,17 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
 // window and are dropped after their window.  State: the canvas (linear: sums + weight plane;
 // multiband: BlendDev's level buffers and masks) plus at most two windows of host sources in the
 // upload ring (common.cuh): window k's upload runs while window k-1's kernels run.
+// A stream of rows [row0, row1) keeps the canvas state of those rows only (blend_plan's strip
+// clipping for multiband) and reads only the sources of the images that reach them.
 struct pano_blend_stream {
   pano_ctx* ctx = nullptr;
   int n = 0, bands = 0, lazy = 0, ordered = 0;
+  int row0 = 0, row1 = 0;
   BlendJob job;
   BlendDev dev;
-  DevBuf<float> d_sum;         // linear: tw×th×3 Σ c·w
-  DevBuf<float> d_wsum;        // linear: tw×th Σ w
+  std::vector<int> slot;       // per image: its entry of job.imgs, or -1 if the rows do not need it
+  DevBuf<float> d_sum;         // linear: tw×rows×3 Σ c·w
+  DevBuf<float> d_wsum;        // linear: tw×rows Σ w
   int added = 0, err = 0;
   bool finished = false;
   UploadRing ring;
@@ -738,14 +745,12 @@ static int stream_fail(pano_blend_stream* s, int rc) { s->err = rc; return rc; }
   } while (0)
 
 // Uploads host window `win` (count images from srcs) into the ring; points win[] at it.
-static int stream_upload(pano_blend_stream* s, int first, int count, const void* const* srcs, bool u8, int channels,
+static int stream_upload(pano_blend_stream* s, int count, const void* const* srcs, bool u8, int channels,
                          BlendImg* win, int* slot_out) {
   std::vector<size_t> bytes(count);
   std::vector<const void*> d_src(count);
-  for (int k = 0; k < count; ++k) {
-    const BlendImg& im = s->job.imgs[first + k];
-    bytes[k] = (size_t)im.w * im.h * (u8 ? (size_t)pix8_bytes(channels) : 3 * sizeof(float));
-  }
+  for (int k = 0; k < count; ++k)
+    bytes[k] = (size_t)win[k].w * win[k].h * (u8 ? (size_t)pix8_bytes(channels) : 3 * sizeof(float));
   if (int rc = s->ring.upload(s->ctx, count, srcs, bytes.data(), d_src.data(), slot_out)) return stream_fail(s, rc);
   for (int k = 0; k < count; ++k) win[k].pix = (const unsigned char*)d_src[k];
   return PANO_OK;
@@ -764,11 +769,11 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
       x0 = std::min(x0, win[k].x0); y0 = std::min(y0, win[k].y0);
       x1 = std::max(x1, win[k].x1 + 1); y1 = std::max(y1, win[k].y1 + 1);
     }
-    x1 = std::min(x1, job.tw); y1 = std::min(y1, job.th);
+    x1 = std::min(x1, job.tw); y0 = std::max(y0, s->row0); y1 = std::min(y1, s->row1);
     if (x0 >= x1 || y0 >= y1) return PANO_OK;
     dim3 g(ceil_div(x1 - x0, 32), ceil_div(y1 - y0, 8));
     PANO_LAUNCH(ctx, pix8 ? "k_linear_accumulate_pix8" : "k_linear_accumulate", k_linear_accumulate<Src>, g, b, 0, d_win,
-                count, job.g, s->lazy, s->ordered, s->d_sum, s->d_wsum, job.tw, x0, y0, x1, y1);
+                count, job.g, s->lazy, s->ordered, s->d_sum, s->d_wsum, job.tw, s->row0, x0, y0, x1, y1);
   } else {
     int rw = 0, rh = 0;
     for (int k = 0; k < count; ++k) { rw = std::max(rw, win[k].rw); rh = std::max(rh, win[k].rh); }
@@ -781,8 +786,12 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
 
 static int stream_resolve(pano_blend_stream* s, float* d_out) {
   pano_ctx* ctx = s->ctx;
-  if (s->bands > 0) return mb_levels(ctx, s->job, &s->dev, s->bands, d_out, 0, s->job.th);
-  const size_t npx = (size_t)s->job.tw * s->job.th;
+  const size_t npx = (size_t)s->job.tw * (s->row1 - s->row0);
+  if (s->bands > 0 && s->job.imgs.empty()) {          // no image reaches the rows
+    PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx * 3 + 255) / 256), 256, 0, d_out, npx * 3, -1.f);
+    return PANO_OK;
+  }
+  if (s->bands > 0) return mb_levels(ctx, s->job, &s->dev, s->bands, d_out, s->row0, s->row1);
   PANO_LAUNCH(ctx, "k_linear_resolve", k_linear_resolve, (unsigned)((npx + 255) / 256), 256, 0, s->d_sum, s->d_wsum,
               d_out, npx, s->lazy);
   return PANO_OK;
@@ -794,6 +803,41 @@ static int stream_finish_check(pano_blend_stream* s, const void* out) {
   if (s->finished) return STREAM_MISUSE(s, "blend stream: already finished");
   if (s->added != s->n) return STREAM_MISUSE(s, "blend stream: finish after %d of %d images", s->added, s->n);
   s->finished = true;
+  return PANO_OK;
+}
+
+static int stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
+                         const pano_params* p, int ow, int oh, int row0, int row1, pano_blend_stream** out) {
+  if (!ctx || !out) return PANO_ERR_INVALID;
+  *out = nullptr;
+  if (n <= 0 || !imgs || !g || !p || bands < 0) return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: bad argument");
+  if (n > PANO_MAX_IMAGES)   // a window's images on gridDim.z of k_mb_first_level
+    return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: %d images (limit %d)", n, PANO_MAX_IMAGES);
+  if (row0 < 0 || row1 > oh || row0 >= row1)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: rows [%d, %d) are no strip of the %d-row canvas", row0, row1, oh);
+  std::unique_ptr<pano_blend_stream> s(new pano_blend_stream);
+  s->ctx = ctx; s->n = n; s->bands = bands; s->lazy = p->lazy_read; s->ordered = p->ordered_input;
+  s->row0 = row0; s->row1 = row1;
+  int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, row0, row1, false, &s->job);
+  if (!rc && !s->job.imgs.empty()) rc = blend_dev_setup(ctx, &s->job, bands, row0, row1, &s->dev);
+  if (rc) return rc;
+  // pano_blend_rows_rgb8_dev's rule: multiband needs the images blend_plan kept (ROI clipped to the rows and
+  // the blur halo); linear those whose ROI meets the rows, every image when the rows are the whole canvas
+  s->slot.assign(n, -1);
+  const bool whole = row0 == 0 && row1 == oh;
+  for (size_t q = 0; q < s->job.imgs.size(); ++q) {
+    const BlendImg& im = s->job.imgs[q];
+    if (bands > 0 || whole || (im.y0 < row1 && im.y1 >= row0)) s->slot[s->job.src[q]] = (int)q;
+  }
+  if (bands == 0) {
+    const size_t npx = (size_t)ow * (row1 - row0);
+    if ((rc = s->d_sum.alloc(ctx, npx * 3)) || (rc = s->d_wsum.alloc(ctx, npx))) return rc;
+    PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx * 3 + 255) / 256), 256, 0, s->d_sum, npx * 3, 0.f);
+    PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx + 255) / 256), 256, 0, s->d_wsum, npx, 0.f);
+  }
+  cudaError_t e = s->ring.init();
+  if (e != cudaSuccess) return ctx_cuda(ctx, e, "blend stream: copy stream / events");
+  *out = s.release();
   return PANO_OK;
 }
 
@@ -840,25 +884,21 @@ int pano_blend_rows_rgb8_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs,
 int pano_blend_stream_create(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
                              const pano_params* p, int ow, int oh, pano_blend_stream** out) {
   ctx_enter(ctx);
-  if (!ctx || !out) return PANO_ERR_INVALID;
-  *out = nullptr;
-  if (n <= 0 || !imgs || !g || !p || bands < 0) return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: bad argument");
-  if (n > PANO_MAX_IMAGES)   // a window's images on gridDim.z of k_mb_first_level
-    return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: %d images (limit %d)", n, PANO_MAX_IMAGES);
-  std::unique_ptr<pano_blend_stream> s(new pano_blend_stream);
-  s->ctx = ctx; s->n = n; s->bands = bands; s->lazy = p->lazy_read; s->ordered = p->ordered_input;
-  int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, 0, oh, false, &s->job);
-  if (!rc) rc = blend_dev_setup(ctx, &s->job, bands, 0, oh, &s->dev);
-  if (rc) return rc;
-  if (bands == 0) {
-    const size_t npx = (size_t)ow * oh;
-    if ((rc = s->d_sum.alloc(ctx, npx * 3)) || (rc = s->d_wsum.alloc(ctx, npx))) return rc;
-    PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx * 3 + 255) / 256), 256, 0, s->d_sum, npx * 3, 0.f);
-    PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx + 255) / 256), 256, 0, s->d_wsum, npx, 0.f);
-  }
-  cudaError_t e = s->ring.init();
-  if (e != cudaSuccess) return ctx_cuda(ctx, e, "blend stream: copy stream / events");
-  *out = s.release();
+  return stream_create(ctx, n, imgs, g, bands, p, ow, oh, 0, oh, out);
+}
+
+int pano_blend_stream_create_rows(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g,
+                                  int bands, const pano_params* p, int ow, int oh, int row0, int row1,
+                                  pano_blend_stream** out) {
+  ctx_enter(ctx);
+  return stream_create(ctx, n, imgs, g, bands, p, ow, oh, row0, row1, out);
+}
+
+int pano_blend_stream_needs(const pano_blend_stream* s, unsigned char* flags) {
+  if (!s) return PANO_ERR_INVALID;
+  ctx_enter(s->ctx);
+  if (!flags) return ctx_fail(s->ctx, PANO_ERR_INVALID, "blend stream: null flags");
+  for (int k = 0; k < s->n; ++k) flags[k] = s->slot[k] >= 0 ? 1 : 0;
   return PANO_OK;
 }
 
@@ -872,27 +912,40 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
     return STREAM_MISUSE(s, "blend stream: images [%d, %d) added, %d of %d so far", first, first + count, s->added, s->n);
   if (!srcs) return STREAM_MISUSE(s, "blend stream: null source list");
   for (int k = 0; k < count; ++k)
-    if (!srcs[k]) return STREAM_MISUSE(s, "blend stream: image %d has no source", first + k);
+    if (!srcs[k] && s->slot[first + k] >= 0) return STREAM_MISUSE(s, "blend stream: image %d has no source", first + k);
   const bool u8 = kind == PANO_SRC_RGB8_DEV || kind == PANO_SRC_RGB8_HOST;
   const bool host = kind == PANO_SRC_F32_HOST || kind == PANO_SRC_RGB8_HOST;
   if (!u8 && kind != PANO_SRC_F32_DEV && kind != PANO_SRC_F32_HOST) return STREAM_MISUSE(s, "blend stream: unknown source kind %d", kind);
   if (u8 ? !pix8_bytes(channels) : channels != 3)
     return STREAM_MISUSE(s, "blend stream: format %#x for source kind %d", channels, kind);
-  if (kind == PANO_SRC_RGB8_DEV && channels == PANO_PIX_RGBA)
-    for (int k = 0; k < count; ++k)
-      if (int rc = pix8_check(ctx, "blend stream", first + k, channels, srcs[k])) return stream_fail(s, rc);
-  std::vector<BlendImg> win(s->job.imgs.begin() + first, s->job.imgs.begin() + first + count);
+  // The window's needed images.  Their table rows go to d_imgs from the first one's entry on: for multiband
+  // they are exactly the consecutive entries mb_levels reads again; linear reads them in this window only.
+  std::vector<BlendImg> win;
+  std::vector<const void*> wsrc;
+  int j0 = -1;
   for (int k = 0; k < count; ++k) {
-    win[k].pix = (const unsigned char*)srcs[k];
-    win[k].channels = u8 ? channels : 3;
+    const int q = s->slot[first + k];
+    if (q < 0) continue;
+    if (kind == PANO_SRC_RGB8_DEV && channels == PANO_PIX_RGBA)
+      if (int rc = pix8_check(ctx, "blend stream", first + k, channels, srcs[k])) return stream_fail(s, rc);
+    if (j0 < 0) j0 = q;
+    win.push_back(s->job.imgs[q]);
+    win.back().pix = (const unsigned char*)srcs[k];
+    win.back().channels = u8 ? channels : 3;
+    wsrc.push_back(srcs[k]);
+  }
+  const int nw = (int)win.size();
+  if (nw == 0) {
+    s->added += count;
+    return PANO_OK;
   }
   int slot = -1, rc = 0;
-  if (host && (rc = stream_upload(s, first, count, srcs, u8, channels, win.data(), &slot))) return rc;
-  BlendImg* d_win = s->dev.d_imgs + first;
-  if ((rc = ctx_put(ctx, d_win, win.data(), count * sizeof(BlendImg)))) return stream_fail(s, rc);
-  rc = !u8 ? stream_launch<SrcF32>(s, d_win, win.data(), count)
-     : pix8_layout(channels) ? stream_launch<SrcPix8>(s, d_win, win.data(), count)
-                             : stream_launch<SrcRgb8>(s, d_win, win.data(), count);
+  if (host && (rc = stream_upload(s, nw, wsrc.data(), u8, channels, win.data(), &slot))) return rc;
+  BlendImg* d_win = s->dev.d_imgs + j0;
+  if ((rc = ctx_put(ctx, d_win, win.data(), nw * sizeof(BlendImg)))) return stream_fail(s, rc);
+  rc = !u8 ? stream_launch<SrcF32>(s, d_win, win.data(), nw)
+     : pix8_layout(channels) ? stream_launch<SrcPix8>(s, d_win, win.data(), nw)
+                             : stream_launch<SrcRgb8>(s, d_win, win.data(), nw);
   if (rc) return stream_fail(s, rc);
   if (slot >= 0) STREAM_CUDA(s, s->ring.release(ctx, slot));
   s->added += count;
@@ -913,7 +966,7 @@ int pano_blend_stream_finish(pano_blend_stream* s, float* out) {
   ctx_enter(ctx);
   int rc = stream_finish_check(s, out);
   if (rc) return stream_fail(s, rc);
-  const size_t nfl = (size_t)s->job.tw * s->job.th * 3;
+  const size_t nfl = (size_t)s->job.tw * (s->row1 - s->row0) * 3;
   DevBuf<float> d_tmp;
   float* d_out = s->d_sum;     // linear: resolved in place
   if (s->bands > 0) {

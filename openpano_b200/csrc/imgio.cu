@@ -86,6 +86,13 @@ __global__ void __launch_bounds__(256) k_pix8_to_f32(const Rgb8Job* __restrict__
 // (2) one CTA per line rebuilds that line's heights from the masks, finds the
 // neighbours through a two-level min hierarchy in shared memory and reduces to the
 // line's best, (3) one CTA reduces the lines.
+//
+// pano_crop_scan runs the same steps on each row strip of a mosaic: the masks are the
+// strip's, the carry starts from the last invalid line of each column in the strips
+// before (kept on the device), and (3) merges the strip's best into the best so far.
+// Up to 40,000 columns its line kernel is (2) as is; wider lines, whose heights do not
+// fit in shared memory, are read from the masks and the carry in global memory, so the
+// width is not bounded by shared memory.
 
 #define CROP_CHUNK 32
 
@@ -112,22 +119,31 @@ struct CropLineBest {
   int area, k, left, right, height;
 };
 
-// carry[c][k] = last invalid line of column k in the chunks before c (-1 if none)
-__global__ void __launch_bounds__(128) k_crop_carry(const unsigned* __restrict__ masks, int w, int chunks,
-                                                    int* __restrict__ carry) {
+// carry[c][k] = last invalid line of column k in the chunks before c (-1 if none).  The masks
+// start at line line0; last_io (null: -1 everywhere) holds each column's last invalid line before
+// them and receives it after them.
+__global__ void __launch_bounds__(128) k_crop_carry(const unsigned* __restrict__ masks, int w, int chunks, int line0,
+                                                    int* __restrict__ last_io, int* __restrict__ carry) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= w) return;
-  int last = -1;
+  int last = last_io ? last_io[k] : -1;
   for (int c = 0; c < chunks; ++c) {
     carry[(size_t)c * w + k] = last;
     unsigned m = masks[(size_t)c * w + k];
-    if (m) last = c * CROP_CHUNK + 31 - __clz(m);
+    if (m) last = line0 + c * CROP_CHUNK + 31 - __clz(m);
   }
+  if (last_io) last_io[k] = last;
 }
 
 #define CROP_RUN_CAP 2048
+// Dynamic shared memory of k_crop_line<true>: the line's heights plus the run arrays (w <= 40,000 fits)
+#define CROP_LINE_SMEM(w) (sizeof(int) * ((size_t)(w) + 4 * CROP_RUN_CAP + 1))
+#define CROP_LINE_SMEM_MAX (200 * 1024)
 
-// One CTA per line.  Columns of equal height that touch share their span, so the line
+// One CTA per line (line line0 + blockIdx.x of the mosaic, masks and carry as k_crop_carry
+// leaves them).  kSmem: the line's heights are first copied to shared memory (w <= 40,000);
+// otherwise every read recomputes a height from the masks and the carry.
+// Columns of equal height that touch share their span, so the line
 // is run-length encoded first (a mosaic line has a handful of runs: flat inside, a
 // staircase at slanted borders) and the nearest-strictly-smaller neighbours are found
 // per RUN by pointer jumping: l[r] starts at r-1 and hops to l[l[r]] while the run it
@@ -135,26 +151,33 @@ __global__ void __launch_bounds__(128) k_crop_carry(const unsigned* __restrict__
 // any interleaving of the in-place updates is valid and the loop ends when a whole
 // round changes nothing.  Lines with more than CROP_RUN_CAP runs take the per-column
 // search through a two-level min hierarchy instead.
+template <bool kSmem>
 __global__ void __launch_bounds__(256) k_crop_line(const unsigned* __restrict__ masks, const int* __restrict__ carry,
-                                                   int w, int h, CropLineBest* __restrict__ best) {
+                                                   int w, int line0, CropLineBest* __restrict__ best) {
   extern __shared__ int crop_smem[];
-  int* hgt = crop_smem;                          // [w]
-  int* r_start = hgt + w;                        // [CAP + 1]   (fallback: l1, l2)
+  int* hgt_s = crop_smem;                        // [w] (kSmem)
+  int* r_start = hgt_s + (kSmem ? w : 0);        // [CAP + 1]   (fallback: l1, l2)
   int* r_h = r_start + CROP_RUN_CAP + 1;         // [CAP]
   int* r_l = r_h + CROP_RUN_CAP;                 // [CAP]
   int* r_r = r_l + CROP_RUN_CAP;                 // [CAP]
   __shared__ int s_warp[8];
   __shared__ unsigned long long s_key[8];
   __shared__ int s_pay[8][3];
-  const int line = blockIdx.x;
-  const int c = line / CROP_CHUNK, bit = line % CROP_CHUNK;
+  const int rel = blockIdx.x, line = line0 + rel;
+  const int c = rel / CROP_CHUNK, bit = rel % CROP_CHUNK;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const unsigned* mrow = masks + (size_t)c * w;
+  const int* crow = carry + (size_t)c * w;
+  const unsigned lowmask = 0xFFFFFFFFu >> (31 - bit);
+  // height of column k at `line`: lines since its last invalid line <= `line`
+  auto hgt = [&](int k) -> int {
+    if (kSmem) return hgt_s[k];
+    const unsigned mm = __ldg(mrow + k) & lowmask;
+    return line - (mm ? line0 + c * CROP_CHUNK + 31 - __clz(mm) : __ldg(crow + k));
+  };
 
-  {
-    // last invalid line <= `line` per column; loads batched 8 deep (the loop is latency-bound otherwise)
-    const unsigned* mrow = masks + (size_t)c * w;
-    const int* crow = carry + (size_t)c * w;
-    const unsigned lowmask = 0xFFFFFFFFu >> (31 - bit);
+  if (kSmem) {
+    // loads batched 8 deep (the loop is latency-bound otherwise)
     for (int k0 = tid; k0 < w; k0 += 8 * 256) {
       unsigned m[8];
       int cr[8];
@@ -169,7 +192,7 @@ __global__ void __launch_bounds__(256) k_crop_line(const unsigned* __restrict__ 
         const int k = k0 + u * 256;
         if (k < w) {
           const unsigned mm = m[u] & lowmask;
-          hgt[k] = line - (mm ? c * CROP_CHUNK + 31 - __clz(mm) : cr[u]);
+          hgt_s[k] = line - (mm ? line0 + c * CROP_CHUNK + 31 - __clz(mm) : cr[u]);
         }
       }
     }
@@ -180,7 +203,7 @@ __global__ void __launch_bounds__(256) k_crop_line(const unsigned* __restrict__ 
   const int seg = ((w + 255) / 256) | 1;
   const int k0 = min(w, tid * seg), k1 = min(w, k0 + seg);
   int cnt = 0;
-  for (int k = k0; k < k1; ++k) cnt += (k == 0 || hgt[k] != hgt[k - 1]);
+  for (int k = k0; k < k1; ++k) cnt += (k == 0 || hgt(k) != hgt(k - 1));
   int incl = cnt;
   for (int o = 1; o < 32; o <<= 1) {
     int v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
@@ -198,8 +221,8 @@ __global__ void __launch_bounds__(256) k_crop_line(const unsigned* __restrict__ 
 
   if (total <= CROP_RUN_CAP) {
     for (int k = k0; k < k1; ++k)
-      if (k == 0 || hgt[k] != hgt[k - 1]) {
-        r_start[off] = k; r_h[off] = hgt[k]; r_l[off] = off - 1; r_r[off] = off + 1;
+      if (k == 0 || hgt(k) != hgt(k - 1)) {
+        r_start[off] = k; r_h[off] = hgt(k); r_l[off] = off - 1; r_r[off] = off + 1;
         ++off;
       }
     if (tid == 0) r_start[total] = w;
@@ -232,7 +255,7 @@ __global__ void __launch_bounds__(256) k_crop_line(const unsigned* __restrict__ 
     for (int g = tid; g < n1; g += blockDim.x) {
       int mn = INT_MAX;
       const int e = min(w, (g + 1) << 5);
-      for (int k = g << 5; k < e; ++k) mn = min(mn, hgt[k]);
+      for (int k = g << 5; k < e; ++k) mn = min(mn, hgt(k));
       l1[g] = mn;
     }
     __syncthreads();
@@ -244,13 +267,13 @@ __global__ void __launch_bounds__(256) k_crop_line(const unsigned* __restrict__ 
     }
     __syncthreads();
     for (int k = tid; k < w; k += blockDim.x) {
-      const int v = hgt[k];
+      const int v = hgt(k);
       if (v == 0) continue;
       int j = k - 1;
       while (j >= 0) {
         if ((j & 1023) == 1023 && l2[j >> 10] >= v) { j -= 1024; continue; }
         if ((j & 31) == 31 && l1[j >> 5] >= v) { j -= 32; continue; }
-        if (hgt[j] < v) break;
+        if (hgt(j) < v) break;
         --j;
       }
       const int left = j + 1;
@@ -258,7 +281,7 @@ __global__ void __launch_bounds__(256) k_crop_line(const unsigned* __restrict__ 
       while (j < w) {
         if ((j & 1023) == 0 && j + 1024 <= w && l2[j >> 10] >= v) { j += 1024; continue; }
         if ((j & 31) == 0 && j + 32 <= w && l1[j >> 5] >= v) { j += 32; continue; }
-        if (hgt[j] < v) break;
+        if (hgt(j) < v) break;
         ++j;
       }
       const int right = j - 1;
@@ -284,11 +307,18 @@ __global__ void __launch_bounds__(256) k_crop_line(const unsigned* __restrict__ 
     r.area = (int)(s_key[bw] >> 32);
     r.k = (int)(0xFFFFFFFFu - (unsigned)(s_key[bw] & 0xFFFFFFFFu));
     r.left = s_pay[bw][0]; r.right = s_pay[bw][1]; r.height = s_pay[bw][2];
-    best[line] = r;
+    best[rel] = r;
   }
 }
 
-__global__ void __launch_bounds__(256) k_crop_final(const CropLineBest* __restrict__ best, int h, int* __restrict__ rect) {
+// The best rectangle so far of a pano_crop_scan: area, last line, left and right column, height.
+struct CropBest { int area, line, left, right, height; };
+
+// Reduces the lines' bests (lines line0 + [0, h)) to crop()'s rectangle.  run (null: a whole
+// mosaic) is the best of the lines above: this block's best replaces it only with a larger area,
+// and the rectangle is the result.
+__global__ void __launch_bounds__(256) k_crop_final(const CropLineBest* __restrict__ best, int h, int line0,
+                                                    CropBest* __restrict__ run, int* __restrict__ rect) {
   unsigned long long key = 0;
   for (int line = threadIdx.x; line < h; line += blockDim.x) {
     int a = best[line].area;
@@ -308,8 +338,13 @@ __global__ void __launch_bounds__(256) k_crop_final(const CropLineBest* __restri
     for (int i = 1; i < 8; ++i) if (s_key[i] > key) key = s_key[i];
     int ll = 0, rr = 0, hh = 0, nl = 0;            // crop()'s initial values (imgproc.cc:205)
     if (key) {
-      nl = (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFu));
-      ll = best[nl].left; rr = best[nl].right; hh = best[nl].height;
+      const int q = (int)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFu));
+      nl = line0 + q;
+      ll = best[q].left; rr = best[q].right; hh = best[q].height;
+    }
+    if (run) {
+      if ((int)(key >> 32) > run->area) *run = CropBest{(int)(key >> 32), nl, ll, rr, hh};
+      else { nl = run->line; ll = run->left; rr = run->right; hh = run->height; }
     }
     rect[0] = ll;                 // offsetx
     rect[1] = nl - hh + 1;        // offsety
@@ -368,6 +403,68 @@ __global__ void __launch_bounds__(256) k_f32_to_pix8(const float* __restrict__ m
   }
 }
 
+// The crop rectangle of a mosaic converted by k_f32_to_rgb8 without a rect, in k_f32_to_pix8's layouts:
+// the same bytes as converting the cropped f32 mosaic, since the conversion works sample by sample.
+template <int FMT>
+__global__ void __launch_bounds__(256) k_rgb8_crop(const unsigned char* __restrict__ rgb, int w, int h,
+                                                   const int* __restrict__ rect, unsigned char* __restrict__ out) {
+  int x0 = 0, y0 = 0, cw = w, ch = h;
+  if (rect) { x0 = rect[0]; y0 = rect[1]; cw = rect[2]; ch = rect[3]; }
+  const long long n = (long long)cw * ch;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int r = (int)(i / cw), c = (int)(i - (long long)r * cw);
+    const unsigned char* p = rgb + ((size_t)(r + y0) * w + (c + x0)) * 3;
+    const unsigned char o0 = p[0], o1 = p[1], o2 = p[2];
+    if (FMT == PANO_PIX_RGBA) {
+      unsigned char* d = out + i * 4;
+      d[0] = o0; d[1] = o1; d[2] = o2; d[3] = 255;
+    } else if (FMT == PANO_PIX_RGB_PLANAR) {
+      out[i] = o0; out[n + i] = o1; out[2 * n + i] = o2;
+    } else {
+      unsigned char* d = out + i * 3;
+      d[0] = o0; d[1] = o1; d[2] = o2;
+    }
+  }
+}
+
+// ------------------------------------------------------------------ crop scan state
+#define CROP_SCAN_MAX_W 80000   // the reference's limit on a mosaic's edge (stitcher_image.cc:105)
+
+struct pano_crop_scan {
+  pano_ctx* ctx = nullptr;
+  int w = 0, h = 0, lines = 0, err = 0;
+  DevBuf<int> d_last;        // [w] last invalid line of each column so far, -1 if none
+  DevBuf<CropBest> d_run;    // the best rectangle so far
+  DevBuf<int> d_rect;        // crop()'s rectangle of the lines so far
+};
+
+static int scan_fail(pano_crop_scan* c, int rc) { c->err = rc; return rc; }
+
+// Steps (1) to (3) on the next `rows` lines of the mosaic.
+static int crop_scan_strip(pano_crop_scan* c, const float* d_strip, int rows) {
+  pano_ctx* ctx = c->ctx;
+  const int w = c->w, chunks = ceil_div(rows, CROP_CHUNK), line0 = c->lines;
+  DevBuf<unsigned> d_masks;
+  DevBuf<int> d_carry;
+  DevBuf<CropLineBest> d_best;
+  int rc = 0;
+  if ((rc = d_masks.alloc(ctx, (size_t)chunks * w)) || (rc = d_carry.alloc(ctx, (size_t)chunks * w)) ||
+      (rc = d_best.alloc(ctx, (size_t)rows)))
+    return rc;
+  // the line kernel of pano_crop_rect_dev where the line's heights fit in shared memory, else the one that reads
+  // them from the masks and the carry (l1 / l2 of CROP_SCAN_MAX_W columns fit in the run arrays)
+  const bool smem_line = CROP_LINE_SMEM(w) <= CROP_LINE_SMEM_MAX;
+  const size_t smem = smem_line ? CROP_LINE_SMEM(w) : sizeof(int) * (4 * CROP_RUN_CAP + 1);
+  if (smem_line && smem > 48 * 1024)
+    PANO_CUDA(ctx, cudaFuncSetAttribute(k_crop_line<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  PANO_LAUNCH(ctx, "k_crop_masks", k_crop_masks, dim3(ceil_div(w, 128), chunks), 128, 0, d_strip, w, rows, d_masks);
+  PANO_LAUNCH(ctx, "k_crop_carry", k_crop_carry, ceil_div(w, 128), 128, 0, d_masks, w, chunks, line0, c->d_last, d_carry);
+  if (smem_line) PANO_LAUNCH(ctx, "k_crop_line", k_crop_line<true>, rows, 256, smem, d_masks, d_carry, w, line0, d_best);
+  else PANO_LAUNCH(ctx, "k_crop_scan_line", k_crop_line<false>, rows, 256, smem, d_masks, d_carry, w, line0, d_best);
+  PANO_LAUNCH(ctx, "k_crop_final", k_crop_final, 1, 256, 0, d_best, rows, line0, c->d_run, c->d_rect);
+  return PANO_OK;
+}
+
 // ------------------------------------------------------------------ C API
 extern "C" {
 
@@ -414,8 +511,8 @@ int pano_crop_rect_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h, int*
   if (!ctx || !d_mat_hwc || !d_rect || w <= 0 || h <= 0)
     return ctx_fail(ctx, PANO_ERR_INVALID, "pano_crop_rect_dev: bad argument");
   const int chunks = ceil_div(h, CROP_CHUNK);
-  const size_t smem = sizeof(int) * ((size_t)w + 4 * CROP_RUN_CAP + 1);   // l1/l2 of the fallback fit in the run arrays
-  if (smem > 200 * 1024) return ctx_fail(ctx, PANO_ERR_INVALID, "pano_crop_rect_dev: width %d exceeds the %d-column limit", w, 40000);
+  const size_t smem = CROP_LINE_SMEM(w);   // l1/l2 of the fallback fit in the run arrays
+  if (smem > CROP_LINE_SMEM_MAX) return ctx_fail(ctx, PANO_ERR_INVALID, "pano_crop_rect_dev: width %d exceeds the %d-column limit", w, 40000);
   DevBuf<unsigned> d_masks;
   DevBuf<int> d_carry;
   DevBuf<CropLineBest> d_best;
@@ -423,11 +520,77 @@ int pano_crop_rect_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h, int*
   if (int rc = d_carry.alloc(ctx, (size_t)chunks * w)) return rc;
   if (int rc = d_best.alloc(ctx, (size_t)h)) return rc;
   if (smem > 48 * 1024)
-    PANO_CUDA(ctx, cudaFuncSetAttribute(k_crop_line, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PANO_CUDA(ctx, cudaFuncSetAttribute(k_crop_line<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   PANO_LAUNCH(ctx, "k_crop_masks", k_crop_masks, dim3(ceil_div(w, 128), chunks), 128, 0, d_mat_hwc, w, h, d_masks);
-  PANO_LAUNCH(ctx, "k_crop_carry", k_crop_carry, ceil_div(w, 128), 128, 0, d_masks, w, chunks, d_carry);
-  PANO_LAUNCH(ctx, "k_crop_line", k_crop_line, h, 256, smem, d_masks, d_carry, w, h, d_best);
-  PANO_LAUNCH(ctx, "k_crop_final", k_crop_final, 1, 256, 0, d_best, h, d_rect);
+  PANO_LAUNCH(ctx, "k_crop_carry", k_crop_carry, ceil_div(w, 128), 128, 0, d_masks, w, chunks, 0, nullptr, d_carry);
+  PANO_LAUNCH(ctx, "k_crop_line", k_crop_line<true>, h, 256, smem, d_masks, d_carry, w, 0, d_best);
+  PANO_LAUNCH(ctx, "k_crop_final", k_crop_final, 1, 256, 0, d_best, h, 0, nullptr, d_rect);
+  return PANO_OK;
+}
+
+int pano_crop_scan_create(pano_ctx* ctx, int w, int h, pano_crop_scan** out) {
+  ctx_enter(ctx);
+  if (!ctx || !out) return PANO_ERR_INVALID;
+  *out = nullptr;
+  if (w <= 0 || h <= 0 || w > CROP_SCAN_MAX_W)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "crop scan: %dx%d (widths 1 to %d)", w, h, CROP_SCAN_MAX_W);
+  std::unique_ptr<pano_crop_scan> c(new pano_crop_scan);
+  c->ctx = ctx; c->w = w; c->h = h;
+  int rc = 0;
+  if ((rc = c->d_last.alloc(ctx, w)) || (rc = c->d_run.alloc(ctx, 1)) || (rc = c->d_rect.alloc(ctx, 4))) return rc;
+  PANO_CUDA(ctx, cudaMemsetAsync(c->d_last, 0xff, sizeof(int) * w, ctx->stream));   // -1
+  PANO_CUDA(ctx, cudaMemsetAsync(c->d_run, 0, sizeof(CropBest), ctx->stream));      // crop()'s initial values
+  *out = c.release();
+  return PANO_OK;
+}
+
+int pano_crop_scan_add_dev(pano_crop_scan* c, const float* d_strip_hwc, int rows) {
+  if (!c) return PANO_ERR_INVALID;
+  pano_ctx* ctx = c->ctx;
+  ctx_enter(ctx);
+  if (c->err) return c->err;
+  if (!d_strip_hwc || rows <= 0 || rows > c->h - c->lines)
+    return scan_fail(c, ctx_fail(ctx, PANO_ERR_INVALID, "crop scan: %d lines at line %d of %d", rows, c->lines, c->h));
+  if (int rc = crop_scan_strip(c, d_strip_hwc, rows)) return scan_fail(c, rc);
+  c->lines += rows;
+  return PANO_OK;
+}
+
+int pano_crop_scan_rect(pano_crop_scan* c, int rect[4]) {
+  if (!c) return PANO_ERR_INVALID;
+  pano_ctx* ctx = c->ctx;
+  ctx_enter(ctx);
+  if (c->err) return c->err;
+  if (!rect) return scan_fail(c, ctx_fail(ctx, PANO_ERR_INVALID, "crop scan: null rect"));
+  if (c->lines != c->h)
+    return scan_fail(c, ctx_fail(ctx, PANO_ERR_INVALID, "crop scan: rect after %d of %d lines", c->lines, c->h));
+  cudaError_t e = cudaMemcpyAsync(rect, c->d_rect, 4 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e != cudaSuccess) return scan_fail(c, ctx_cuda(ctx, e, "crop scan: rect"));
+  return PANO_OK;
+}
+
+void pano_crop_scan_free(pano_crop_scan* c) {
+  if (c) ctx_enter(c->ctx);
+  delete c;
+}
+
+int pano_rgb8_crop_to_pix8_dev(pano_ctx* ctx, const unsigned char* d_rgb8, int w, int h, const int* d_rect, int format,
+                               unsigned char* d_out) {
+  ctx_enter(ctx);
+  if (!ctx || !d_rgb8 || !d_out || w <= 0 || h <= 0)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "pano_rgb8_crop_to_pix8_dev: bad argument");
+  long long blocks = ((long long)w * h + 255) / 256;
+  int grid = (int)std::min<long long>(blocks, (long long)ctx->num_sms * 16);
+  if (format == PANO_PIX_RGB)
+    PANO_LAUNCH(ctx, "k_rgb8_crop", k_rgb8_crop<PANO_PIX_RGB>, grid, 256, 0, d_rgb8, w, h, d_rect, d_out);
+  else if (format == PANO_PIX_RGBA)
+    PANO_LAUNCH(ctx, "k_rgb8_crop_rgba", k_rgb8_crop<PANO_PIX_RGBA>, grid, 256, 0, d_rgb8, w, h, d_rect, d_out);
+  else if (format == PANO_PIX_RGB_PLANAR)
+    PANO_LAUNCH(ctx, "k_rgb8_crop_planar", k_rgb8_crop<PANO_PIX_RGB_PLANAR>, grid, 256, 0, d_rgb8, w, h, d_rect, d_out);
+  else
+    return ctx_fail(ctx, PANO_ERR_INVALID, "pano_rgb8_crop_to_pix8_dev: format %#x (PANO_PIX_RGB, _RGBA or _RGB_PLANAR)",
+                    format);
   return PANO_OK;
 }
 

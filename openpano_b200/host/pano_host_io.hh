@@ -5,10 +5,14 @@
 //   B200PixelBlender  B200LazyBlender's blend (LinearBlender / MultiBandBlender, bit for bit) from such buffers
 //   write_mosaic      crop + write_rgb of main.cc:226-234 from a device mosaic: the 8-bit conversion on the
 //                     device, lodepng::encode for a .png, CImg::save otherwise
+//   B200PixelBlender::write_strips
+//                     blend + crop + write_rgb of main.cc:226-234 one strip of canvas rows at a time: no f32
+//                     mosaic of the whole canvas, on the host or the device
 // The buffers go to B200SIFTDetector::detect_batch_rgb8, B200PixelBlender or the streams (pano_b200.h) with
 // their format as the `channels` argument; no Mat32f of a source is built.  Include after the reference's
 // headers are on the include path (-I <reference>/src -isystem <reference>/src/third-party), as pano_host.hh.
 #pragma once
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -66,6 +70,19 @@ inline Pixels load_pixels(const char* fname) {
   return px;
 }
 
+// write_rgb's encoder step (imgio.cc:98-113): buf is the cw×ch mosaic in the layout write_mosaic converts to,
+// RGBA (alpha 255) for a .png, CImg's planes otherwise.
+inline void encode_mosaic(const char* fname, const std::vector<unsigned char>& buf, int cw, int ch) {
+  if (endswith(fname, ".png")) {
+    const unsigned error = lodepng::encode(fname, buf, (unsigned)cw, (unsigned)ch);
+    if (error) error_exit(ssprintf("png encoder error %u: %s", error, lodepng_error_text(error)));
+  } else {
+    cimg_library::CImg<unsigned char> img(cw, ch, 1, 3);
+    memcpy(img.data(), buf.data(), buf.size());
+    img.save(fname);
+  }
+}
+
 // Blends decoded buffers through a pano_blend_stream: the mosaic of LinearBlender / MultiBandBlender (and of
 // B200Blender) on read_img's images of the same files, bit for bit.  Consecutive images of one format go in
 // windows of up to `window`; the caller keeps the buffers until run() returns.
@@ -104,6 +121,68 @@ class B200PixelBlender {
     pano_blend_stream_free(s);
     return out;
   }
+
+  // main.cc:226-234 on run()'s mosaic — crop() when `crop`, then write_rgb(fname) — without that mosaic: the canvas
+  // is blended `rows` rows at a time by row-strip streams (pano_blend_stream_create_rows), each fed only the
+  // images that reach its rows (an image that reaches k strips is uploaded k times).  The crop scan carries crop()
+  // across the strips, and each strip is converted into an 8-bit canvas that is cropped at the end.  Device memory:
+  // one strip's blend state and 12 B per strip pixel, two windows of sources, 3 B per canvas pixel and the
+  // encoder's layout of it (4 B per pixel for a .png).  The file is write_rgb's, byte for byte, for canvases up to
+  // 80,000 columns wide when `crop`.
+  void write_strips(int rows, bool crop, const char* fname) {
+    const int n = (int)imgs_.size();
+    int ow = 0, oh = 0;
+    c_.check(pano_blend_target_size(n, imgs_.data(), &ow, &oh));
+    if (rows < 1) rows = 1;
+    const bool png = endswith(fname, ".png");
+    pano_params p = snapshot_params();
+    void *d_strip = nullptr, *d_rgb8 = nullptr, *d_out = nullptr, *d_rect = nullptr;
+    int rect[4] = {0, 0, ow, oh};
+    c_.check(pano_dev_alloc(c_.get(), (size_t)std::min(rows, oh) * ow * 3 * sizeof(float), &d_strip));
+    c_.check(pano_dev_alloc(c_.get(), (size_t)ow * oh * 3, &d_rgb8));
+    c_.check(pano_dev_alloc(c_.get(), (size_t)ow * oh * (png ? 4 : 3), &d_out));
+    c_.check(pano_dev_alloc(c_.get(), sizeof(rect), &d_rect));
+    pano_crop_scan* scan = nullptr;
+    if (crop) c_.check(pano_crop_scan_create(c_.get(), ow, oh, &scan));
+    std::vector<unsigned char> need(n);
+    for (int r0 = 0; r0 < oh; r0 += rows) {
+      const int r1 = std::min(oh, r0 + rows);
+      pano_blend_stream* s = nullptr;
+      c_.check(pano_blend_stream_create_rows(c_.get(), n, imgs_.data(), &g_, bands_, &p, ow, oh, r0, r1, &s));
+      c_.check(pano_blend_stream_needs(s, need.data()));
+      // windows of up to window_ needed images of one format; the others are passed as null
+      for (int k0 = 0; k0 < n;) {
+        int fmt = -1, used = 0, k1 = k0;
+        std::vector<const void*> src;
+        for (; k1 < n; ++k1) {
+          if (need[k1]) {
+            if (used == window_ || (fmt >= 0 && px_[k1]->format != fmt)) break;
+            fmt = px_[k1]->format;
+            ++used;
+          }
+          src.push_back(need[k1] ? px_[k1]->ptr() : nullptr);
+        }
+        c_.check(pano_blend_stream_add(s, k0, k1 - k0, src.data(), PANO_SRC_RGB8_HOST, fmt < 0 ? PANO_PIX_RGB : fmt));
+        k0 = k1;
+      }
+      c_.check(pano_blend_stream_finish_dev(s, (float*)d_strip));
+      pano_blend_stream_free(s);
+      if (crop) c_.check(pano_crop_scan_add_dev(scan, (const float*)d_strip, r1 - r0));
+      c_.check(pano_mat32f_to_rgb8_dev(c_.get(), (const float*)d_strip, ow, r1 - r0, nullptr,
+                                       (unsigned char*)d_rgb8 + (size_t)r0 * ow * 3));
+    }
+    if (crop) {
+      c_.check(pano_crop_scan_rect(scan, rect));
+      pano_crop_scan_free(scan);
+    }
+    c_.check(pano_dev_upload(c_.get(), d_rect, rect, sizeof(rect)));
+    c_.check(pano_rgb8_crop_to_pix8_dev(c_.get(), (const unsigned char*)d_rgb8, ow, oh, (const int*)d_rect,
+                                        png ? PANO_PIX_RGBA : PANO_PIX_RGB_PLANAR, (unsigned char*)d_out));
+    std::vector<unsigned char> buf((size_t)rect[2] * rect[3] * (png ? 4 : 3));
+    if (!buf.empty()) c_.check(pano_dev_download(c_.get(), buf.data(), d_out, buf.size()));
+    for (void* d : {d_strip, d_rgb8, d_out, d_rect}) c_.check(pano_dev_free(c_.get(), d));
+    encode_mosaic(fname, buf, rect[2], rect[3]);
+  }
  private:
   const Context& c_;
   int bands_, window_;
@@ -132,14 +211,7 @@ inline void write_mosaic(const Context& c, const float* d_mosaic, int w, int h, 
   c.check(pano_dev_download(c.get(), buf.data(), d_out, buf.size()));
   c.check(pano_dev_free(c.get(), d_out));
   if (d_rect) c.check(pano_dev_free(c.get(), d_rect));
-  if (png) {
-    const unsigned error = lodepng::encode(fname, buf, (unsigned)cw, (unsigned)ch);
-    if (error) error_exit(ssprintf("png encoder error %u: %s", error, lodepng_error_text(error)));
-  } else {
-    cimg_library::CImg<unsigned char> img(cw, ch, 1, 3);
-    memcpy(img.data(), buf.data(), buf.size());
-    img.save(fname);
-  }
+  encode_mosaic(fname, buf, cw, ch);
 }
 
 }  // namespace pano_b200

@@ -17,7 +17,7 @@ from __future__ import annotations
 import numpy as np
 
 from ._abi import default_params
-from .capi import PIX_FORMATS, PIX_RGB, PIX_RGBA, PIX_RGB_PLANAR, Engine
+from .capi import PIX_FORMATS, PIX_RGB, PIX_RGBA, PIX_RGB_PLANAR, Engine, pix_format
 
 
 from .synth import all_pairs, ordered_pairs  # noqa: F401  (task lists live with the workload generator)
@@ -329,6 +329,65 @@ def unpack_rgb8_mosaic(buf: np.ndarray, out_wh, cropped: bool = True, out_format
         return (x0, y0, w, h), buf[hdr:hdr + w * h * 3].reshape(3, h, w)
     bpp = 4 if code == PIX_RGBA else 3
     return (x0, y0, w, h), buf[hdr:hdr + w * h * bpp].reshape(h, w, bpp)
+
+
+def mosaic_rgb8_strips(engine: Engine, items, geom, bands, sources, strip_rows, window=1, out_format="rgb",
+                       crop=True, params=None, kind=None, channels=3, shapes=None, fmt=None):
+    """ConnectedImages::blend() + crop() + write_rgb's conversion strip by strip, without the f32 mosaic.
+
+    Each strip of `strip_rows` canvas rows is a row-strip blend stream fed only the sources it needs, `window` of
+    them per add (None: all in one add).  Its f32 rows go through the crop scan and into an uncropped 8-bit canvas,
+    which is cropped at the end.  sources: numpy arrays (host uint8 read in layout `fmt`, or float32 H×W×3), or
+    pointers of source kind `kind` with PANO_PIX_* code `channels` and `shapes` [(h, w)].  Device memory holds
+    one strip's blend state and f32 rows, two windows of sources, and 3 + 3 (4 for "rgba") bytes per canvas pixel.
+    Returns (rect or None, pixels) as Engine.crop_write_pix8 does: the same bytes as crop_write_pix8 on the
+    mosaic of Engine.blend."""
+    n = len(items)
+    if shapes is None:
+        shapes = [pix_format(a, fmt)[1:] if a.dtype == np.uint8 and fmt is not None else a.shape[:2] for a in sources]
+    ow, oh = max(it[2] for it in items), max(it[3] for it in items)
+    code = PIX_FORMATS[out_format]
+    bpp = 4 if code == PIX_RGBA else 3
+    window = window or n
+    d_strip = engine.dev_alloc(min(strip_rows, oh) * ow * 12)
+    d_rgb = engine.dev_alloc(ow * oh * 3)
+    d_out = engine.dev_alloc(ow * oh * bpp)
+    d_rect = engine.dev_alloc(256)
+    scan = engine.crop_scan(ow, oh) if crop else None
+    try:
+        for r0 in range(0, oh, strip_rows):
+            r1 = min(oh, r0 + strip_rows)
+            s = engine.blend_stream_rows(shapes, items, geom, r0, r1, bands, params)
+            try:
+                need = s.needs()
+                batch, used = [], 0
+                for k in range(n):          # adds of `window` needed images each, unneeded ones passed as None
+                    batch.append(sources[k] if need[k] else None)
+                    used += int(need[k])
+                    if used == window or k == n - 1:
+                        s.add(batch, kind, channels, fmt)
+                        batch, used = [], 0
+                s.finish_dev(d_strip)
+            finally:
+                s.close()
+            if scan is not None:
+                scan.add_dev(d_strip, r1 - r0)
+            engine.mat32f_to_rgb8_dev(d_strip, ow, r1 - r0, 0, d_rgb + r0 * ow * 3)
+        rect = None
+        if scan is not None:
+            rect = scan.rect()
+            engine.dev_upload(d_rect, rect)
+        engine.rgb8_crop_to_pix8_dev(d_rgb, ow, oh, d_rect if crop else 0, code, d_out)
+        cw, ch = (int(rect[2]), int(rect[3])) if crop else (ow, oh)
+        px = np.empty(cw * ch * bpp, np.uint8)
+        if px.size:
+            engine.dev_download(px, d_out)
+    finally:
+        if scan is not None:
+            scan.close()
+        for d in (d_strip, d_rgb, d_out, d_rect):
+            engine.dev_free(d)
+    return rect, (px.reshape(3, ch, cw) if code == PIX_RGB_PLANAR else px.reshape(ch, cw, bpp))
 
 
 class StitchLanes:
