@@ -49,7 +49,8 @@ typedef enum pano_status {
 
 /* Pixel formats of decoded 8-bit images: the per-image `channels` argument of every 8-bit entry point
  * (pano_sift_detect_batch_rgb8[_dev], pano_sift_stream_add and pano_blend_stream_add with the 8-bit kinds,
- * pano_blend_rgb8_dev, pano_blend_rows_rgb8_dev, pano_cyl_warp_batch_rgb8_dev, pano_rgb8_to_mat32f[_batch]_dev)
+ * pano_blend_rgb8_dev, pano_blend_rows_rgb8_dev, pano_cyl_warp_batch_rgb8_dev, pano_planet_pix8[_dev],
+ * pano_rgb8_to_mat32f[_batch]_dev)
  * takes one of these.  Batches may mix formats per image; a stream add takes one format for its window.
  * Each reads the f32 image read_img (lib/imgio.cc:67-90) would build from the decoder's buffer, bit for bit:
  *   GREY        h×w u8: CImg's spectrum-1 rule, the value replicated to r, g, b and NOT divided by 255.
@@ -581,6 +582,16 @@ int pano_planet(pano_ctx* ctx, const float* rgb_hwc, int w, int h, float* out_hw
 /* Device in/out (e.g. the mosaic pano_blend_dev leaves on the device), asynchronous on the ctx
  * stream; d_out_hwc holds 1000×1000×3 f32. */
 int pano_planet_dev(pano_ctx* ctx, const float* d_rgb_hwc, int w, int h, float* d_out_hwc);
+/* The planet straight from a decoded 8-bit image (the `planet` command's read_img input): pix is w×h pixels in
+ * `format`, any PANO_PIX_* value (1, 3 or 4 bytes per pixel; planar is three w×h planes).  The output bits equal
+ * pano_planet's on read_img's f32 image of the same pixels (pano_rgb8_to_mat32f_dev's image), h == 1 and
+ * w == 1 included; no f32 copy of the input is made.  write_rgb's bytes of the result come from
+ * pano_mat32f_to_pix8_dev.  Null pointers, w < 1 or h < 1, a value that is no PANO_PIX_* format and a device
+ * RGBA source that is not 4-byte aligned return PANO_ERR_INVALID and launch nothing.
+ * Host in/out (pix pageable or pinned, uploaded as it is), returns when done: */
+int pano_planet_pix8(pano_ctx* ctx, const unsigned char* pix, int format, int w, int h, float* out_hwc);
+/* Device in/out, asynchronous on the ctx stream; d_out_hwc holds 1000×1000×3 f32: */
+int pano_planet_pix8_dev(pano_ctx* ctx, const unsigned char* d_pix, int format, int w, int h, float* d_out_hwc);
 
 /* --------------------------------------------------------- multi-GPU
  * One process (or host thread) per GPU, one pano_ctx each (SURVEY.md §8e).  The path shards on

@@ -120,6 +120,8 @@ def _load():
         "pano_mem_high_water": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t), C.c_int]),
         "pano_planet": (C.c_int, [C.c_void_p, _fp, C.c_int, C.c_int, _fp]),
         "pano_planet_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+        "pano_planet_pix8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, _fp]),
+        "pano_planet_pix8_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
         "pano_featureset_import_dev": (C.c_int, [C.c_void_p, C.c_int, _ip, _vpp, _vpp, _vpp]),
         "pano_featureset_export_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
         "pano_featureset_export_all_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -1023,6 +1025,22 @@ class Engine:
     def planet_dev(self, d_src, w, h, d_out):
         """Device pointers in and out (d_out: 1000×1000×3 f32), asynchronous on the context's stream."""
         self._check(LIB.pano_planet_dev(self._h, C.c_void_p(d_src or 0), w, h, C.c_void_p(d_out or 0)))
+
+    def planet_pix8(self, pix, fmt=None):
+        """planet() of a decoded 8-bit image (uint8 H×W, H×W×1 or H×W×3; lodepng's H×W×4 with fmt="rgba", CImg's
+        3×H×W with fmt="planar"; see pix_format), uploaded as it is -> (1000, 1000, 3) float32: the bits of
+        planet(read_img_rgb8(pix, fmt)) without that f32 image."""
+        pix = np.ascontiguousarray(pix, np.uint8)
+        code, h, w = pix_format(pix, fmt)
+        out = np.empty((self.PLANET_SIZE, self.PLANET_SIZE, 3), np.float32)
+        self._check(LIB.pano_planet_pix8(self._h, C.c_void_p(pix.ctypes.data), code, w, h, _f(out)))
+        return out
+
+    def planet_pix8_dev(self, d_pix, fmt, w, h, d_out):
+        """Device pointers in and out (d_out: 1000×1000×3 f32), asynchronous on the context's stream; fmt is a
+        PANO_PIX_* code or "grey" / "rgb" / "rgba" / "planar"."""
+        code = PIX_FORMATS.get(fmt, fmt) if isinstance(fmt, str) else fmt
+        self._check(LIB.pano_planet_pix8_dev(self._h, C.c_void_p(d_pix or 0), int(code), w, h, C.c_void_p(d_out or 0)))
 
     # ---- 8-bit boundary: read_img / crop / write_rgb formats (device pointers)
     def rgb8_to_mat32f_batch_dev(self, d_pix, ws, hs, channels, d_out):

@@ -8,12 +8,14 @@
 //   B200PixelBlender::write_strips
 //                     blend + crop + write_rgb of main.cc:226-234 one strip of canvas rows at a time: no f32
 //                     mosaic of the whole canvas, on the host or the device
+//   b200_planet       planet() of main.cc:294-331 from load_pixels' buffer, left on the device for write_mosaic
 // The buffers go to B200SIFTDetector::detect_batch_rgb8, B200PixelBlender or the streams (pano_b200.h) with
 // their format as the `channels` argument; no Mat32f of a source is built.  Include after the reference's
 // headers are on the include path (-I <reference>/src -isystem <reference>/src/third-party), as pano_host.hh.
 #pragma once
 #include <algorithm>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -212,6 +214,28 @@ inline void write_mosaic(const Context& c, const float* d_mosaic, int w, int h, 
   c.check(pano_dev_free(c.get(), d_out));
   if (d_rect) c.check(pano_dev_free(c.get(), d_rect));
   encode_mosaic(fname, buf, cw, ch);
+}
+
+// A device block from pano_dev_alloc, given back to its context with the owner.
+struct DevFree {
+  const Context* c;
+  void operator()(float* d) const { pano_dev_free(c->get(), d); }
+};
+using DevImage = std::unique_ptr<float, DevFree>;
+
+// planet()'s image (main.cc:294-331) of a decoded file, left on the device (1000×1000×3 f32): the planet of
+// read_img's image of the same file, bit for bit, without that image.  The `planet` command becomes
+//   write_mosaic(ctx, b200_planet(ctx, load_pixels(fname)).get(), 1000, 1000, false, IMGFILE(planet));
+inline DevImage b200_planet(const Context& c, const Pixels& px) {
+  void* d_pix = nullptr;
+  void* d_out = nullptr;
+  c.check(pano_dev_alloc(c.get(), px.data.size(), &d_pix));
+  c.check(pano_dev_alloc(c.get(), (size_t)PANO_PLANET_SIZE * PANO_PLANET_SIZE * 3 * sizeof(float), &d_out));
+  DevImage out((float*)d_out, DevFree{&c});
+  c.check(pano_dev_upload(c.get(), d_pix, px.ptr(), px.data.size()));
+  c.check(pano_planet_pix8_dev(c.get(), (const unsigned char*)d_pix, px.format, px.w, px.h, out.get()));
+  c.check(pano_dev_free(c.get(), d_pix));
+  return out;
 }
 
 }  // namespace pano_b200

@@ -3,8 +3,8 @@
 
   python tools/sass_diff.py OLD.so NEW.so
 
-Each library is disassembled with `cuobjdump -sass`; the source-file identifier lines are dropped, so two builds of
-the same code in different directories compare equal.  Exit status 1 when a kernel of OLD is changed or missing."""
+Each library is disassembled with `cuobjdump -sass`; the source-file identifier lines are dropped and runs of blanks
+collapsed, so two builds of the same code in different directories, or next to different kernels, compare equal.  Exit status 1 when a kernel of OLD is changed or missing."""
 import re
 import subprocess
 import sys
@@ -20,7 +20,9 @@ def kernels(so):
             funcs[cur] = []
         elif cur is not None and not line.startswith("identifier =") and "Fatbin" not in line \
                 and "code for sm_" not in line:
-            funcs[cur].append(line)
+            # runs of blanks collapsed: cuobjdump pads its columns to the widest instruction of the whole
+            # module, so a new kernel in the same file would otherwise shift an unchanged kernel's lines
+            funcs[cur].append(" ".join(line.split()))
     return {k: "\n".join(v) for k, v in funcs.items()}
 
 
