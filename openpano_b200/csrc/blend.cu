@@ -682,8 +682,8 @@ static int blend_run(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands,
     return PANO_OK;
   }
   dim3 gr(ceil_div(job.max_rw, 32), ceil_div(job.max_rh, 8), n);
-  PANO_LAUNCH(ctx, pix8 ? "k_mb_first_level_pix8" : "k_mb_first_level", k_mb_first_level<Src>, gr, b, 0, d->d_imgs, job.g,
-              d->d_cur, d->d_mask);
+  PANO_LAUNCH(ctx, pix8 ? "k_mb_first_level_pix8" : Src::kLut ? "k_mb_first_level_rgb8" : "k_mb_first_level",
+              k_mb_first_level<Src>, gr, b, 0, d->d_imgs, job.g, d->d_cur, d->d_mask);
   return mb_levels(ctx, job, d, bands, d_out, row0, row1);
 }
 
@@ -772,14 +772,15 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
     x1 = std::min(x1, job.tw); y0 = std::max(y0, s->row0); y1 = std::min(y1, s->row1);
     if (x0 >= x1 || y0 >= y1) return PANO_OK;
     dim3 g(ceil_div(x1 - x0, 32), ceil_div(y1 - y0, 8));
-    PANO_LAUNCH(ctx, pix8 ? "k_linear_accumulate_pix8" : "k_linear_accumulate", k_linear_accumulate<Src>, g, b, 0, d_win,
-                count, job.g, s->lazy, s->ordered, s->d_sum, s->d_wsum, job.tw, s->row0, x0, y0, x1, y1);
+    PANO_LAUNCH(ctx, pix8 ? "k_linear_accumulate_pix8" : Src::kLut ? "k_linear_accumulate_rgb8" : "k_linear_accumulate",
+                k_linear_accumulate<Src>, g, b, 0, d_win, count, job.g, s->lazy, s->ordered, s->d_sum, s->d_wsum, job.tw,
+                s->row0, x0, y0, x1, y1);
   } else {
     int rw = 0, rh = 0;
     for (int k = 0; k < count; ++k) { rw = std::max(rw, win[k].rw); rh = std::max(rh, win[k].rh); }
     dim3 g(ceil_div(rw, 32), ceil_div(rh, 8), count);
-    PANO_LAUNCH(ctx, pix8 ? "k_mb_first_level_pix8" : "k_mb_first_level", k_mb_first_level<Src>, g, b, 0, d_win, job.g,
-                s->dev.d_cur, s->dev.d_mask);
+    PANO_LAUNCH(ctx, pix8 ? "k_mb_first_level_pix8" : Src::kLut ? "k_mb_first_level_rgb8" : "k_mb_first_level",
+                k_mb_first_level<Src>, g, b, 0, d_win, job.g, s->dev.d_cur, s->dev.d_mask);
   }
   return PANO_OK;
 }

@@ -284,6 +284,36 @@ def test_blend_stream_layouts(engine, bands, lazy):
     assert gu.same_bits(got_dev, want)
 
 
+@pytest.mark.parametrize("bands", [0, 3])
+def test_blend_stream_profile_names(engine, bands):
+    """Each instantiation of the stream's source-reading kernel (k_linear_accumulate, k_mb_first_level) is profiled
+    under its own name: f32 sources under the kernel's, grey and interleaved RGB under _rgb8, RGBA and planar under
+    _pix8; one launch for a window of two images."""
+    p = default_params(multiband=max(bands, 1))
+    kernel = "k_mb_first_level" if bands else "k_linear_accumulate"
+    rgb, _, items, geom = _stack(2, ["rgb"] * 2)
+    dev = _Dev(engine)
+    try:
+        for fmt, name in (("f32", kernel), ("grey", kernel + "_rgb8"), ("rgb", kernel + "_rgb8"),
+                          ("rgba", kernel + "_pix8"), ("planar", kernel + "_pix8")):
+            s = engine.blend_stream([x.shape[:2] for x in rgb], items, geom, bands, p)
+            try:
+                engine.profile(True)
+                engine.profile_reset()
+                if fmt == "f32":
+                    s.add([engine.read_img_rgb8(x) for x in rgb])
+                else:
+                    _dev_stream_add(s, dev, [_lay(x, fmt) for x in rgb], fmt)
+                engine.sync()
+                prof = engine.profile_read()
+            finally:
+                engine.profile(False)
+                s.close()
+            assert {k: v[0] for k, v in prof.items() if k.startswith(kernel)} == {name: 1}, (fmt, prof)
+    finally:
+        dev.free()
+
+
 # ----------------------------------------------------------------------------- cylinder warp, conversion
 @pytest.mark.parametrize("hf", [1.0, 1.2])
 def test_cyl_warp_layouts_equal_interleaved(engine, hf):

@@ -13,11 +13,14 @@ featureset's counts are on the host.  Rows:
   planar direct      CImg's planes sent as they are (3 B/px)
   strip only         the host pass alone over all images
 Wall ms, median over --reps after one warm-up; every featureset is checked bit for bit against rgb direct's.
-Part `kernels`: device-resident sources of configs 2 and 5 (--views5 of config 5's views), per-launch times (eng
-profiling: CUDA events around each launch, median-free mean over --reps calls) of the RGB8 instantiations of
-k_pyramid_grey, k_mb_first_level (MULTIBAND 2) and k_cyl_warp_batch against the SrcPix8 ones reading RGBA or planar
-sources.  Prints one JSON line per row and a summary line with the card's name and power limit read in the same
-run.  Needs an H100."""
+Part `kernels`: device-resident grey, RGB, RGBA and planar sources of configs 2 and 5 (--views5 of config 5's
+views), per-launch times (eng profiling: CUDA events around each launch, median-free mean over --reps calls) of
+every kernel that reads 8-bit sources: k_pyramid_grey (SIFT batch), k_linear_blend (blend_rgb8_dev, bands 0),
+k_linear_accumulate (a blend stream of device sources, windows of 1), k_mb_first_level (MULTIBAND 2),
+k_cyl_warp_batch and k_planet8 (each source image as the mosaic).  Each row names the profile entry it read: the
+one kernel the call launched whose name starts with the kernel's, so the same script times builds that name their
+8-bit instantiations differently (PANO_B200_LIB picks the build).  Prints one JSON line per row and a summary line
+with the card's name and power limit read in the same run.  Needs an H100."""
 from __future__ import annotations
 
 import argparse
@@ -130,7 +133,7 @@ def stream_part(a, rows):
 def kernel_part(a, rows):
     from openpano_b200 import synth
     from openpano_b200._abi import default_params
-    from openpano_b200.capi import PIX_RGB, PIX_RGB_PLANAR, PIX_RGBA, Engine
+    from openpano_b200.capi import PIX_FORMATS, SRC_RGB8_DEV, Engine
 
     eng = Engine(0)
     for cfg in ("2", "5"):
@@ -138,25 +141,39 @@ def kernel_part(a, rows):
         n, (h, w) = len(imgs), imgs[0].shape[:2]
         rgb = [(im * 255.0 + 0.5).astype(np.uint8) for im in imgs]
         del imgs
-        bufs = {"rgb": rgb, "rgba": [np.concatenate([x, np.full((h, w, 1), 255, np.uint8)], 2) for x in rgb],
+        bufs = {"grey": [np.ascontiguousarray(x[..., 0]) for x in rgb], "rgb": rgb,
+                "rgba": [np.concatenate([x, np.full((h, w, 1), 255, np.uint8)], 2) for x in rgb],
                 "planar": [np.ascontiguousarray(np.moveaxis(x, 2, 0)) for x in rgb]}
-        codes = {"rgb": PIX_RGB, "rgba": PIX_RGBA, "planar": PIX_RGB_PLANAR}
         items, geom = synth.translation_blend_setup(org, w, h)
         tw, th = max(it[2] for it in items), max(it[3] for it in items)
         p = default_params()
         pb = default_params(multiband=2)
         ow, oh = eng.cyl_warp_shape(w, h, 1.0, p)[:2]
-        d_out = eng.dev_alloc(max(tw * th, ow * oh * n) * 12)
+        d_out = eng.dev_alloc(max(tw * th, ow * oh * n, Engine.PLANET_SIZE ** 2) * 12)
         warp_out = [d_out + k * ow * oh * 12 for k in range(n)]
-        for fmt in ("rgb", "rgba", "planar"):
+
+        def stream_blend(d_src, code):
+            s = eng.blend_stream([(h, w)] * n, items, geom, 0, p)
+            try:
+                for d in d_src:
+                    s.add([d], SRC_RGB8_DEV, code)
+                s.finish_dev(d_out)
+            finally:
+                s.close()
+
+        for fmt, code in PIX_FORMATS.items():
             d_src = [eng.dev_alloc(x.nbytes) for x in bufs[fmt]]
             for d, x in zip(d_src, bufs[fmt]):
                 eng.dev_upload(d, x)
-            ch = [codes[fmt]] * n
+            ch = [code] * n
+            # kernel -> a call that launches it; the profile entry is the one name that starts with the kernel's
             ops = {
                 "k_pyramid_grey": lambda: eng.sift_detect_batch_rgb8_ptr(d_src, [w] * n, [h] * n, ch, p, device=True).free(),
+                "k_linear_blend": lambda: eng.blend_rgb8_dev(d_src, ch, [(h, w)] * n, items, geom, d_out, tw, th, 0, p),
+                "k_linear_accumulate": lambda: stream_blend(d_src, code),
                 "k_mb_first_level": lambda: eng.blend_rgb8_dev(d_src, ch, [(h, w)] * n, items, geom, d_out, tw, th, 2, pb),
-                "k_cyl_warp_batch": lambda: eng.cyl_warp_batch_rgb8_dev(d_src, ch, [(h, w)] * n, warp_out, None, 1.0, p),
+                "k_cyl_warp": lambda: eng.cyl_warp_batch_rgb8_dev(d_src, ch, [(h, w)] * n, warp_out, None, 1.0, p),
+                "k_planet": lambda: [eng.planet_pix8_dev(d, code, w, h, d_out) for d in d_src],
             }
             for kernel, op in ops.items():
                 op()
@@ -168,8 +185,7 @@ def kernel_part(a, rows):
                 eng.sync()
                 prof = eng.profile_read()
                 eng.profile(False)
-                name = [k for k in prof if k.startswith(kernel.replace("_batch", "")) and
-                        (k.endswith("_pix8") == (fmt != "rgb"))]
+                name = [k for k in prof if k.startswith(kernel)]
                 assert len(name) == 1, (kernel, fmt, sorted(prof))
                 launches, ms = prof[name[0]]
                 rows.append(emit(dict(part="kernels", config=cfg, n=n, w=w, h=h, kernel=name[0], source=fmt,
