@@ -522,6 +522,76 @@ int  pano_blend_stream_create_rows(pano_ctx* ctx, int n, const pano_blend_image*
  * rows [y0, y1] meet [row0, row1).  A stream of the whole canvas needs every image. */
 int  pano_blend_stream_needs(const pano_blend_stream* s, unsigned char* flags);
 
+/* A sweep of the canvas's row strips, top to bottom, that hands each source over once while it stays in use:
+ * blend, crop() and write_rgb's conversion of pano_blend's mosaic strip by strip (the bytes of
+ * pano_rgb8_crop_to_pix8_dev on the canvas the row-strip streams give), with a source kept on the device from
+ * the first strip that reads it to the last one, as far as `keep_bytes` allows.
+ *
+ * The schedule is fixed up front by pano_blend_sweep_plan, which needs no device.  Strip s covers rows
+ * [s * strip_rows, min(out_h, (s + 1) * strip_rows)) and reads the images blend_stream_needs reports for a row
+ * stream of those rows.  Between strips the sweep keeps at most keep_bytes of sources (src_bytes[k] each) that
+ * a later strip reads; when one must make room, the kept source whose next use is farthest away goes (ties: the
+ * higher image index).  The sources of the current strip are always on the device.  So keep_bytes = 0 hands
+ * over every source each strip reads, strip by strip, and keep_bytes = SIZE_MAX each source that some strip
+ * reads exactly once; a source no strip reads is never asked for.
+ *
+ * pano_blend_sweep_plan: imgs / g / bands / p / out_w / out_h as for pano_blend (g is not read: the read sets
+ * do not depend on the projection), strip_rows >= 1, src_bytes[k] > 0.  Every output may be NULL.  With
+ * S = ceil(out_h / strip_rows) strips, reads / uploads / kept are S×n flags: strip s reads image k; image k is
+ * handed over for strip s; that copy is kept for a later strip.  *uploads and *upload_bytes count the
+ * hand-overs, *retained_high is the most bytes kept between two strips.  Bad arguments return
+ * PANO_ERR_INVALID. */
+int  pano_blend_sweep_plan(int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
+                           const pano_params* p, int out_w, int out_h, int strip_rows, const size_t* src_bytes,
+                           size_t keep_bytes, int* n_strips, unsigned char* reads, unsigned char* uploads,
+                           unsigned char* kept, long long* n_uploads, unsigned long long* upload_bytes,
+                           unsigned long long* retained_high);
+/* The sweep object: create; then, until next returns -1, next and strip; then finish_dev once.
+ *
+ * Device memory, besides the per-image table and the projection tables (8 B per canvas row and column for
+ * non-flat projections, built once):
+ *   - one strip's row-stream state (pano_blend_stream_create_rows; the tallest strip's at most), and 12 B per
+ *     strip pixel of its f32 rows;
+ *   - 3 B per canvas pixel (the 8-bit canvas) plus the output's bytes per canvas pixel (finish_dev's d_out is
+ *     the caller's);
+ *   - two host sources in a two-slot ring (each slot as large as the largest source uploaded through it): a
+ *     host source handed over starts a window of the strip's row stream and is uploaded just before it;
+ *   - copies of the kept ones: at most keep_bytes between strips, and during a strip at most keep_bytes plus
+ *     the bytes of that strip's sources.
+ * Device sources are read in place and take none of the last two.
+ *
+ * Calls on a sweep are calls on its ctx (same threading rule); the ctx must outlive it.  A misuse (null
+ * pointers, bad arguments, a source missing where `want` was set or given where it was not, a source larger
+ * than its src_bytes, a strip after the last, finish before the last strip or twice) returns
+ * PANO_ERR_INVALID, and every failure is sticky.  pano_blend_sweep_free is always valid, and the ctx stays
+ * usable. */
+typedef struct pano_blend_sweep pano_blend_sweep;
+/* imgs / g / bands / p / out_w / out_h as for pano_blend; strip_rows / src_bytes / keep_bytes as for
+ * pano_blend_sweep_plan (src_bytes NULL: w·h·3 per image).  crop != 0: finish_dev crops as crop() does
+ * (canvases up to 80,000 columns).  Builds the projection tables and the plan. */
+int  pano_blend_sweep_create(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g,
+                             int bands, const pano_params* p, int out_w, int out_h, int strip_rows,
+                             const size_t* src_bytes, size_t keep_bytes, int crop, pano_blend_sweep** out);
+/* The index of the next strip, or -1 once every strip has run.  want (n bytes, may be NULL): 1 for the images
+ * the caller must hand to that strip (the plan's uploads), else 0. */
+int  pano_blend_sweep_next(pano_blend_sweep* s, unsigned char* want);
+/* Runs the next strip.  srcs has n entries, non-null exactly where next's `want` is set; formats[k] is the
+ * PANO_PIX_* format of srcs[k] for the 8-bit kinds (3 for f32; formats may be NULL for f32 kinds), and kind
+ * one pano_src_kind for every source of the call.  Host sources are uploaded on the sweep's copy stream while
+ * the previous strip's kernels run; PAGEABLE buffers are staged and may be reused on return, PINNED ones must
+ * stay untouched until the next strip or finish call has returned.  Device sources are read in place, also by
+ * the later strips the plan keeps them for: they must stay valid until finish_dev has been queued. */
+int  pano_blend_sweep_strip(pano_blend_sweep* s, const void* const* srcs, const int* formats, int kind);
+/* Valid once every strip has run, once.  Queues the mosaic's bytes in out_format (PANO_PIX_RGB, _RGBA or
+ * _RGB_PLANAR, as pano_rgb8_crop_to_pix8_dev) into d_out (out_w·out_h·(4 for RGBA, else 3) bytes) on the ctx
+ * stream and writes the rectangle {x0, y0, width, height} to rect (the whole canvas without crop). */
+int  pano_blend_sweep_finish_dev(pano_blend_sweep* s, int out_format, unsigned char* d_out, int rect[4]);
+/* What the strips run so far handed over: sources, their src_bytes, and the most bytes kept between two strips
+ * (the plan's numbers once every strip has run).  Any output may be NULL. */
+int  pano_blend_sweep_stats(const pano_blend_sweep* s, long long* uploads, unsigned long long* upload_bytes,
+                            unsigned long long* retained_high);
+void pano_blend_sweep_free(pano_blend_sweep* s);
+
 /* SIFT whose sources arrive in windows: LAZY_READ's feature stage (config.cfg:10-11, calc_feature in
  * stitcherbase.cc:9-27 loads, detects and releases one image at a time) on the device.  For every
  * partition of the images into windows and every source kind, the featureset from pano_sift_stream_finish

@@ -113,6 +113,19 @@ def _load():
                                                     C.POINTER(PanoBlendGeom), C.c_int, P, C.c_int, C.c_int, C.c_int,
                                                     C.c_int, _vpp]),
         "pano_blend_stream_needs": (C.c_int, [C.c_void_p, C.c_void_p]),
+        "pano_blend_sweep_plan": (C.c_int, [C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom), C.c_int, P,
+                                            C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t), C.c_size_t, _ip,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong),
+                                            C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]),
+        "pano_blend_sweep_create": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom),
+                                              C.c_int, P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t),
+                                              C.c_size_t, C.c_int, _vpp]),
+        "pano_blend_sweep_next": (C.c_int, [C.c_void_p, C.c_void_p]),
+        "pano_blend_sweep_strip": (C.c_int, [C.c_void_p, _vpp, _ip, C.c_int]),
+        "pano_blend_sweep_finish_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, _ip]),
+        "pano_blend_sweep_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_longlong), C.POINTER(C.c_ulonglong),
+                                             C.POINTER(C.c_ulonglong)]),
+        "pano_blend_sweep_free": (None, [C.c_void_p]),
         "pano_sift_stream_create": (C.c_int, [C.c_void_p, C.c_int, _ip, _ip, P, _vpp]),
         "pano_sift_stream_add": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _vpp, C.c_int, C.c_int]),
         "pano_sift_stream_finish": (C.c_int, [C.c_void_p, _vpp]),
@@ -470,6 +483,83 @@ class BlendStream(_SourceStream):
 
     def finish_dev(self, d_out):
         self._call(LIB.pano_blend_stream_finish_dev(self._h, C.c_void_p(d_out or 0)))
+
+
+SIZE_MAX = (1 << 64) - 1     # keep_bytes without a limit
+
+
+def blend_sweep_plan(shapes, items, geom, bands, strip_rows, src_bytes, keep_bytes, params=None):
+    """pano_blend_sweep_plan (no device needed): the strip schedule of a blend sweep.  Returns a dict with the
+    strips × n bool arrays "reads", "uploads" and "kept" and the totals "n_uploads", "upload_bytes" and
+    "retained_high"."""
+    params = params or default_params()
+    n = len(items)
+    arr, g = Engine._blend_args([None] * n, shapes, items, geom)
+    ow, oh = max(it[2] for it in items), max(it[3] for it in items)
+    S = -(-oh // strip_rows) if strip_rows > 0 else 0
+    flags = [np.zeros(max(S * n, 1), np.uint8) for _ in range(3)]
+    nb = (C.c_size_t * n)(*[int(b) for b in src_bytes])
+    ns, nu = C.c_int(), C.c_longlong()
+    ub, rh = C.c_ulonglong(), C.c_ulonglong()
+    rc = LIB.pano_blend_sweep_plan(n, arr, C.byref(g), bands, C.byref(params), ow, oh, strip_rows, nb,
+                                   min(int(keep_bytes), SIZE_MAX), C.byref(ns), *(f.ctypes.data for f in flags),
+                                   C.byref(nu), C.byref(ub), C.byref(rh))
+    if rc != 0:
+        raise PanoError(rc, "blend sweep plan: bad argument")
+    reads, uploads, kept = (f[:S * n].reshape(S, n).astype(bool) for f in flags)
+    return {"reads": reads, "uploads": uploads, "kept": kept, "n_uploads": nu.value, "upload_bytes": ub.value,
+            "retained_high": rh.value}
+
+
+class BlendSweep:
+    """A pano_blend_sweep: the canvas's row strips top to bottom, each source handed over once while a later strip
+    still reads it (within keep_bytes), then the cropped 8-bit mosaic.  next() gives the next strip and the images
+    it wants, strip() takes them."""
+
+    def __init__(self, eng, handle, n, out_w, out_h):
+        self.eng, self._h, self.n, self.out_w, self.out_h = eng, handle, n, out_w, out_h
+
+    def _call(self, rc):
+        if rc != 0:
+            self.eng._raise(rc)
+
+    def next(self):
+        """(strip index or -1, bool array of the images strip() must be given)."""
+        want = np.zeros(max(self.n, 1), np.uint8)
+        r = LIB.pano_blend_sweep_next(self._h, want.ctypes.data)
+        if r < -1:
+            self._call(r)
+        return r, want[:self.n].astype(bool)
+
+    def strip(self, ptrs, formats, kind):
+        """ptrs: n raw pointers (0 where next() did not ask), formats: n PANO_PIX_* codes (3 for f32 kinds)."""
+        src = (C.c_void_p * max(self.n, 1))(*[int(q or 0) for q in ptrs])
+        fm = (C.c_int * max(self.n, 1))(*[int(f) for f in formats])
+        self._call(LIB.pano_blend_sweep_strip(self._h, src, fm, kind))
+
+    def finish_dev(self, fmt, d_out):
+        """Queues the mosaic's bytes in layout fmt into d_out; returns the rectangle {x0, y0, w, h}."""
+        code = PIX_FORMATS.get(fmt, fmt) if isinstance(fmt, str) else fmt
+        r = np.zeros(4, np.int32)
+        self._call(LIB.pano_blend_sweep_finish_dev(self._h, int(code), C.c_void_p(d_out or 0), _i(r)))
+        return r
+
+    def stats(self):
+        """(uploads, uploaded bytes, most bytes kept between two strips) so far."""
+        u, b, r = C.c_longlong(), C.c_ulonglong(), C.c_ulonglong()
+        self._call(LIB.pano_blend_sweep_stats(self._h, C.byref(u), C.byref(b), C.byref(r)))
+        return u.value, b.value, r.value
+
+    def close(self):
+        if self._h:
+            LIB.pano_blend_sweep_free(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class SiftStream(_SourceStream):
@@ -996,6 +1086,22 @@ class Engine:
         self._check(LIB.pano_blend_stream_create_rows(self._h, len(items), arr, C.byref(g), bands, C.byref(params),
                                                       ow.value, oh.value, row0, row1, C.byref(h)))
         return BlendStream(self, h, shapes, ow.value, oh.value, (row0, row1))
+
+    def blend_sweep(self, shapes, items, geom, strip_rows, keep_bytes, bands=0, params=None, crop=True,
+                    src_bytes=None) -> BlendSweep:
+        """A blend sweep (pano_blend_sweep_create) of strips of strip_rows canvas rows, keeping at most keep_bytes of
+        sources (SIZE_MAX: no limit) between strips; src_bytes: each source's bytes (None: h·w·3)."""
+        params = params or default_params()
+        n = len(items)
+        arr, g = self._blend_args([None] * n, shapes, items, geom)
+        ow, oh = C.c_int(), C.c_int()
+        self._check(LIB.pano_blend_target_size(n, arr, C.byref(ow), C.byref(oh)))
+        nb = (C.c_size_t * n)(*[int(b) for b in src_bytes]) if src_bytes is not None else None
+        h = C.c_void_p()
+        self._check(LIB.pano_blend_sweep_create(self._h, n, arr, C.byref(g), bands, C.byref(params), ow.value, oh.value,
+                                                strip_rows, nb, min(int(keep_bytes), SIZE_MAX), 1 if crop else 0,
+                                                C.byref(h)))
+        return BlendSweep(self, h, n, ow.value, oh.value)
 
     def blend_lazy(self, imgs, items, geom, bands=0, params=None, window=1, fmt=None):
         """blend() with the sources added `window` images at a time (an int, or a list of window sizes):

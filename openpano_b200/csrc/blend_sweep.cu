@@ -1,0 +1,357 @@
+// blend_sweep.cu — the row strips of the canvas, top to bottom, with every source handed over once while it stays
+// in use (pano_blend_sweep_*, pano_b200.h).
+//
+// A row-strip stream (pano_blend_stream_create_rows) holds two windows of sources at most, so a strip-by-strip
+// writer uploads a source once for every strip it reaches.  The strips run in order and the images each one reads
+// are known up front (blend_strip_reads), so the sweep plans the whole access sequence at creation: a source read
+// again later is kept on the device, within keep_bytes, evicting the kept source whose next use is farthest away.
+// Each strip then runs an ordinary row-strip stream over device pointers (its kernels, its bits), feeds the crop
+// scan and converts its rows into the 8-bit canvas, as stitcher.mosaic_rgb8_strips does.
+//
+// Host sources go one per window through an UploadRing on the ring's copy stream, so each crosses PCIe while the
+// kernels of the window before it run, this strip's or the previous one's.  A kept one is then copied on the ctx
+// stream into a block of its own, freed in stream order when the plan drops it: every reader and the free are on the
+// ctx stream, so the ring's ordering is the only cross-stream ordering there is.
+#include "common.cuh"
+#include "blend_rows.cuh"
+
+#include <algorithm>
+#include <climits>
+#include <cstdint>
+#include <memory>
+#include <vector>
+
+namespace {
+
+struct SweepPlan {
+  int n = 0, strips = 0;
+  std::vector<unsigned char> reads, uploads, kept, held;   // strips × n; held: kept once the strip has run
+  long long n_uploads = 0;
+  unsigned long long upload_bytes = 0, retained_high = 0;
+};
+
+int make_plan(int n, const pano_blend_image* imgs, int bands, const pano_params* p, int ow, int oh, int strip_rows,
+              const size_t* bytes, size_t keep, SweepPlan* pl) {
+  if (n <= 0 || n > PANO_MAX_IMAGES || !imgs || !p || !bytes || bands < 0 || strip_rows < 1 || ow <= 0 || oh <= 0)
+    return PANO_ERR_INVALID;
+  int tw = 0, th = 0;
+  for (int k = 0; k < n; ++k) {
+    const pano_blend_image& s = imgs[k];
+    if (s.w < 2 || s.h < 2 || s.x1 < s.x0 || s.y1 < s.y0 || s.x0 < 0 || s.y0 < 0 || bytes[k] == 0) return PANO_ERR_INVALID;
+    tw = std::max(tw, s.x1); th = std::max(th, s.y1);
+  }
+  if (tw != ow || th != oh) return PANO_ERR_INVALID;
+  const int halo = blend_halo(bands, p);
+  if (halo < 0) return PANO_ERR_INVALID;
+  const int S = (int)(((long long)oh + strip_rows - 1) / strip_rows);
+  const size_t cells = (size_t)S * n;
+  pl->n = n; pl->strips = S;
+  pl->reads.assign(cells, 0); pl->uploads.assign(cells, 0); pl->kept.assign(cells, 0); pl->held.assign(cells, 0);
+  for (int s = 0; s < S; ++s) {
+    const int r0 = s * strip_rows, r1 = (int)std::min<long long>(oh, (long long)r0 + strip_rows);
+    for (int k = 0; k < n; ++k) pl->reads[(size_t)s * n + k] = blend_strip_reads(imgs[k], bands, halo, oh, r0, r1);
+  }
+  // next_use[s * n + k]: the first strip after s that reads k, S for none
+  std::vector<int> next_use(cells), nxt(n, S);
+  for (int s = S - 1; s >= 0; --s)
+    for (int k = 0; k < n; ++k) {
+      next_use[(size_t)s * n + k] = nxt[k];
+      if (pl->reads[(size_t)s * n + k]) nxt[k] = s;
+    }
+  std::vector<unsigned char> resident(n, 0);
+  std::vector<int> cand;
+  for (int s = 0; s < S; ++s) {
+    const unsigned char* rd = &pl->reads[(size_t)s * n];
+    const int* nu = &next_use[(size_t)s * n];
+    for (int k = 0; k < n; ++k)
+      if (rd[k] && !resident[k]) {
+        pl->uploads[(size_t)s * n + k] = 1;
+        ++pl->n_uploads;
+        pl->upload_bytes += bytes[k];
+      }
+    // what may stay once the strip has run: resident or just read, and read again later
+    cand.clear();
+    unsigned long long total = 0;
+    for (int k = 0; k < n; ++k)
+      if ((resident[k] || rd[k]) && nu[k] < S) { cand.push_back(k); total += bytes[k]; }
+    // evict the farthest next use first (ties: the higher index) until the rest fits
+    std::sort(cand.begin(), cand.end(), [&](int a, int b) { return nu[a] != nu[b] ? nu[a] > nu[b] : a > b; });
+    size_t q = 0;
+    while (q < cand.size() && total > keep) total -= bytes[cand[q++]];
+    std::fill(resident.begin(), resident.end(), 0);
+    for (; q < cand.size(); ++q) resident[cand[q]] = 1;
+    for (int k = 0; k < n; ++k) {
+      pl->held[(size_t)s * n + k] = resident[k];
+      pl->kept[(size_t)s * n + k] = pl->uploads[(size_t)s * n + k] && resident[k];
+    }
+    pl->retained_high = std::max(pl->retained_high, total);
+  }
+  return PANO_OK;
+}
+
+// One image's source while the plan keeps it: a block of the sweep's own (host sources) or the caller's device
+// pointer.
+struct Held {
+  const void* ptr = nullptr;
+  DevBuf<unsigned char> own;
+  bool u8 = true;
+  int fmt = PANO_PIX_RGB;
+};
+
+struct StreamFree { void operator()(pano_blend_stream* s) const { pano_blend_stream_free(s); } };
+struct ScanFree { void operator()(pano_crop_scan* c) const { pano_crop_scan_free(c); } };
+
+}  // namespace
+
+struct pano_blend_sweep {
+  pano_ctx* ctx = nullptr;
+  int n = 0, bands = 0, ow = 0, oh = 0, rows = 0;
+  pano_params p;
+  pano_blend_geom g;
+  std::vector<pano_blend_image> imgs;
+  std::vector<size_t> bytes;
+  SweepPlan plan;
+  DevBuf<double> d_tab;            // projection tables of every strip (empty for flat)
+  DevBuf<float> d_strip;           // one strip's f32 rows
+  DevBuf<unsigned char> d_rgb;     // the 8-bit canvas
+  DevBuf<int> d_rect;
+  std::unique_ptr<pano_crop_scan, ScanFree> scan;
+  std::vector<Held> held;
+  int done = 0, err = 0;
+  bool finished = false;
+  long long uploads = 0;
+  unsigned long long upload_bytes = 0, retained_high = 0;
+  UploadRing ring;                 // last: its copy stream drains before the blocks above go
+};
+
+static int sweep_fail(pano_blend_sweep* s, int rc) { s->err = rc; return rc; }
+#define SWEEP_MISUSE(s, ...) sweep_fail((s), ctx_fail((s)->ctx, PANO_ERR_INVALID, __VA_ARGS__))
+#define SWEEP_CUDA(s, call)                                                \
+  do {                                                                     \
+    cudaError_t _e = (call);                                               \
+    if (_e != cudaSuccess) return sweep_fail((s), ctx_cuda((s)->ctx, _e, #call)); \
+  } while (0)
+
+// The uploads of the previous strip are over: its pinned buffers are the caller's again.
+static int sweep_wait_previous(pano_blend_sweep* s) {
+  if (s->ring.copy)
+    for (int b = 0; b < 2; ++b) SWEEP_CUDA(s, cudaEventSynchronize(s->ring.ev_copied[b].get()));
+  return PANO_OK;
+}
+
+// Runs rows [row0, row1) of strip st as a row-strip stream into d_strip.  Windows are runs of sources of one kind
+// and format, and a host source handed over starts a window of its own: it is uploaded through the ring just
+// before that window is added, so the ring holds two sources and the next upload overlaps this window's kernels.
+// A kept one is then copied into a block of its own.  srcs / u8 / host / fmt / sz: the strip call's, checked.
+static int sweep_blend(pano_blend_sweep* s, int st, const void* const* srcs, bool u8, bool host,
+                       const std::vector<int>& fmt, const std::vector<size_t>& sz) {
+  pano_ctx* ctx = s->ctx;
+  const int n = s->n;
+  const unsigned char* up = &s->plan.uploads[(size_t)st * n];
+  const unsigned char* rd = &s->plan.reads[(size_t)st * n];
+  const unsigned char* keep = &s->plan.kept[(size_t)st * n];
+  const int row0 = st * s->rows, row1 = std::min(s->oh, row0 + s->rows);
+  std::vector<const void*> src(n, nullptr);   // null: not read, or a host source not uploaded yet
+  std::vector<char> su8(n, 0);
+  std::vector<int> sf(n, 3);
+  for (int k = 0; k < n; ++k) {
+    if (!rd[k]) continue;
+    if (up[k]) {
+      su8[k] = u8; sf[k] = fmt[k];
+      if (host) continue;
+      src[k] = srcs[k];
+      if (keep[k]) { s->held[k] = Held(); s->held[k].ptr = srcs[k]; s->held[k].u8 = u8; s->held[k].fmt = fmt[k]; }
+    } else {
+      src[k] = s->held[k].ptr; su8[k] = s->held[k].u8; sf[k] = s->held[k].fmt;
+    }
+  }
+  pano_blend_stream* raw = nullptr;
+  int rc = blend_stream_open(ctx, n, s->imgs.data(), &s->g, s->bands, &s->p, s->ow, s->oh, row0, row1,
+                             s->d_tab.get(), &raw);
+  if (rc) return rc;
+  std::unique_ptr<pano_blend_stream, StreamFree> bs(raw);
+  for (int k0 = 0; k0 < n;) {
+    int k1 = k0, first = -1, upload = -1;
+    for (; k1 < n; ++k1) {
+      if (!rd[k1]) continue;
+      const bool fresh = host && up[k1];
+      if (first >= 0 && (fresh || su8[k1] != su8[first] || sf[k1] != sf[first])) break;
+      if (first < 0) { first = k1; if (fresh) upload = k1; }
+    }
+    int slot = -1;
+    if (upload >= 0) {
+      if (!s->ring.copy)
+        if (cudaError_t e = s->ring.init()) return ctx_cuda(ctx, e, "blend sweep: copy stream / events");
+      if ((rc = s->ring.upload(ctx, 1, &srcs[upload], &sz[upload], &src[upload], &slot))) return rc;
+      if (keep[upload]) {
+        Held& h = s->held[upload];
+        h = Held();
+        h.u8 = u8; h.fmt = fmt[upload];
+        if ((rc = h.own.alloc(ctx, sz[upload]))) return rc;
+        PANO_CUDA(ctx, cudaMemcpyAsync(h.own, src[upload], sz[upload], cudaMemcpyDeviceToDevice, ctx->stream));
+        h.ptr = h.own.get();
+      }
+    }
+    const bool w8 = first >= 0 && su8[first];
+    if ((rc = pano_blend_stream_add(bs.get(), k0, k1 - k0, src.data() + k0, w8 ? PANO_SRC_RGB8_DEV : PANO_SRC_F32_DEV,
+                                    first >= 0 ? sf[first] : 3)))
+      return rc;
+    if (slot >= 0) PANO_CUDA(ctx, s->ring.release(ctx, slot));
+    k0 = k1;
+  }
+  return pano_blend_stream_finish_dev(bs.get(), s->d_strip);
+}
+
+extern "C" {
+
+int pano_blend_sweep_plan(int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
+                          const pano_params* p, int out_w, int out_h, int strip_rows, const size_t* src_bytes,
+                          size_t keep_bytes, int* n_strips, unsigned char* reads, unsigned char* uploads,
+                          unsigned char* kept, long long* n_uploads, unsigned long long* upload_bytes,
+                          unsigned long long* retained_high) {
+  if (!g) return PANO_ERR_INVALID;
+  SweepPlan pl;
+  if (int rc = make_plan(n, imgs, bands, p, out_w, out_h, strip_rows, src_bytes, keep_bytes, &pl)) return rc;
+  if (n_strips) *n_strips = pl.strips;
+  if (reads) std::copy(pl.reads.begin(), pl.reads.end(), reads);
+  if (uploads) std::copy(pl.uploads.begin(), pl.uploads.end(), uploads);
+  if (kept) std::copy(pl.kept.begin(), pl.kept.end(), kept);
+  if (n_uploads) *n_uploads = pl.n_uploads;
+  if (upload_bytes) *upload_bytes = pl.upload_bytes;
+  if (retained_high) *retained_high = pl.retained_high;
+  return PANO_OK;
+}
+
+int pano_blend_sweep_create(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g,
+                            int bands, const pano_params* p, int out_w, int out_h, int strip_rows,
+                            const size_t* src_bytes, size_t keep_bytes, int crop, pano_blend_sweep** out) {
+  ctx_enter(ctx);
+  if (!ctx || !out) return PANO_ERR_INVALID;
+  *out = nullptr;
+  if (n <= 0 || !imgs || !g || !p || bands < 0 || strip_rows < 1) return ctx_fail(ctx, PANO_ERR_INVALID, "blend sweep: bad argument");
+  if (n > PANO_MAX_IMAGES) return ctx_fail(ctx, PANO_ERR_INVALID, "blend sweep: %d images (limit %d)", n, PANO_MAX_IMAGES);
+  std::unique_ptr<pano_blend_sweep> s(new pano_blend_sweep);
+  s->ctx = ctx; s->n = n; s->bands = bands; s->ow = out_w; s->oh = out_h; s->rows = std::min(strip_rows, out_h);
+  s->p = *p; s->g = *g;
+  s->imgs.assign(imgs, imgs + n);
+  std::vector<double> tab;
+  int rc = blend_sweep_tables(ctx, n, imgs, g, bands, p, out_w, out_h, &tab);
+  if (rc) return rc;
+  s->bytes.resize(n);
+  for (int k = 0; k < n; ++k) s->bytes[k] = src_bytes ? src_bytes[k] : (size_t)imgs[k].w * imgs[k].h * 3;
+  if (make_plan(n, imgs, bands, p, out_w, out_h, strip_rows, s->bytes.data(), keep_bytes, &s->plan))
+    return ctx_fail(ctx, PANO_ERR_INVALID, "blend sweep: a source of 0 bytes");
+  if (!tab.empty()) {
+    if ((rc = s->d_tab.alloc(ctx, tab.size()))) return rc;
+    if ((rc = ctx_put(ctx, s->d_tab, tab.data(), tab.size() * sizeof(double)))) return rc;
+  }
+  if ((rc = s->d_strip.alloc(ctx, (size_t)s->rows * out_w * 3))) return rc;
+  if ((rc = s->d_rgb.alloc(ctx, (size_t)out_w * out_h * 3))) return rc;
+  if ((rc = s->d_rect.alloc(ctx, 4))) return rc;
+  if (crop) {
+    pano_crop_scan* c = nullptr;
+    if ((rc = pano_crop_scan_create(ctx, out_w, out_h, &c))) return rc;
+    s->scan.reset(c);
+  }
+  s->held.resize(n);
+  *out = s.release();
+  return PANO_OK;
+}
+
+int pano_blend_sweep_next(pano_blend_sweep* s, unsigned char* want) {
+  if (!s) return PANO_ERR_INVALID;
+  ctx_enter(s->ctx);
+  if (s->err) return s->err;
+  const bool over = s->done >= s->plan.strips;
+  if (want)
+    for (int k = 0; k < s->n; ++k) want[k] = over ? 0 : s->plan.uploads[(size_t)s->done * s->n + k];
+  return over ? -1 : s->done;
+}
+
+int pano_blend_sweep_strip(pano_blend_sweep* s, const void* const* srcs, const int* formats, int kind) {
+  if (!s) return PANO_ERR_INVALID;
+  pano_ctx* ctx = s->ctx;
+  ctx_enter(ctx);
+  if (s->err) return s->err;
+  if (s->finished || s->done >= s->plan.strips) return SWEEP_MISUSE(s, "blend sweep: strip after the last");
+  if (!srcs) return SWEEP_MISUSE(s, "blend sweep: null source list");
+  const bool u8 = kind == PANO_SRC_RGB8_DEV || kind == PANO_SRC_RGB8_HOST;
+  const bool host = kind == PANO_SRC_F32_HOST || kind == PANO_SRC_RGB8_HOST;
+  if (!u8 && kind != PANO_SRC_F32_DEV && kind != PANO_SRC_F32_HOST) return SWEEP_MISUSE(s, "blend sweep: unknown source kind %d", kind);
+  if (u8 && !formats) return SWEEP_MISUSE(s, "blend sweep: null format list");
+  const int n = s->n, st = s->done;
+  const unsigned char* up = &s->plan.uploads[(size_t)st * n];
+  std::vector<int> fmt(n, 3);
+  std::vector<size_t> sz(n, 0);
+  std::vector<int> list;           // the images handed over, in order
+  for (int k = 0; k < n; ++k) {
+    if (!srcs[k] && up[k]) return SWEEP_MISUSE(s, "blend sweep: strip %d needs image %d", st, k);
+    if (srcs[k] && !up[k]) return SWEEP_MISUSE(s, "blend sweep: strip %d was not to be given image %d", st, k);
+    if (!srcs[k]) continue;
+    fmt[k] = u8 ? formats[k] : 3;
+    if (u8 && !pix8_bytes(fmt[k])) return SWEEP_MISUSE(s, "blend sweep: image %d: format %#x", k, fmt[k]);
+    if (u8 && !host)
+      if (int rc = pix8_check(ctx, "blend sweep", k, fmt[k], srcs[k])) return sweep_fail(s, rc);
+    sz[k] = (size_t)s->imgs[k].w * s->imgs[k].h * (u8 ? (size_t)pix8_bytes(fmt[k]) : 3 * sizeof(float));
+    if (sz[k] > s->bytes[k])
+      return SWEEP_MISUSE(s, "blend sweep: image %d takes %zu bytes, planned with %zu", k, sz[k], s->bytes[k]);
+    list.push_back(k);
+  }
+  if (int rc = sweep_wait_previous(s)) return rc;
+  if (int rc = sweep_blend(s, st, srcs, u8, host, fmt, sz)) return sweep_fail(s, rc);
+  const int row0 = st * s->rows, row1 = std::min(s->oh, row0 + s->rows);
+  if (s->scan)
+    if (int rc = pano_crop_scan_add_dev(s->scan.get(), s->d_strip, row1 - row0)) return sweep_fail(s, rc);
+  if (int rc = pano_mat32f_to_rgb8_dev(ctx, s->d_strip, s->ow, row1 - row0, nullptr, s->d_rgb + (size_t)row0 * s->ow * 3))
+    return sweep_fail(s, rc);
+  // drop what the plan does not keep past this strip (freed in stream order, after its readers)
+  unsigned long long kept_bytes = 0;
+  const unsigned char* hold = &s->plan.held[(size_t)st * n];
+  for (int k = 0; k < n; ++k) {
+    if (!hold[k]) s->held[k] = Held();
+    else kept_bytes += s->bytes[k];
+  }
+  s->uploads += (long long)list.size();
+  for (int k : list) s->upload_bytes += s->bytes[k];
+  s->retained_high = std::max(s->retained_high, kept_bytes);
+  ++s->done;
+  return PANO_OK;
+}
+
+int pano_blend_sweep_finish_dev(pano_blend_sweep* s, int out_format, unsigned char* d_out, int rect[4]) {
+  if (!s) return PANO_ERR_INVALID;
+  pano_ctx* ctx = s->ctx;
+  ctx_enter(ctx);
+  if (s->err) return s->err;
+  if (!d_out || !rect) return SWEEP_MISUSE(s, "blend sweep: null output");
+  if (s->finished) return SWEEP_MISUSE(s, "blend sweep: already finished");
+  if (s->done < s->plan.strips) return SWEEP_MISUSE(s, "blend sweep: finish after %d of %d strips", s->done, s->plan.strips);
+  if (out_format != PANO_PIX_RGB && out_format != PANO_PIX_RGBA && out_format != PANO_PIX_RGB_PLANAR)
+    return SWEEP_MISUSE(s, "blend sweep: output format %#x", out_format);
+  s->finished = true;
+  if (int rc = sweep_wait_previous(s)) return rc;
+  int r[4] = {0, 0, s->ow, s->oh};
+  if (s->scan)
+    if (int rc = pano_crop_scan_rect(s->scan.get(), r)) return sweep_fail(s, rc);
+  if (int rc = ctx_put(ctx, s->d_rect, r, sizeof(r))) return sweep_fail(s, rc);
+  if (int rc = pano_rgb8_crop_to_pix8_dev(ctx, s->d_rgb, s->ow, s->oh, s->d_rect, out_format, d_out))
+    return sweep_fail(s, rc);
+  for (int q = 0; q < 4; ++q) rect[q] = r[q];
+  return PANO_OK;
+}
+
+int pano_blend_sweep_stats(const pano_blend_sweep* s, long long* uploads, unsigned long long* upload_bytes,
+                           unsigned long long* retained_high) {
+  if (!s) return PANO_ERR_INVALID;
+  if (uploads) *uploads = s->uploads;
+  if (upload_bytes) *upload_bytes = s->upload_bytes;
+  if (retained_high) *retained_high = s->retained_high;
+  return PANO_OK;
+}
+
+void pano_blend_sweep_free(pano_blend_sweep* s) {
+  if (s) ctx_enter(s->ctx);
+  delete s;
+}
+
+}  // extern "C"

@@ -8,6 +8,9 @@
 //   B200PixelBlender::write_strips
 //                     blend + crop + write_rgb of main.cc:226-234 one strip of canvas rows at a time: no f32
 //                     mosaic of the whole canvas, on the host or the device
+//   B200PixelBlender::write_sweep
+//                     the same from one blend sweep: each source is decoded and uploaded once while later strips
+//                     read it (within a byte budget), files decoded on demand
 //   b200_planet       planet() of main.cc:294-331 from load_pixels' buffer, left on the device for write_mosaic
 // The buffers go to B200SIFTDetector::detect_batch_rgb8, B200PixelBlender or the streams (pano_b200.h) with
 // their format as the `channels` argument; no Mat32f of a source is built.  Include after the reference's
@@ -102,7 +105,22 @@ class B200PixelBlender {
     memcpy(b.homo_inv, homo_inv.data, sizeof(double) * 9);
     imgs_.push_back(b);
     px_.push_back(&px);
+    files_.emplace_back();
   }
+  // An image that write_sweep decodes from `fname` (load_pixels) whenever a strip asks for it; w×h is its shape.
+  // run() and write_strips take add_image's images only.
+  void add_file(const Coor& upper_left, const Coor& bottom_right, const std::string& fname, int w, int h,
+                const pano::Homography& homo_inv) {
+    pano_blend_image b;
+    b.rgb_hwc = nullptr; b.w = w; b.h = h;
+    b.x0 = upper_left.x; b.y0 = upper_left.y; b.x1 = bottom_right.x; b.y1 = bottom_right.y;
+    memcpy(b.homo_inv, homo_inv.data, sizeof(double) * 9);
+    imgs_.push_back(b);
+    px_.push_back(nullptr);
+    files_.push_back(fname);
+  }
+  // load_pixels calls write_sweep made so far
+  long decodes() const { return decodes_; }
   Mat32f run() {
     const int n = (int)imgs_.size();
     int ow = 0, oh = 0;
@@ -185,12 +203,73 @@ class B200PixelBlender {
     for (void* d : {d_strip, d_rgb8, d_out, d_rect}) c_.check(pano_dev_free(c_.get(), d));
     encode_mosaic(fname, buf, rect[2], rect[3]);
   }
+
+  // write_strips' file from one blend sweep (pano_blend_sweep_*): the strips of `rows` canvas rows run top to
+  // bottom, and a source read by several strips stays on the device from the first to the last, as far as
+  // keep_bytes (bytes of sources kept between strips; SIZE_MAX: no limit) allows.  A file image is decoded once for
+  // each upload the sweep's plan asks for and released after that strip; add_image's buffers are handed over as
+  // they are.  Device memory: pano_blend_sweep_create's bound (pano_b200.h) and the encoder's layout of the canvas.
+  // The file is write_rgb's, byte for byte, for canvases up to 80,000 columns wide when `crop`.
+  void write_sweep(int rows, size_t keep_bytes, bool crop, const char* fname) {
+    const int n = (int)imgs_.size();
+    int ow = 0, oh = 0;
+    c_.check(pano_blend_target_size(n, imgs_.data(), &ow, &oh));
+    const bool png = endswith(fname, ".png");
+    pano_params p = snapshot_params();
+    std::vector<size_t> bytes(n);
+    for (int k = 0; k < n; ++k)   // a file's bytes before it is decoded: RGBA for a .png, else 3 planes (grey: 1)
+      bytes[k] = px_[k] ? px_[k]->data.size()
+                        : (size_t)imgs_[k].w * imgs_[k].h * (endswith(files_[k].c_str(), ".png") ? 4 : 3);
+    pano_blend_sweep* s = nullptr;
+    c_.check(pano_blend_sweep_create(c_.get(), n, imgs_.data(), &g_, bands_, &p, ow, oh, std::max(rows, 1),
+                                     bytes.data(), keep_bytes, crop ? 1 : 0, &s));
+    std::vector<unsigned char> want(n);
+    std::vector<const void*> src(n);
+    std::vector<int> fmt(n);
+    std::vector<Pixels> loaded(n);
+    int st = 0;
+    while ((st = pano_blend_sweep_next(s, want.data())) >= 0) {
+      for (int k = 0; k < n; ++k) {
+        src[k] = nullptr; fmt[k] = PANO_PIX_RGB;
+        if (!want[k]) continue;
+        const Pixels* px = px_[k];
+        if (!px) {
+          loaded[k] = load_pixels(files_[k].c_str());
+          ++decodes_;
+          m_assert(loaded[k].w == imgs_[k].w && loaded[k].h == imgs_[k].h);
+          px = &loaded[k];
+        }
+        src[k] = px->ptr(); fmt[k] = px->format;
+      }
+      c_.check(pano_blend_sweep_strip(s, src.data(), fmt.data(), PANO_SRC_RGB8_HOST));
+      for (Pixels& px : loaded) px = Pixels();       // pageable: staged by the call
+    }
+    if (st < -1) c_.check(st);
+    void* d_out = nullptr;
+    int rect[4] = {0, 0, ow, oh};
+    c_.check(pano_dev_alloc(c_.get(), (size_t)ow * oh * (png ? 4 : 3), &d_out));
+    c_.check(pano_blend_sweep_finish_dev(s, png ? PANO_PIX_RGBA : PANO_PIX_RGB_PLANAR, (unsigned char*)d_out, rect));
+    std::vector<unsigned char> buf((size_t)rect[2] * rect[3] * (png ? 4 : 3));
+    if (!buf.empty()) c_.check(pano_dev_download(c_.get(), buf.data(), d_out, buf.size()));
+    c_.check(pano_dev_free(c_.get(), d_out));
+    long long uploads = 0;
+    c_.check(pano_blend_sweep_stats(s, &uploads, nullptr, nullptr));
+    last_sweep_uploads_ = uploads;
+    pano_blend_sweep_free(s);
+    encode_mosaic(fname, buf, rect[2], rect[3]);
+  }
+  // the hand-overs of the last write_sweep (pano_blend_sweep_stats)
+  long long last_sweep_uploads() const { return last_sweep_uploads_; }
+
  private:
   const Context& c_;
   int bands_, window_;
   pano_blend_geom g_;
   std::vector<pano_blend_image> imgs_;
   std::vector<const Pixels*> px_;
+  std::vector<std::string> files_;   // add_file's images (empty for add_image's)
+  long decodes_ = 0;
+  long long last_sweep_uploads_ = 0;
 };
 
 // main.cc:226-234 on a device mosaic (h×w×3 f32, Color::NO < 0): crop() when `crop`, then write_rgb(fname).

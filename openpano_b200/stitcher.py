@@ -17,7 +17,8 @@ from __future__ import annotations
 import numpy as np
 
 from ._abi import default_params
-from .capi import PIX_FORMATS, PIX_RGB, PIX_RGBA, PIX_RGB_PLANAR, Engine, pix_format
+from .capi import (PIX_FORMATS, PIX_RGB, PIX_RGBA, PIX_RGB_PLANAR, SRC_F32_HOST, SRC_RGB8_DEV, SRC_RGB8_HOST, Engine,
+                   pix_format)
 
 
 from .synth import all_pairs, ordered_pairs  # noqa: F401  (task lists live with the workload generator)
@@ -388,6 +389,61 @@ def mosaic_rgb8_strips(engine: Engine, items, geom, bands, sources, strip_rows, 
         for d in (d_strip, d_rgb, d_out, d_rect):
             engine.dev_free(d)
     return rect, (px.reshape(3, ch, cw) if code == PIX_RGB_PLANAR else px.reshape(ch, cw, bpp))
+
+
+_PIX_BYTES = {1: 1, 3: 3, PIX_RGBA: 4, PIX_RGB_PLANAR: 3}
+
+
+def mosaic_rgb8_sweep(engine: Engine, items, geom, bands, sources, strip_rows, keep_bytes, out_format="rgb", crop=True,
+                      params=None, kind=None, formats=None, shapes=None, fmt=None, stats=None):
+    """mosaic_rgb8_strips' bytes from one blend sweep (Engine.blend_sweep): the strips run top to bottom and each
+    source is handed over once while a later strip still reads it, keeping at most keep_bytes of sources between
+    strips (capi.SIZE_MAX: no limit; 0 hands over every source each strip reads).
+
+    sources: numpy arrays (host, pageable: uint8 read in layout `fmt`, one value or one per image, or float32
+    H×W×3), or pointers of source kind `kind` with PANO_PIX_* codes `formats` (one per image; None: 3) and `shapes`
+    [(h, w)].  Device memory holds one strip's blend state and f32 rows, two sources in the upload ring, the kept
+    sources, and 3 + 3 (4 for "rgba") bytes per canvas pixel.  stats: a dict that receives
+    "uploads", "upload_bytes" and "retained_high" (pano_blend_sweep_stats).  Returns (rect or None, pixels) as
+    mosaic_rgb8_strips does."""
+    n = len(items)
+    if kind is None:
+        arrs = [np.ascontiguousarray(a) for a in sources]
+        u8 = arrs[0].dtype == np.uint8
+        if u8:
+            info = [pix_format(a, f) for a, f in zip(arrs, fmt if isinstance(fmt, (list, tuple)) else [fmt] * n)]
+            formats, shapes = [c for c, _, _ in info], [(h, w) for _, h, w in info]
+        else:
+            formats, shapes = [3] * n, [a.shape[:2] for a in arrs]
+        kind = SRC_RGB8_HOST if u8 else SRC_F32_HOST
+        ptrs, nbytes = [a.ctypes.data for a in arrs], [a.nbytes for a in arrs]
+    else:
+        u8 = kind in (SRC_RGB8_DEV, SRC_RGB8_HOST)
+        formats = list(formats) if formats is not None else [3] * n
+        ptrs = list(sources)
+        nbytes = [h * w * (_PIX_BYTES[f] if u8 else 12) for (h, w), f in zip(shapes, formats)]
+    ow, oh = max(it[2] for it in items), max(it[3] for it in items)
+    code = PIX_FORMATS[out_format]
+    bpp = 4 if code == PIX_RGBA else 3
+    sweep = engine.blend_sweep(shapes, items, geom, strip_rows, keep_bytes, bands, params, crop, nbytes)
+    d_out = engine.dev_alloc(max(ow * oh * bpp, 256))
+    try:
+        while True:
+            st, want = sweep.next()
+            if st < 0:
+                break
+            sweep.strip([q if w else 0 for q, w in zip(ptrs, want)], formats, kind)
+        rect = sweep.finish_dev(code, d_out)
+        cw, ch = int(rect[2]), int(rect[3])
+        px = np.empty(cw * ch * bpp, np.uint8)
+        if px.size:
+            engine.dev_download(px, d_out)
+        if stats is not None:
+            stats["uploads"], stats["upload_bytes"], stats["retained_high"] = sweep.stats()
+    finally:
+        sweep.close()
+        engine.dev_free(d_out)
+    return (rect if crop else None), (px.reshape(3, ch, cw) if code == PIX_RGB_PLANAR else px.reshape(ch, cw, bpp))
 
 
 class StitchLanes:
