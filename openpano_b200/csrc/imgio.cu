@@ -356,6 +356,8 @@ __global__ void __launch_bounds__(256) k_crop_final(const CropLineBest* __restri
 // ------------------------------------------------------------------ f32 -> u8
 // (v < 0 ? 1 : v) * 255 truncated to unsigned char (imgio.cc:107-109): Color::NO
 // turns white.  One thread per output pixel of the (cropped) rectangle.
+// The conversion is x86-64's: the float goes to int (f2i_x86), whose low byte is the sample.  A mosaic the caller
+// hands in may hold anything: products in [256, 2^31) keep their low byte, and products >= 2^31, +inf and NaN give 0.
 __global__ void __launch_bounds__(256) k_f32_to_rgb8(const float* __restrict__ mat, int w, int h,
                                                      const int* __restrict__ rect, unsigned char* __restrict__ out) {
   int x0 = 0, y0 = 0, cw = w, ch = h;
@@ -369,8 +371,7 @@ __global__ void __launch_bounds__(256) k_f32_to_rgb8(const float* __restrict__ m
     for (int q = 0; q < 3; ++q) {
       float v = p[q];
       v = (v < 0 ? 1.0f : v) * 255.0f;
-      // C's float -> unsigned char conversion truncates; values are in [0, 255]
-      o[q] = (unsigned char)(int)v;
+      o[q] = (unsigned char)f2i_x86(v);
     }
   }
 }
@@ -392,7 +393,7 @@ __global__ void __launch_bounds__(256) k_f32_to_pix8(const float* __restrict__ m
     for (int q = 0; q < 3; ++q) {
       float v = p[q];
       v = (v < 0 ? 1.0f : v) * 255.0f;
-      o[q] = (unsigned char)(int)v;
+      o[q] = (unsigned char)f2i_x86(v);
     }
     if (FMT == PANO_PIX_RGBA) {
       unsigned char* d = out + i * 4;
