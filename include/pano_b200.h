@@ -517,6 +517,21 @@ void pano_blend_stream_free(pano_blend_stream* s);
 int  pano_blend_stream_create_rows(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g,
                                    int bands, const pano_params* p, int out_w, int out_h, int row0, int row1,
                                    pano_blend_stream** out);
+/* A blend stream over cylinder mode's warped images that takes the UNWARPED sources: CylinderStitcher::build's
+ * `warper.warp(*imgs[k].img, ...)` (cylstitcher.cc:65-67) and blend of the warped images (:24-27) in one, with
+ * LAZY_READ's windows.  imgs[k].w / imgs[k].h are the warped shape and must equal pano_cyl_warp_shape(src_w[k],
+ * src_h[k], h_factor, p), else PANO_ERR_INVALID; ranges and homo_inv are those of the warped images.  Each add
+ * passes image k's source of src_w[k]×src_h[k] (every kind and PANO_PIX_* format of pano_blend_stream_add);
+ * add, finish and free are pano_blend_stream's.  The mosaic is pano_blend_dev's over the images
+ * pano_cyl_warp_batch_dev / pano_cyl_warp_batch_rgb8_dev warp from the same sources, bit for bit, for every
+ * window partition, linear and multiband: each blend tap computes the warped pixels it reads from the source, with
+ * the warp's own operations, so no warped image is ever stored.
+ * Device memory: the canvas state and the two windows of (unwarped) sources of pano_blend_stream_create, plus
+ * 16 B per warped column per image (the warp's column tables) and a 72 B entry per image.  Keypoints are not
+ * touched: pano_cyl_warp_shape's offsets warp them on the host. */
+int  pano_blend_stream_create_cyl(pano_ctx* ctx, int n, const pano_blend_image* imgs, const int* src_w,
+                                  const int* src_h, double h_factor, const pano_blend_geom* g, int bands,
+                                  const pano_params* p, int out_w, int out_h, pano_blend_stream** out);
 /* flags[k] (k < n) = 1 if the stream reads image k, else 0.  bands > 0: the images whose ROI, clipped to
  * [row0 - H, row1 + H) on a strip with rows above or below it, keeps a row; bands == 0: the images whose
  * rows [y0, y1] meet [row0, row1).  A stream of the whole canvas needs every image. */

@@ -113,6 +113,8 @@ def _load():
                                                     C.POINTER(PanoBlendGeom), C.c_int, P, C.c_int, C.c_int, C.c_int,
                                                     C.c_int, _vpp]),
         "pano_blend_stream_needs": (C.c_int, [C.c_void_p, C.c_void_p]),
+        "pano_blend_stream_create_cyl": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), _ip, _ip, C.c_double,
+                                                   C.POINTER(PanoBlendGeom), C.c_int, P, C.c_int, C.c_int, _vpp]),
         "pano_blend_sweep_plan": (C.c_int, [C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom), C.c_int, P,
                                             C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t), C.c_size_t, _ip,
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong),
@@ -1086,6 +1088,29 @@ class Engine:
         self._check(LIB.pano_blend_stream_create_rows(self._h, len(items), arr, C.byref(g), bands, C.byref(params),
                                                       ow.value, oh.value, row0, row1, C.byref(h)))
         return BlendStream(self, h, shapes, ow.value, oh.value, (row0, row1))
+
+    def blend_stream_cyl(self, src_shapes, items, geom, h_factor, bands=0, params=None) -> BlendStream:
+        """blend_stream over cylinder mode's warped images, fed the UNWARPED sources: src_shapes are the sources'
+        (h, w), items / geom those of the warped images (each of cyl_warp_shape's size).  add() takes the sources;
+        finish() gives blend_dev's mosaic of the images cyl_warp_batch_dev warps from them."""
+        params = params or default_params()
+        n = len(items)
+        shapes = []
+        for h, w in src_shapes:
+            try:
+                ow, oh, _, _ = self.cyl_warp_shape(w, h, h_factor, params)
+            except PanoError:
+                ow, oh = 0, 0
+            shapes.append((oh, ow))
+        arr, g = self._blend_args([None] * n, shapes, items, geom)
+        ow, oh = C.c_int(), C.c_int()
+        self._check(LIB.pano_blend_target_size(n, arr, C.byref(ow), C.byref(oh)))
+        sw = (C.c_int * max(n, 1))(*[int(s[1]) for s in src_shapes])
+        sh = (C.c_int * max(n, 1))(*[int(s[0]) for s in src_shapes])
+        h = C.c_void_p()
+        self._check(LIB.pano_blend_stream_create_cyl(self._h, n, arr, sw, sh, h_factor, C.byref(g), bands,
+                                                     C.byref(params), ow.value, oh.value, C.byref(h)))
+        return BlendStream(self, h, src_shapes, ow.value, oh.value)
 
     def blend_sweep(self, shapes, items, geom, strip_rows, keep_bytes, bands=0, params=None, crop=True,
                     src_bytes=None) -> BlendSweep:

@@ -22,6 +22,7 @@ struct BlendImg {
   union {
     const float* rgb;           // device, h×w×3 f32 (SrcF32)
     const unsigned char* pix;   // device, 8-bit pixels in format `channels` (SrcRgb8 / SrcPix8)
+    const CylImg* cyl;          // device, the image's cylinder warp (SrcCyl: pano_blend_stream_create_cyl)
   };
   int w, h;
   int x0, y0, x1, y1;
@@ -44,6 +45,24 @@ template <> __device__ __forceinline__ SrcRgb8 blend_src<SrcRgb8>(const BlendImg
 template <> __device__ __forceinline__ SrcPix8 blend_src<SrcPix8>(const BlendImg& im, const float* lut) {
   return SrcPix8{im.pix, lut, im.channels, (size_t)im.w * im.h};
 }
+template <>
+__device__ __forceinline__ SrcCyl<SrcF32> blend_src<SrcCyl<SrcF32>>(const BlendImg& im, const float* lut) {
+  return SrcCyl<SrcF32>::of(im.cyl, lut);
+}
+template <>
+__device__ __forceinline__ SrcCyl<SrcRgb8> blend_src<SrcCyl<SrcRgb8>>(const BlendImg& im, const float* lut) {
+  return SrcCyl<SrcRgb8>::of(im.cyl, lut);
+}
+template <>
+__device__ __forceinline__ SrcCyl<SrcPix8> blend_src<SrcCyl<SrcPix8>>(const BlendImg& im, const float* lut) {
+  return SrcCyl<SrcPix8>::of(im.cyl, lut);
+}
+
+// The profile-name suffix of a tap source's kernels: "", "_rgb8", "_pix8", and "_cyl" before them for SrcCyl
+template <class Src> struct SrcTag {
+  static constexpr int v = std::is_same<Src, SrcPix8>::value ? 2 : Src::kLut ? 1 : 0;
+};
+template <class Inner> struct SrcTag<SrcCyl<Inner>> { static constexpr int v = 3 + SrcTag<Inner>::v; };
 
 struct BlendGeom {
   int projection;
@@ -761,6 +780,10 @@ struct pano_blend_stream {
   std::vector<int> slot;       // per image: its entry of job.imgs, or -1 if the rows do not need it
   DevBuf<float> d_sum;         // linear: tw×rows×3 Σ c·w
   DevBuf<float> d_wsum;        // linear: tw×rows Σ w
+  // cylinder streams (pano_blend_stream_create_cyl), else empty: sources are unwarped and read through SrcCyl
+  std::vector<CylImg> cyl;     // per entry of job.imgs: the warp's constants and its tables in d_cyl_tab
+  DevBuf<CylImg> d_cyl;        // per entry, with its source pointer: written by the add of its window
+  DevBuf<double> d_cyl_tab;    // col_x then col_cos of every image, 16 B per warped column
   int added = 0, err = 0;
   bool finished = false;
   UploadRing ring;
@@ -775,24 +798,17 @@ static int stream_fail(pano_blend_stream* s, int rc) { s->err = rc; return rc; }
     if (_e != cudaSuccess) return stream_fail((s), ctx_cuda((s)->ctx, _e, #call)); \
   } while (0)
 
-// Uploads host window `win` (count images from srcs) into the ring; points win[] at it.
-static int stream_upload(pano_blend_stream* s, int count, const void* const* srcs, bool u8, int channels,
-                         BlendImg* win, int* slot_out) {
-  std::vector<size_t> bytes(count);
-  std::vector<const void*> d_src(count);
-  for (int k = 0; k < count; ++k)
-    bytes[k] = (size_t)win[k].w * win[k].h * (u8 ? (size_t)pix8_bytes(channels) : 3 * sizeof(float));
-  if (int rc = s->ring.upload(s->ctx, count, srcs, bytes.data(), d_src.data(), slot_out)) return stream_fail(s, rc);
-  for (int k = 0; k < count; ++k) win[k].pix = (const unsigned char*)d_src[k];
-  return PANO_OK;
-}
-
 template <class Src>
 static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const BlendImg* win, int count) {
   pano_ctx* ctx = s->ctx;
   const BlendJob& job = s->job;
   const dim3 b(32, 8);
-  constexpr bool pix8 = std::is_same<Src, SrcPix8>::value;
+  static const char* const acc_name[6] = {"k_linear_accumulate", "k_linear_accumulate_rgb8", "k_linear_accumulate_pix8",
+                                          "k_linear_accumulate_cyl", "k_linear_accumulate_cyl_rgb8",
+                                          "k_linear_accumulate_cyl_pix8"};
+  static const char* const first_name[6] = {"k_mb_first_level", "k_mb_first_level_rgb8", "k_mb_first_level_pix8",
+                                            "k_mb_first_level_cyl", "k_mb_first_level_cyl_rgb8",
+                                            "k_mb_first_level_cyl_pix8"};
   if (s->bands == 0) {
     // bounding rectangle of the window on the canvas (inclusive ranges: a superset of both range rules)
     int x0 = INT_MAX, y0 = INT_MAX, x1 = 0, y1 = 0;
@@ -803,15 +819,14 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
     x1 = std::min(x1, job.tw); y0 = std::max(y0, s->row0); y1 = std::min(y1, s->row1);
     if (x0 >= x1 || y0 >= y1) return PANO_OK;
     dim3 g(ceil_div(x1 - x0, 32), ceil_div(y1 - y0, 8));
-    PANO_LAUNCH(ctx, pix8 ? "k_linear_accumulate_pix8" : Src::kLut ? "k_linear_accumulate_rgb8" : "k_linear_accumulate",
-                k_linear_accumulate<Src>, g, b, 0, d_win, count, job.g, s->lazy, s->ordered, s->d_sum, s->d_wsum, job.tw,
-                s->row0, x0, y0, x1, y1);
+    PANO_LAUNCH(ctx, acc_name[SrcTag<Src>::v], k_linear_accumulate<Src>, g, b, 0, d_win, count, job.g, s->lazy,
+                s->ordered, s->d_sum, s->d_wsum, job.tw, s->row0, x0, y0, x1, y1);
   } else {
     int rw = 0, rh = 0;
     for (int k = 0; k < count; ++k) { rw = std::max(rw, win[k].rw); rh = std::max(rh, win[k].rh); }
     dim3 g(ceil_div(rw, 32), ceil_div(rh, 8), count);
-    PANO_LAUNCH(ctx, pix8 ? "k_mb_first_level_pix8" : Src::kLut ? "k_mb_first_level_rgb8" : "k_mb_first_level",
-                k_mb_first_level<Src>, g, b, 0, d_win, job.g, s->dev.d_cur, s->dev.d_mask);
+    PANO_LAUNCH(ctx, first_name[SrcTag<Src>::v], k_mb_first_level<Src>, g, b, 0, d_win, job.g, s->dev.d_cur,
+                s->dev.d_mask);
   }
   return PANO_OK;
 }
@@ -930,6 +945,55 @@ int pano_blend_stream_create_rows(pano_ctx* ctx, int n, const pano_blend_image* 
   return blend_stream_open(ctx, n, imgs, g, bands, p, ow, oh, row0, row1, nullptr, out);
 }
 
+int pano_blend_stream_create_cyl(pano_ctx* ctx, int n, const pano_blend_image* imgs, const int* src_w,
+                                 const int* src_h, double h_factor, const pano_blend_geom* g, int bands,
+                                 const pano_params* p, int ow, int oh, pano_blend_stream** out) {
+  ctx_enter(ctx);
+  if (!ctx || !out) return PANO_ERR_INVALID;
+  *out = nullptr;
+  if (n <= 0 || !imgs || !src_w || !src_h || !p)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder blend stream: bad argument");
+  if (n > PANO_MAX_IMAGES)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: %d images (limit %d)", n, PANO_MAX_IMAGES);
+  // the warp of every source (host arithmetic, as pano_cyl_warp_batch_dev does it) must be the image blended
+  std::vector<CylMap> maps(n);
+  std::vector<size_t> tab_off(n);
+  std::vector<double> tabs;
+  for (int k = 0; k < n; ++k) {
+    if (src_w[k] < 2 || src_h[k] < 2)
+      return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder blend stream: source %d is %dx%d, under 2x2", k, src_w[k],
+                      src_h[k]);
+    tab_off[k] = tabs.size();
+    if (!cyl_map(src_w[k], src_h[k], h_factor, p, nullptr, 0, &maps[k], &tabs))
+      return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder radius <= 0");
+    if (maps[k].ow != imgs[k].w || maps[k].oh != imgs[k].h)
+      return ctx_fail(ctx, PANO_ERR_INVALID,
+                      "cylinder blend stream: image %d is %dx%d but its %dx%d source warps to %dx%d", k, imgs[k].w,
+                      imgs[k].h, src_w[k], src_h[k], maps[k].ow, maps[k].oh);
+  }
+  pano_blend_stream* raw = nullptr;
+  if (int rc = blend_stream_open(ctx, n, imgs, g, bands, p, ow, oh, 0, oh, nullptr, &raw)) return rc;
+  std::unique_ptr<pano_blend_stream> s(raw);
+  const size_t ne = s->job.imgs.size();
+  int rc = 0;
+  if ((rc = s->d_cyl_tab.alloc(ctx, std::max<size_t>(tabs.size(), 1))) ||
+      (rc = s->d_cyl.alloc(ctx, std::max<size_t>(ne, 1))))
+    return rc;
+  if ((rc = ctx_put(ctx, s->d_cyl_tab, tabs.data(), tabs.size() * sizeof(double)))) return rc;
+  s->cyl.resize(ne);
+  for (size_t q = 0; q < ne; ++q) {
+    const int k = s->job.src[q];
+    CylImg& c = s->cyl[q];
+    memset(&c, 0, sizeof(c));
+    c.w = src_w[k]; c.h = src_h[k];
+    c.col_x = s->d_cyl_tab + tab_off[k];
+    c.col_cos = c.col_x + maps[k].ow;
+    c.r = maps[k].r; c.cy = maps[k].cy; c.offy = maps[k].offy; c.sizefactor_inv = maps[k].sizefactor_inv;
+  }
+  *out = s.release();
+  return PANO_OK;
+}
+
 int pano_blend_stream_needs(const pano_blend_stream* s, unsigned char* flags) {
   if (!s) return PANO_ERR_INVALID;
   ctx_enter(s->ctx);
@@ -956,8 +1020,13 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
     return STREAM_MISUSE(s, "blend stream: format %#x for source kind %d", channels, kind);
   // The window's needed images.  Their table rows go to d_imgs from the first one's entry on: for multiband
   // they are exactly the consecutive entries mb_levels reads again; linear reads them in this window only.
+  // A cylinder stream's entries point at their warp entries in d_cyl, and those at the sources.
+  const bool cyl = !s->cyl.empty();
+  const size_t px_bytes = u8 ? (size_t)pix8_bytes(channels) : 3 * sizeof(float);
   std::vector<BlendImg> win;
+  std::vector<CylImg> cwin;
   std::vector<const void*> wsrc;
+  std::vector<size_t> bytes;
   int j0 = -1;
   for (int k = 0; k < count; ++k) {
     const int q = s->slot[first + k];
@@ -966,8 +1035,15 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
       if (int rc = pix8_check(ctx, "blend stream", first + k, channels, srcs[k])) return stream_fail(s, rc);
     if (j0 < 0) j0 = q;
     win.push_back(s->job.imgs[q]);
-    win.back().pix = (const unsigned char*)srcs[k];
     win.back().channels = u8 ? channels : 3;
+    if (cyl) {
+      cwin.push_back(s->cyl[q]);
+      cwin.back().channels = u8 ? channels : 3;
+      win.back().cyl = s->d_cyl + q;
+      bytes.push_back((size_t)cwin.back().w * cwin.back().h * px_bytes);
+    } else {
+      bytes.push_back((size_t)win.back().w * win.back().h * px_bytes);
+    }
     wsrc.push_back(srcs[k]);
   }
   const int nw = (int)win.size();
@@ -980,12 +1056,24 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
     cudaError_t e = s->ring.init();
     if (e != cudaSuccess) return stream_fail(s, ctx_cuda(ctx, e, "blend stream: copy stream / events"));
   }
-  if (host && (rc = stream_upload(s, nw, wsrc.data(), u8, channels, win.data(), &slot))) return rc;
+  std::vector<const void*> d_src(wsrc);   // host sources: their copies in the ring
+  if (host && (rc = s->ring.upload(ctx, nw, wsrc.data(), bytes.data(), d_src.data(), &slot))) return stream_fail(s, rc);
+  for (int k = 0; k < nw; ++k) (cyl ? cwin[k].pix : win[k].pix) = (const unsigned char*)d_src[k];
   BlendImg* d_win = s->dev.d_imgs + j0;
-  if ((rc = ctx_put(ctx, d_win, win.data(), nw * sizeof(BlendImg)))) return stream_fail(s, rc);
-  rc = !u8 ? stream_launch<SrcF32>(s, d_win, win.data(), nw)
-     : pix8_layout(channels) ? stream_launch<SrcPix8>(s, d_win, win.data(), nw)
-                             : stream_launch<SrcRgb8>(s, d_win, win.data(), nw);
+  if (cyl) {
+    void* dsts[2] = {d_win, s->d_cyl + j0};
+    const void* hsrcs[2] = {win.data(), cwin.data()};
+    size_t sizes[2] = {nw * sizeof(BlendImg), nw * sizeof(CylImg)};
+    if ((rc = ctx_put_many(ctx, 2, dsts, hsrcs, sizes))) return stream_fail(s, rc);
+    rc = !u8 ? stream_launch<SrcCyl<SrcF32>>(s, d_win, win.data(), nw)
+       : pix8_layout(channels) ? stream_launch<SrcCyl<SrcPix8>>(s, d_win, win.data(), nw)
+                               : stream_launch<SrcCyl<SrcRgb8>>(s, d_win, win.data(), nw);
+  } else {
+    if ((rc = ctx_put(ctx, d_win, win.data(), nw * sizeof(BlendImg)))) return stream_fail(s, rc);
+    rc = !u8 ? stream_launch<SrcF32>(s, d_win, win.data(), nw)
+       : pix8_layout(channels) ? stream_launch<SrcPix8>(s, d_win, win.data(), nw)
+                               : stream_launch<SrcRgb8>(s, d_win, win.data(), nw);
+  }
   if (rc) return stream_fail(s, rc);
   if (slot >= 0) STREAM_CUDA(s, s->ring.release(ctx, slot));
   s->added += count;

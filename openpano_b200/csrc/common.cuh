@@ -298,6 +298,14 @@ static inline bool pix8_layout(int fmt) { return fmt == PANO_PIX_RGBA || fmt == 
 // needs; fails the context with `what` in the message.
 int pix8_check(pano_ctx* ctx, const char* what, int i, int fmt, const void* d_pix);
 
+// The inverse map of CylinderWarper(h_factor).warp on a w×h image (warp.cu; host arithmetic): the warped shape
+// ow×oh, the constants, and the per-column tables col_x[ow] then col_cos[ow] appended to *tabs when the shape is
+// not empty.  kpts (nk image-centred pairs) are rewritten in place as warp() rewrites them.  False for a
+// cylinder radius <= 0.
+struct CylMap { int ow, oh; double r, cy, offy, sizefactor_inv; };
+bool cyl_map(int w, int h, double h_factor, const pano_params* p, double* kpts, int nk, CylMap* m,
+             std::vector<double>* tabs);
+
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 // gridDim.y for `count` items (at least 1 block).  CUDA refuses a grid.y above 65,535, so kernels whose
 // y index is an input count (pairs, sides, segments) loop: item = blockIdx.y; item < count; item += gridDim.y.
@@ -547,5 +555,64 @@ __device__ __forceinline__ bool interpolate_rgb(const float* __restrict__ img, i
                                                 float* o0, float* o1, float* o2) {
   return interpolate_rgb(SrcF32{img}, w, h, r, c, o0, o1, o2);
 }
+
+// One pixel (i, j) of CylinderWarper::warp's image (stitch/warp.cc:33-41) from the w×h source that src() returns
+// (a tap source, made only where a tap is read): col_x / col_cos are the warp's per-column tables (warp.cu), -1
+// (Color::NO) where the inverse map leaves the source.  The one statement of the warp's float and double
+// operations: the stored warp (k_cyl_warp_batch) and the warp read at blend time (SrcCyl) both call it, so the two
+// give the same bits.
+template <class MakeSrc>
+__device__ __forceinline__ void cyl_warp_px(MakeSrc src, int w, int h, const double* col_x, const double* col_cos,
+                                            double r, double cy, double offy, double sizefactor_inv, int i, int j,
+                                            float* o0, float* o1, float* o2) {
+  double py = ((double)i - offy) * sizefactor_inv;
+  double x = col_x[j];
+  double y = py * r / col_cos[j] + cy;
+  float v0 = -1.f, v1 = -1.f, v2 = -1.f;
+  if (x >= 0 && x <= (double)(w - 1) && y >= 0 && y <= (double)(h - 1)) {
+    float c0, c1, c2;
+    if (interpolate_rgb(src(), w, h, (float)y, (float)x, &c0, &c1, &c2)) { v0 = c0; v1 = c1; v2 = c2; }
+  }
+  *o0 = v0; *o1 = v1; *o2 = v2;
+}
+
+// One image's cylinder warp as a blend reads it (pano_blend_stream_create_cyl): the unwarped source and the
+// constants and device tables of its inverse map.
+struct CylImg {
+  union {
+    const float* rgb;           // h×w×3 f32 (SrcF32)
+    const unsigned char* pix;   // 8-bit pixels in format `channels` (SrcRgb8 / SrcPix8)
+  };
+  int w, h;                     // the source's shape
+  int channels;
+  const double* col_x;          // [warped width] each
+  const double* col_cos;
+  double r, cy, offy, sizefactor_inv;
+};
+
+// The warped image of a CylImg as a tap source: each of the four taps is the pixel k_cyl_warp_batch would have
+// stored there, computed from the source through Inner when the blend asks for it, so no warped image is ever
+// held.  Unmapped pixels are Color::NO, as in the stored image.
+template <class Inner>
+struct SrcCyl {
+  using inner_type = Inner;
+  Inner src;
+  const CylImg* c;
+  static constexpr bool kMayBeNo = true, kLut = Inner::kLut;
+  static __device__ __forceinline__ SrcCyl of(const CylImg* c, const float* lut) {
+    if constexpr (std::is_same<Inner, SrcF32>::value) return SrcCyl{SrcF32{c->rgb}, c};
+    else if constexpr (std::is_same<Inner, SrcRgb8>::value) return SrcCyl{SrcRgb8{c->pix, lut, c->channels}, c};
+    else return SrcCyl{SrcPix8{c->pix, lut, c->channels, (size_t)c->w * c->h}, c};
+  }
+  __device__ __forceinline__ void fetch(int, int fr, int fc, float* q) const {
+    const int w = c->w, h = c->h;
+    const double r = c->r, cy = c->cy, offy = c->offy, sfi = c->sizefactor_inv;
+    const auto src = [this] { return this->src; };
+    cyl_warp_px(src, w, h, c->col_x, c->col_cos, r, cy, offy, sfi, fr, fc, q, q + 1, q + 2);
+    cyl_warp_px(src, w, h, c->col_x, c->col_cos, r, cy, offy, sfi, fr, fc + 1, q + 3, q + 4, q + 5);
+    cyl_warp_px(src, w, h, c->col_x, c->col_cos, r, cy, offy, sfi, fr + 1, fc, q + 6, q + 7, q + 8);
+    cyl_warp_px(src, w, h, c->col_x, c->col_cos, r, cy, offy, sfi, fr + 1, fc + 1, q + 9, q + 10, q + 11);
+  }
+};
 
 #endif  // __CUDACC__

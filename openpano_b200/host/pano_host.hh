@@ -309,6 +309,67 @@ class B200LazyBlender : public pano::BlenderBase {
   std::vector<pano::ImageRef*> refs_;
 };
 
+// ---- cylinder mode's warp and blend in one (cylstitcher.cc:24-27, 65-67): CylinderWarper(h_factor).warp of every
+// image followed by the flat-projection blend of ConnectedImages::blend, from the UNWARPED images.  run() loads
+// them `window` at a time into a cylinder blend stream (pano_blend_stream_create_cyl) and releases them before
+// the next window; no warped image is made, on the host or the device.  add_image takes the unwarped ImageRef
+// (loaded once before, for its shape) and the range and homo_inv of its warped image; the mosaic is that of
+// LinearBlender / MultiBandBlender over the warped images, bit for bit.
+class B200CylinderBlender : public pano::BlenderBase {
+ public:
+  B200CylinderBlender(const Context& c, int bands, real_t h_factor, Vec2D resolution, Vec2D proj_min, int window = 1)
+      : c_(c), bands_(bands), window_(window < 1 ? 1 : window), h_factor_(h_factor) {
+    g_.projection = PANO_PROJ_FLAT; g_.res_x = resolution.x; g_.res_y = resolution.y;
+    g_.proj_min_x = proj_min.x; g_.proj_min_y = proj_min.y;
+  }
+  void add_image(const Coor& upper_left, const Coor& bottom_right, pano::ImageRef& img, const pano::Homography& homo_inv) {
+    pano_params p = snapshot_params();
+    pano_blend_image b;
+    double ox, oy;
+    c_.check(pano_cyl_warp_shape(img.width(), img.height(), h_factor_, &p, &b.w, &b.h, &ox, &oy));
+    b.rgb_hwc = nullptr;
+    b.x0 = upper_left.x; b.y0 = upper_left.y; b.x1 = bottom_right.x; b.y1 = bottom_right.y;
+    memcpy(b.homo_inv, homo_inv.data, sizeof(double) * 9);
+    imgs_.push_back(b);
+    src_w_.push_back(img.width()); src_h_.push_back(img.height());
+    refs_.push_back(&img);
+  }
+  void add_image(const Coor&, const Coor&, pano::ImageRef&, std::function<Vec2D(Coor)>) override {
+    error_exit("B200CylinderBlender: pass the homography (add_image(ul, br, img, homo_inv)), a closure cannot cross the C ABI");
+  }
+  Mat32f run() override {
+    const int n = (int)imgs_.size();
+    int ow = 0, oh = 0;
+    c_.check(pano_blend_target_size(n, imgs_.data(), &ow, &oh));
+    pano_params p = snapshot_params();
+    pano_blend_stream* s = nullptr;
+    c_.check(pano_blend_stream_create_cyl(c_.get(), n, imgs_.data(), src_w_.data(), src_h_.data(), h_factor_, &g_,
+                                          bands_, &p, ow, oh, &s));
+    for (int k0 = 0; k0 < n; k0 += window_) {
+      const int k1 = std::min(n, k0 + window_);
+      std::vector<const void*> src;
+      for (int k = k0; k < k1; ++k) {
+        refs_[k]->load();
+        src.push_back(refs_[k]->img->ptr());
+      }
+      c_.check(pano_blend_stream_add(s, k0, k1 - k0, src.data(), PANO_SRC_F32_HOST, 3));   // pageable: staged
+      for (int k = k0; k < k1; ++k) refs_[k]->release();
+    }
+    Mat32f out(oh, ow, 3);
+    c_.check(pano_blend_stream_finish(s, out.ptr()));
+    pano_blend_stream_free(s);
+    return out;
+  }
+ private:
+  const Context& c_;
+  int bands_, window_;
+  real_t h_factor_;
+  pano_blend_geom g_;
+  std::vector<pano_blend_image> imgs_;
+  std::vector<int> src_w_, src_h_;
+  std::vector<pano::ImageRef*> refs_;
+};
+
 // ---- cylinder warp: CylinderWarper(h_factor).warp(mat, kpts) (warp.hh:41-66)
 class B200CylinderWarper {
  public:
