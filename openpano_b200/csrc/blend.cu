@@ -19,11 +19,8 @@
 #include <memory>
 
 struct BlendImg {
-  union {
-    const float* rgb;           // device, h×w×3 f32 (SrcF32)
-    const unsigned char* pix;   // device, 8-bit pixels in format `channels` (SrcRgb8 / SrcPix8)
-    const CylImg* cyl;          // device, the image's cylinder warp (SrcCyl: pano_blend_stream_create_cyl)
-  };
+  const void* src;        // device: h×w×3 f32 (SrcF32), 8-bit pixels in format `channels` (SrcRgb8 / SrcPix8),
+                          // or the image's cylinder warp, a CylImg (SrcCyl: pano_blend_stream_create_cyl)
   int w, h;
   int x0, y0, x1, y1;
   double hi[9];
@@ -36,33 +33,6 @@ struct BlendImg {
   int rw, rh, pitch;
   int channels;           // 8-bit sources only: the PANO_PIX_* format
 };
-
-template <class Src> __device__ __forceinline__ Src blend_src(const BlendImg& im, const float* lut);
-template <> __device__ __forceinline__ SrcF32 blend_src<SrcF32>(const BlendImg& im, const float*) { return SrcF32{im.rgb}; }
-template <> __device__ __forceinline__ SrcRgb8 blend_src<SrcRgb8>(const BlendImg& im, const float* lut) {
-  return SrcRgb8{im.pix, lut, im.channels};
-}
-template <> __device__ __forceinline__ SrcPix8 blend_src<SrcPix8>(const BlendImg& im, const float* lut) {
-  return SrcPix8{im.pix, lut, im.channels, (size_t)im.w * im.h};
-}
-template <>
-__device__ __forceinline__ SrcCyl<SrcF32> blend_src<SrcCyl<SrcF32>>(const BlendImg& im, const float* lut) {
-  return SrcCyl<SrcF32>::of(im.cyl, lut);
-}
-template <>
-__device__ __forceinline__ SrcCyl<SrcRgb8> blend_src<SrcCyl<SrcRgb8>>(const BlendImg& im, const float* lut) {
-  return SrcCyl<SrcRgb8>::of(im.cyl, lut);
-}
-template <>
-__device__ __forceinline__ SrcCyl<SrcPix8> blend_src<SrcCyl<SrcPix8>>(const BlendImg& im, const float* lut) {
-  return SrcCyl<SrcPix8>::of(im.cyl, lut);
-}
-
-// The profile-name suffix of a tap source's kernels: "", "_rgb8", "_pix8", and "_cyl" before them for SrcCyl
-template <class Src> struct SrcTag {
-  static constexpr int v = std::is_same<Src, SrcPix8>::value ? 2 : Src::kLut ? 1 : 0;
-};
-template <class Inner> struct SrcTag<SrcCyl<Inner>> { static constexpr int v = 3 + SrcTag<Inner>::v; };
 
 struct BlendGeom {
   int projection;
@@ -143,7 +113,7 @@ __device__ __forceinline__ void linear_add_px(const BlendImg* __restrict__ imgs,
     if (x < 0 || x >= im.w || y < 0 || y >= im.h) continue;       // map_coor -> NaN
     float r = (float)y, c = (float)x;
     float c0, c1, c2;
-    if (!interpolate_rgb(blend_src<Src>(im, lut), im.w, im.h, r, c, &c0, &c1, &c2)) continue;
+    if (!interpolate_rgb(Src::at(im.src, im.w, im.h, im.channels, lut), im.w, im.h, r, c, &c0, &c1, &c2)) continue;
     if (c0 < 0) continue;
     float w = (float)(0.5 - fabs((double)(c / (float)im.w) - 0.5));
     if (!ordered) w = (float)((double)w * (0.5 - fabs((double)(r / (float)im.h) - 0.5)));
@@ -235,7 +205,8 @@ __global__ void k_mb_first_level(const BlendImg* __restrict__ imgs, BlendGeom g,
   double x, y;
   coor_func(im, g, j + im.x0, i + im.y0, &x, &y);
   float c0, c1, c2;
-  bool ok = interpolate_rgb(blend_src<Src>(im, lut), im.w, im.h, (float)y, (float)x, &c0, &c1, &c2);
+  bool ok = interpolate_rgb(Src::at(im.src, im.w, im.h, im.channels, lut), im.w, im.h, (float)y, (float)x, &c0, &c1,
+                            &c2);
   if (ok && fminf(c0, fminf(c1, c2)) < 0) ok = false;
   const size_t o = (size_t)i * im.pitch + j;
   float* p = cur + im.roi_off + o;
@@ -566,8 +537,8 @@ static int blend_plan(pano_ctx* ctx, int n, const pano_blend_image* imgs, const 
     job->tw = std::max(job->tw, s.x1); job->th = std::max(job->th, s.y1);
     BlendImg d;
     memset(&d, 0, sizeof(d));
-    d.rgb = s.rgb_hwc; d.w = s.w; d.h = s.h;
-    if (pix) d.pix = pix[k];
+    d.src = pix ? (const void*)pix[k] : s.rgb_hwc;
+    d.w = s.w; d.h = s.h;
     d.x0 = s.x0; d.x1 = s.x1;
     d.y0 = std::max(s.y0, job->clip0); d.y1 = std::min(s.y1, job->clip1);
     if (d.y0 > d.y1) continue;                         // no row of this image reaches the strip
@@ -724,16 +695,15 @@ static int blend_run(pano_ctx* ctx, const BlendJob& job, BlendDev* d, int bands,
                      int row0, int row1) {
   const int n = (int)job.imgs.size(), tw = job.tw;
   const dim3 b(32, 8);   // 256 threads: the 8-bit kernels' conversion table
-  constexpr bool pix8 = std::is_same<Src, SrcPix8>::value;
   if (bands == 0) {
     dim3 gs(ceil_div(tw, 32), ceil_div(row1 - row0, 8));
-    PANO_LAUNCH(ctx, pix8 ? "k_linear_blend_pix8" : Src::kLut ? "k_linear_blend_rgb8" : "k_linear_blend",
-                k_linear_blend<Src>, gs, b, 0, d->d_imgs, n, job.g, p->lazy_read, p->ordered_input, d_out, tw, row0, row1);
+    PANO_LAUNCH(ctx, src_name<Src>(SRC_NAMES("k_linear_blend")), k_linear_blend<Src>, gs, b, 0, d->d_imgs, n, job.g,
+                p->lazy_read, p->ordered_input, d_out, tw, row0, row1);
     return PANO_OK;
   }
   dim3 gr(ceil_div(job.max_rw, 32), ceil_div(job.max_rh, 8), n);
-  PANO_LAUNCH(ctx, pix8 ? "k_mb_first_level_pix8" : Src::kLut ? "k_mb_first_level_rgb8" : "k_mb_first_level",
-              k_mb_first_level<Src>, gr, b, 0, d->d_imgs, job.g, d->d_cur, d->d_mask);
+  PANO_LAUNCH(ctx, src_name<Src>(SRC_NAMES("k_mb_first_level")), k_mb_first_level<Src>, gr, b, 0, d->d_imgs, job.g,
+              d->d_cur, d->d_mask);
   return mb_levels(ctx, job, d, bands, d_out, row0, row1);
 }
 
@@ -758,10 +728,9 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
   }
   BlendDev dev;
   if ((rc = blend_dev_setup(ctx, &job, bands, row0, row1, &dev))) return rc;
-  if (pix && std::any_of(channels, channels + n, pix8_layout))
-    return blend_run<SrcPix8>(ctx, job, &dev, bands, p, d_out, row0, row1);
-  return pix ? blend_run<SrcRgb8>(ctx, job, &dev, bands, p, d_out, row0, row1)
-             : blend_run<SrcF32>(ctx, job, &dev, bands, p, d_out, row0, row1);
+  return with_reader(src_reader(pix ? channels : nullptr, n), [&](auto tag) {
+    return blend_run<typename decltype(tag)::type>(ctx, job, &dev, bands, p, d_out, row0, row1);
+  });
 }
 
 // ------------------------------------------------------------------ blend stream
@@ -803,12 +772,6 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
   pano_ctx* ctx = s->ctx;
   const BlendJob& job = s->job;
   const dim3 b(32, 8);
-  static const char* const acc_name[6] = {"k_linear_accumulate", "k_linear_accumulate_rgb8", "k_linear_accumulate_pix8",
-                                          "k_linear_accumulate_cyl", "k_linear_accumulate_cyl_rgb8",
-                                          "k_linear_accumulate_cyl_pix8"};
-  static const char* const first_name[6] = {"k_mb_first_level", "k_mb_first_level_rgb8", "k_mb_first_level_pix8",
-                                            "k_mb_first_level_cyl", "k_mb_first_level_cyl_rgb8",
-                                            "k_mb_first_level_cyl_pix8"};
   if (s->bands == 0) {
     // bounding rectangle of the window on the canvas (inclusive ranges: a superset of both range rules)
     int x0 = INT_MAX, y0 = INT_MAX, x1 = 0, y1 = 0;
@@ -819,14 +782,14 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
     x1 = std::min(x1, job.tw); y0 = std::max(y0, s->row0); y1 = std::min(y1, s->row1);
     if (x0 >= x1 || y0 >= y1) return PANO_OK;
     dim3 g(ceil_div(x1 - x0, 32), ceil_div(y1 - y0, 8));
-    PANO_LAUNCH(ctx, acc_name[SrcTag<Src>::v], k_linear_accumulate<Src>, g, b, 0, d_win, count, job.g, s->lazy,
-                s->ordered, s->d_sum, s->d_wsum, job.tw, s->row0, x0, y0, x1, y1);
+    PANO_LAUNCH(ctx, src_name<Src>(SRC_NAMES("k_linear_accumulate")), k_linear_accumulate<Src>, g, b, 0, d_win, count,
+                job.g, s->lazy, s->ordered, s->d_sum, s->d_wsum, job.tw, s->row0, x0, y0, x1, y1);
   } else {
     int rw = 0, rh = 0;
     for (int k = 0; k < count; ++k) { rw = std::max(rw, win[k].rw); rh = std::max(rh, win[k].rh); }
     dim3 g(ceil_div(rw, 32), ceil_div(rh, 8), count);
-    PANO_LAUNCH(ctx, first_name[SrcTag<Src>::v], k_mb_first_level<Src>, g, b, 0, d_win, job.g, s->dev.d_cur,
-                s->dev.d_mask);
+    PANO_LAUNCH(ctx, src_name<Src>(SRC_NAMES("k_mb_first_level")), k_mb_first_level<Src>, g, b, 0, d_win, job.g,
+                s->dev.d_cur, s->dev.d_mask);
   }
   return PANO_OK;
 }
@@ -1013,16 +976,15 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
   if (!srcs) return STREAM_MISUSE(s, "blend stream: null source list");
   for (int k = 0; k < count; ++k)
     if (!srcs[k] && s->slot[first + k] >= 0) return STREAM_MISUSE(s, "blend stream: image %d has no source", first + k);
-  const bool u8 = kind == PANO_SRC_RGB8_DEV || kind == PANO_SRC_RGB8_HOST;
-  const bool host = kind == PANO_SRC_F32_HOST || kind == PANO_SRC_RGB8_HOST;
-  if (!u8 && kind != PANO_SRC_F32_DEV && kind != PANO_SRC_F32_HOST) return STREAM_MISUSE(s, "blend stream: unknown source kind %d", kind);
-  if (u8 ? !pix8_bytes(channels) : channels != 3)
-    return STREAM_MISUSE(s, "blend stream: format %#x for source kind %d", channels, kind);
+  SrcKind sk;
+  if (int rc = src_kind(ctx, "blend stream", kind, &sk)) return stream_fail(s, rc);
+  for (int k = 0; k < count; ++k)   // the alignment of the needed images only
+    if (int rc = src_check(ctx, "blend stream", sk, first + k, channels, s->slot[first + k] >= 0 ? srcs[k] : nullptr))
+      return stream_fail(s, rc);
   // The window's needed images.  Their table rows go to d_imgs from the first one's entry on: for multiband
   // they are exactly the consecutive entries mb_levels reads again; linear reads them in this window only.
   // A cylinder stream's entries point at their warp entries in d_cyl, and those at the sources.
   const bool cyl = !s->cyl.empty();
-  const size_t px_bytes = u8 ? (size_t)pix8_bytes(channels) : 3 * sizeof(float);
   std::vector<BlendImg> win;
   std::vector<CylImg> cwin;
   std::vector<const void*> wsrc;
@@ -1031,18 +993,16 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
   for (int k = 0; k < count; ++k) {
     const int q = s->slot[first + k];
     if (q < 0) continue;
-    if (kind == PANO_SRC_RGB8_DEV && channels == PANO_PIX_RGBA)
-      if (int rc = pix8_check(ctx, "blend stream", first + k, channels, srcs[k])) return stream_fail(s, rc);
     if (j0 < 0) j0 = q;
     win.push_back(s->job.imgs[q]);
-    win.back().channels = u8 ? channels : 3;
+    win.back().channels = channels;
     if (cyl) {
       cwin.push_back(s->cyl[q]);
-      cwin.back().channels = u8 ? channels : 3;
-      win.back().cyl = s->d_cyl + q;
-      bytes.push_back((size_t)cwin.back().w * cwin.back().h * px_bytes);
+      cwin.back().channels = channels;
+      win.back().src = s->d_cyl + q;
+      bytes.push_back(src_bytes(cwin.back().w, cwin.back().h, sk.u8, channels));
     } else {
-      bytes.push_back((size_t)win.back().w * win.back().h * px_bytes);
+      bytes.push_back(src_bytes(win.back().w, win.back().h, sk.u8, channels));
     }
     wsrc.push_back(srcs[k]);
   }
@@ -1052,28 +1012,26 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
     return PANO_OK;
   }
   int slot = -1, rc = 0;
-  if (host && !s->ring.copy) {      // the copy stream and events of the first host window
+  if (sk.host && !s->ring.copy) {      // the copy stream and events of the first host window
     cudaError_t e = s->ring.init();
     if (e != cudaSuccess) return stream_fail(s, ctx_cuda(ctx, e, "blend stream: copy stream / events"));
   }
   std::vector<const void*> d_src(wsrc);   // host sources: their copies in the ring
-  if (host && (rc = s->ring.upload(ctx, nw, wsrc.data(), bytes.data(), d_src.data(), &slot))) return stream_fail(s, rc);
-  for (int k = 0; k < nw; ++k) (cyl ? cwin[k].pix : win[k].pix) = (const unsigned char*)d_src[k];
+  if (sk.host && (rc = s->ring.upload(ctx, nw, wsrc.data(), bytes.data(), d_src.data(), &slot))) return stream_fail(s, rc);
+  for (int k = 0; k < nw; ++k) (cyl ? cwin[k].src : win[k].src) = d_src[k];
   BlendImg* d_win = s->dev.d_imgs + j0;
   if (cyl) {
     void* dsts[2] = {d_win, s->d_cyl + j0};
     const void* hsrcs[2] = {win.data(), cwin.data()};
     size_t sizes[2] = {nw * sizeof(BlendImg), nw * sizeof(CylImg)};
     if ((rc = ctx_put_many(ctx, 2, dsts, hsrcs, sizes))) return stream_fail(s, rc);
-    rc = !u8 ? stream_launch<SrcCyl<SrcF32>>(s, d_win, win.data(), nw)
-       : pix8_layout(channels) ? stream_launch<SrcCyl<SrcPix8>>(s, d_win, win.data(), nw)
-                               : stream_launch<SrcCyl<SrcRgb8>>(s, d_win, win.data(), nw);
   } else {
     if ((rc = ctx_put(ctx, d_win, win.data(), nw * sizeof(BlendImg)))) return stream_fail(s, rc);
-    rc = !u8 ? stream_launch<SrcF32>(s, d_win, win.data(), nw)
-       : pix8_layout(channels) ? stream_launch<SrcPix8>(s, d_win, win.data(), nw)
-                               : stream_launch<SrcRgb8>(s, d_win, win.data(), nw);
   }
+  rc = with_reader(src_reader(sk.u8 ? &channels : nullptr, 1), [&](auto tag) {
+    using Src = typename decltype(tag)::type;
+    return cyl ? stream_launch<SrcCyl<Src>>(s, d_win, win.data(), nw) : stream_launch<Src>(s, d_win, win.data(), nw);
+  });
   if (rc) return stream_fail(s, rc);
   if (slot >= 0) STREAM_CUDA(s, s->ring.release(ctx, slot));
   s->added += count;

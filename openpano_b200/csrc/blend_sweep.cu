@@ -275,9 +275,9 @@ int pano_blend_sweep_strip(pano_blend_sweep* s, const void* const* srcs, const i
   if (s->err) return s->err;
   if (s->finished || s->done >= s->plan.strips) return SWEEP_MISUSE(s, "blend sweep: strip after the last");
   if (!srcs) return SWEEP_MISUSE(s, "blend sweep: null source list");
-  const bool u8 = kind == PANO_SRC_RGB8_DEV || kind == PANO_SRC_RGB8_HOST;
-  const bool host = kind == PANO_SRC_F32_HOST || kind == PANO_SRC_RGB8_HOST;
-  if (!u8 && kind != PANO_SRC_F32_DEV && kind != PANO_SRC_F32_HOST) return SWEEP_MISUSE(s, "blend sweep: unknown source kind %d", kind);
+  SrcKind sk;
+  if (int rc = src_kind(ctx, "blend sweep", kind, &sk)) return sweep_fail(s, rc);
+  const bool u8 = sk.u8;
   if (u8 && !formats) return SWEEP_MISUSE(s, "blend sweep: null format list");
   const int n = s->n, st = s->done;
   const unsigned char* up = &s->plan.uploads[(size_t)st * n];
@@ -289,16 +289,14 @@ int pano_blend_sweep_strip(pano_blend_sweep* s, const void* const* srcs, const i
     if (srcs[k] && !up[k]) return SWEEP_MISUSE(s, "blend sweep: strip %d was not to be given image %d", st, k);
     if (!srcs[k]) continue;
     fmt[k] = u8 ? formats[k] : 3;
-    if (u8 && !pix8_bytes(fmt[k])) return SWEEP_MISUSE(s, "blend sweep: image %d: format %#x", k, fmt[k]);
-    if (u8 && !host)
-      if (int rc = pix8_check(ctx, "blend sweep", k, fmt[k], srcs[k])) return sweep_fail(s, rc);
-    sz[k] = (size_t)s->imgs[k].w * s->imgs[k].h * (u8 ? (size_t)pix8_bytes(fmt[k]) : 3 * sizeof(float));
+    if (int rc = src_check(ctx, "blend sweep", sk, k, fmt[k], srcs[k])) return sweep_fail(s, rc);
+    sz[k] = src_bytes(s->imgs[k].w, s->imgs[k].h, u8, fmt[k]);
     if (sz[k] > s->bytes[k])
       return SWEEP_MISUSE(s, "blend sweep: image %d takes %zu bytes, planned with %zu", k, sz[k], s->bytes[k]);
     list.push_back(k);
   }
   if (int rc = sweep_wait_previous(s)) return rc;
-  if (int rc = sweep_blend(s, st, srcs, u8, host, fmt, sz)) return sweep_fail(s, rc);
+  if (int rc = sweep_blend(s, st, srcs, u8, sk.host, fmt, sz)) return sweep_fail(s, rc);
   const int row0 = st * s->rows, row1 = std::min(s->oh, row0 + s->rows);
   if (s->scan)
     if (int rc = pano_crop_scan_add_dev(s->scan.get(), s->d_strip, row1 - row0)) return sweep_fail(s, rc);

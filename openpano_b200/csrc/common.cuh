@@ -14,6 +14,7 @@
 #include <stdint.h>
 #include <string>
 #include <vector>
+#include <algorithm>
 #include <map>
 #include <memory>
 #include <type_traits>
@@ -292,11 +293,23 @@ static inline int pix8_bytes(int fmt) {
     default: return 0;
   }
 }
-// RGBA and planar images are read through SrcPix8; grey and interleaved RGB through SrcRgb8
+// RGBA and planar images are read through SrcPix8; grey and interleaved RGB through SrcRgb8 (src_reader)
 static inline bool pix8_layout(int fmt) { return fmt == PANO_PIX_RGBA || fmt == PANO_PIX_RGB_PLANAR; }
 // Checks image i's format and, for device sources (d_pix non-null), the 4-byte alignment an RGBA tap load
 // needs; fails the context with `what` in the message.
 int pix8_check(pano_ctx* ctx, const char* what, int i, int fmt, const void* d_pix);
+
+// A PANO_SRC_* kind: u8, 8-bit pixels in a PANO_PIX_* format (else h×w×3 f32); host, in host memory (else device).
+struct SrcKind { int kind; bool u8, host; };
+// Decodes `kind`; fails the context with `what` in the message for an unknown kind.
+int src_kind(pano_ctx* ctx, const char* what, int kind, SrcKind* out);
+// Bytes of a w×h source (fmt: its PANO_PIX_* format when u8)
+static inline size_t src_bytes(int w, int h, bool u8, int fmt) {
+  return (size_t)w * h * (u8 ? (size_t)pix8_bytes(fmt) : 3 * sizeof(float));
+}
+// Checks image i of a source argument: its format (a PANO_PIX_* format for 8-bit sources, 3 for f32 ones) and, for
+// a device source px (null: not checked), pix8_check's alignment; fails the context with `what` in the message.
+int src_check(pano_ctx* ctx, const char* what, const SrcKind& k, int i, int fmt, const void* px);
 
 // The inverse map of CylinderWarper(h_factor).warp on a w×h image (warp.cu; host arithmetic): the warped shape
 // ow×oh, the constants, and the per-column tables col_x[ow] then col_cos[ow] appended to *tabs when the shape is
@@ -445,12 +458,18 @@ __device__ __forceinline__ void mag_ort_at(const float* __restrict__ img, int w,
   *ort = (float)((double)fast_atan(dy, dx) + PANO_PI);
 }
 
-// Sources of the interpolate_rgb gather.  Each fetches the two horizontally adjacent pixels
-// (fr, fc), (fr, fc + 1) and the two below them as 12 floats: q[0..5] row fr, q[6..11] row fr + 1.
+// Sources of the interpolate_rgb gather (tap readers, DESIGN.md §9).  at(px, w, h, fmt, lut) is the reader of one
+// w×h image, its pixels px in format fmt (ignored by SrcF32) and lut the table of build_rgb8_lut (kLut readers).
+// fetch gives the two horizontally adjacent pixels (fr, fc), (fr, fc + 1) and the two below them as 12 floats:
+// q[0..5] row fr, q[6..11] row fr + 1.  kMayBeNo: a tap can be Color::NO; kName: the index into SRC_NAMES.
 // A Mat32f, h×w×3 f32 (Color::NO = negative samples):
 struct SrcF32 {
   const float* img;
   static constexpr bool kMayBeNo = true, kLut = false;
+  static constexpr int kName = 0;
+  static __device__ __forceinline__ SrcF32 at(const void* px, int, int, int, const float*) {
+    return SrcF32{static_cast<const float*>(px)};
+  }
   __device__ __forceinline__ void fetch(int w, int fr, int fc, float* q) const {
     const float* p00 = img + ((size_t)fr * w + fc) * 3;
     const float* p10 = p00 + (size_t)w * 3;
@@ -469,6 +488,10 @@ struct SrcRgb8 {
   const float* lut;
   int channels;
   static constexpr bool kMayBeNo = false, kLut = true;
+  static constexpr int kName = 1;
+  static __device__ __forceinline__ SrcRgb8 at(const void* px, int, int, int fmt, const float* lut) {
+    return SrcRgb8{static_cast<const unsigned char*>(px), lut, fmt};
+  }
   __device__ __forceinline__ void fetch(int w, int fr, int fc, float* q) const {
     if (channels == 1) {
       const unsigned char* p00 = pix + (size_t)fr * w + fc;
@@ -495,6 +518,10 @@ struct SrcPix8 {
   int fmt;
   size_t plane;   // w * h: the planar layout's plane stride
   static constexpr bool kMayBeNo = false, kLut = true;
+  static constexpr int kName = 2;
+  static __device__ __forceinline__ SrcPix8 at(const void* px, int w, int h, int fmt, const float* lut) {
+    return SrcPix8{static_cast<const unsigned char*>(px), lut, fmt, (size_t)w * h};
+  }
   __device__ __forceinline__ void fetch(int w, int fr, int fc, float* q) const {
     if (fmt == PANO_PIX_RGBA) {
       const unsigned* p00 = reinterpret_cast<const unsigned*>(pix) + (size_t)fr * w + fc;
@@ -579,10 +606,7 @@ __device__ __forceinline__ void cyl_warp_px(MakeSrc src, int w, int h, const dou
 // One image's cylinder warp as a blend reads it (pano_blend_stream_create_cyl): the unwarped source and the
 // constants and device tables of its inverse map.
 struct CylImg {
-  union {
-    const float* rgb;           // h×w×3 f32 (SrcF32)
-    const unsigned char* pix;   // 8-bit pixels in format `channels` (SrcRgb8 / SrcPix8)
-  };
+  const void* src;              // h×w×3 f32 or 8-bit pixels in format `channels`, as the stream's reader reads them
   int w, h;                     // the source's shape
   int channels;
   const double* col_x;          // [warped width] each
@@ -599,10 +623,11 @@ struct SrcCyl {
   Inner src;
   const CylImg* c;
   static constexpr bool kMayBeNo = true, kLut = Inner::kLut;
-  static __device__ __forceinline__ SrcCyl of(const CylImg* c, const float* lut) {
-    if constexpr (std::is_same<Inner, SrcF32>::value) return SrcCyl{SrcF32{c->rgb}, c};
-    else if constexpr (std::is_same<Inner, SrcRgb8>::value) return SrcCyl{SrcRgb8{c->pix, lut, c->channels}, c};
-    else return SrcCyl{SrcPix8{c->pix, lut, c->channels, (size_t)c->w * c->h}, c};
+  static constexpr int kName = 3 + Inner::kName;
+  // px: the image's CylImg; the warped image's shape and format are not needed
+  static __device__ __forceinline__ SrcCyl at(const void* px, int, int, int, const float* lut) {
+    const CylImg* c = static_cast<const CylImg*>(px);
+    return SrcCyl{Inner::at(c->src, c->w, c->h, c->channels, lut), c};
   }
   __device__ __forceinline__ void fetch(int, int fr, int fc, float* q) const {
     const int w = c->w, h = c->h;
@@ -614,5 +639,27 @@ struct SrcCyl {
     cyl_warp_px(src, w, h, c->col_x, c->col_cos, r, cy, offy, sfi, fr + 1, fc + 1, q + 9, q + 10, q + 11);
   }
 };
+
+// The profile name of a kernel templated on its reader: SRC_NAMES(base) lists the six names in kName order, and
+// src_name<Src> picks one.  They are literals because the profiler keeps the pointer until it drains.
+#define SRC_NAMES(base) {base, base "_rgb8", base "_pix8", base "_cyl", base "_cyl_rgb8", base "_cyl_pix8"}
+template <class Src> static inline const char* src_name(const char* const (&names)[6]) { return names[Src::kName]; }
+
+// The reader of a set of formats: F32 for f32 sources (fmts null), PIX8 when one of the n formats is RGBA or
+// planar, else RGB8.  with_reader(r, f) calls f(ReaderTag<Src>{}) for r's reader type Src.
+enum class SrcReader { F32, RGB8, PIX8 };
+template <class Src> struct ReaderTag { using type = Src; };
+static inline SrcReader src_reader(const int* fmts, int n) {
+  if (!fmts) return SrcReader::F32;
+  return std::any_of(fmts, fmts + n, pix8_layout) ? SrcReader::PIX8 : SrcReader::RGB8;
+}
+template <class F>
+static inline auto with_reader(SrcReader r, F&& f) {
+  switch (r) {
+    case SrcReader::PIX8: return f(ReaderTag<SrcPix8>{});
+    case SrcReader::RGB8: return f(ReaderTag<SrcRgb8>{});
+    default: return f(ReaderTag<SrcF32>{});
+  }
+}
 
 #endif  // __CUDACC__

@@ -31,6 +31,20 @@ int pix8_check(pano_ctx* ctx, const char* what, int i, int fmt, const void* d_pi
   return PANO_OK;
 }
 
+int src_kind(pano_ctx* ctx, const char* what, int kind, SrcKind* out) {
+  const bool u8 = kind == PANO_SRC_RGB8_DEV || kind == PANO_SRC_RGB8_HOST;
+  if (!u8 && kind != PANO_SRC_F32_DEV && kind != PANO_SRC_F32_HOST)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "%s: unknown source kind %d", what, kind);
+  *out = SrcKind{kind, u8, kind == PANO_SRC_F32_HOST || kind == PANO_SRC_RGB8_HOST};
+  return PANO_OK;
+}
+
+int src_check(pano_ctx* ctx, const char* what, const SrcKind& k, int i, int fmt, const void* px) {
+  if (k.u8 ? !pix8_bytes(fmt) : fmt != 3)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "%s: image %d: format %#x for source kind %d", what, i, fmt, k.kind);
+  return k.u8 ? pix8_check(ctx, what, i, fmt, k.host ? nullptr : px) : PANO_OK;
+}
+
 int ctx_cuda(pano_ctx* ctx, cudaError_t e, const char* what) {
   return ctx_fail(ctx, PANO_ERR_CUDA, "CUDA error %s (%s) at %s", cudaGetErrorName(e), cudaGetErrorString(e), what);
 }
@@ -725,7 +739,7 @@ static int upload_images(pano_ctx* ctx, int n, const void* const* src, const int
   for (int i = 0; i < n; ++i) {
     if (!src[i] || w[i] <= 0 || h[i] <= 0) return ctx_fail(ctx, PANO_ERR_INVALID, "image %d: null or empty", i);
     offs[i] = total;
-    bytes[i] = (size_t)w[i] * h[i] * (channels ? (size_t)pix8_bytes(channels[i]) : 3 * sizeof(float));
+    bytes[i] = src_bytes(w[i], h[i], channels, channels ? channels[i] : 3);
     total += align_up(bytes[i], 256);
   }
   if (int rc = d_block.alloc(ctx, total)) return rc;

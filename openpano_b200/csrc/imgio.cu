@@ -480,12 +480,10 @@ int pano_rgb8_to_mat32f_batch_dev(pano_ctx* ctx, int n, const unsigned char* con
   if (n == 0) return PANO_OK;
   std::vector<Rgb8Job> jobs(n);
   long long max_px = 0;
-  bool layouts = false;   // an RGBA or planar image: k_pix8_to_f32
   for (int i = 0; i < n; ++i) {
     if (w[i] <= 0 || h[i] <= 0 || !d_pix[i] || !d_out_hwc[i])
       return ctx_fail(ctx, PANO_ERR_INVALID, "pano_rgb8_to_mat32f_batch_dev: image %d: w=%d h=%d", i, w[i], h[i]);
     if (int rc = pix8_check(ctx, "pano_rgb8_to_mat32f_batch_dev", i, channels[i], d_pix[i])) return rc;
-    layouts = layouts || pix8_layout(channels[i]);
     if ((reinterpret_cast<uintptr_t>(d_pix[i]) & 3) || (reinterpret_cast<uintptr_t>(d_out_hwc[i]) & 15))
       return ctx_fail(ctx, PANO_ERR_INVALID, "pano_rgb8_to_mat32f_batch_dev: image %d: source must be 4-byte and "
                       "destination 16-byte aligned", i);
@@ -495,6 +493,7 @@ int pano_rgb8_to_mat32f_batch_dev(pano_ctx* ctx, int n, const unsigned char* con
   DevBuf<Rgb8Job> d_jobs;
   if (int rc = d_jobs.alloc(ctx, n)) return rc;
   if (int rc = ctx_put(ctx, d_jobs, jobs.data(), sizeof(Rgb8Job) * n)) return rc;
+  const bool layouts = src_reader(channels, n) == SrcReader::PIX8;   // an RGBA or planar image: k_pix8_to_f32
   long long per_img = ((layouts ? max_px : max_px * 3 / 4) + 255) / 256;
   int gx = (int)std::min<long long>(std::max<long long>(per_img, 1), std::max(1, ctx->num_sms * 8 / n));
   if (layouts) PANO_LAUNCH(ctx, "k_pix8_to_f32", k_pix8_to_f32, dim3(gx, n), 256, 0, d_jobs);

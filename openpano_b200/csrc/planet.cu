@@ -98,8 +98,7 @@ __global__ void k_planet8(const double2* __restrict__ tab, const unsigned char* 
   __shared__ float lut[256];
   build_rgb8_lut(lut, threadIdx.y * blockDim.x + threadIdx.x);   // all 256 threads, before any leaves at the edge
   __syncthreads();
-  if constexpr (std::is_same<Src, SrcPix8>::value) planet_px(tab, SrcPix8{pix, lut, fmt, (size_t)w * h}, w, h, dst);
-  else planet_px(tab, SrcRgb8{pix, lut, fmt}, w, h, dst);
+  planet_px(tab, Src::at(pix, w, h, fmt, lut), w, h, dst);
 }
 
 extern "C" {
@@ -143,11 +142,12 @@ int pano_planet_pix8_dev(pano_ctx* ctx, const unsigned char* d_pix, int format, 
   int rc = planet_table_dev(ctx, &tab);
   if (rc) return rc;
   dim3 b(32, 8), g(ceil_div(kSize, 32), ceil_div(kSize, 8));   // 256 threads: the 8-bit conversion table
-  if (pix8_layout(format))
-    PANO_LAUNCH(ctx, "k_planet_pix8", k_planet8<SrcPix8>, g, b, 0, tab, d_pix, format, w, h, d_out_hwc);
-  else
-    PANO_LAUNCH(ctx, "k_planet_rgb8", k_planet8<SrcRgb8>, g, b, 0, tab, d_pix, format, w, h, d_out_hwc);
-  return PANO_OK;
+  return with_reader(src_reader(&format, 1), [&](auto tag) -> int {
+    using Src = typename decltype(tag)::type;
+    if constexpr (Src::kLut)   // SrcF32 (f32 sources only) has no k_planet8
+      PANO_LAUNCH(ctx, src_name<Src>(SRC_NAMES("k_planet")), k_planet8<Src>, g, b, 0, tab, d_pix, format, w, h, d_out_hwc);
+    return PANO_OK;
+  });
 }
 
 int pano_planet_pix8(pano_ctx* ctx, const unsigned char* pix, int format, int w, int h, float* out_hwc) {

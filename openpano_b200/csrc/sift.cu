@@ -68,15 +68,11 @@ __global__ void __launch_bounds__(PG_THREADS) k_pyramid_grey(const ImgMeta* __re
   if (C0 >= im.w0 || R0 >= im.h0) return;
   const int own_w = min(PG_TW, im.w0 - C0), own_h = min(PG_TH, im.h0 - R0);
   const int last_c = min(PG_TW, im.w0 - 1 - C0), last_r = min(PG_TH, im.h0 - 1 - R0);   // halo included
-  Src src;
   if constexpr (Src::kLut) {
     build_rgb8_lut(lut, threadIdx.x);
     __syncthreads();
-    if constexpr (std::is_same<Src, SrcPix8>::value) src = Src{im.pix, lut, im.channels, (size_t)im.in_w * im.in_h};
-    else src = Src{im.pix, lut, im.channels};
-  } else {
-    src = Src{im.src};
   }
+  const Src src = Src::at(im.src, im.in_w, im.in_h, im.channels, lut);
   const OctMeta& o0 = octs[blockIdx.z * n_oct];
   float* g0 = arena + o0.gauss_off;
   // One working pixel of the staged tile; the column's taps (sy, ry) are the caller's.
@@ -1324,10 +1320,7 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
   const GaussTable& gt = plan->gt;
   const bool fast = plan->fast;
   const size_t seam_cap = plan->seam_cap;
-  for (int i = 0; i < n; ++i) {   // the sources are the one thing a repeat batch changes
-    if (channels) wk->h_img[i].pix = (const unsigned char*)d_src[i];
-    else wk->h_img[i].src = (const float*)d_src[i];
-  }
+  for (int i = 0; i < n; ++i) wk->h_img[i].src = d_src[i];   // the sources are the one thing a repeat batch changes
 
   // featureset outputs (per-image capacity `cap`; compact on download)
   const size_t nlist = (size_t)n * cap;
@@ -1366,12 +1359,13 @@ int sift_run_batch(pano_ctx* ctx, int n, const void* const* d_src, const int* ch
   {
     dim3 g(ceil_div(plan->max_w0, PG_TW), ceil_div(plan->max_h0, PG_TH), n);
     float* work = keep ? wk->arena.get() : nullptr;
-    if (channels && std::any_of(channels, channels + n, pix8_layout))
-      PANO_LAUNCH(ctx, "k_pyramid_grey_pix8", k_pyramid_grey<SrcPix8>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);
-    else if (channels)
-      PANO_LAUNCH(ctx, "k_pyramid_grey_rgb8", k_pyramid_grey<SrcRgb8>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);
-    else
-      PANO_LAUNCH(ctx, "k_pyramid_grey", k_pyramid_grey<SrcF32>, g, PG_THREADS, 0, wk->d_img, wk->d_oct, n_oct, wk->arena, work);
+    if (int rc = with_reader(src_reader(channels, n), [&](auto tag) -> int {
+          using Src = typename decltype(tag)::type;
+          PANO_LAUNCH(ctx, src_name<Src>(SRC_NAMES("k_pyramid_grey")), k_pyramid_grey<Src>, g, PG_THREADS, 0,
+                      wk->d_img, wk->d_oct, n_oct, wk->arena, work);
+          return PANO_OK;
+        }))
+      return rc;
   }
   {
     const ExtremaParams ep{n_scale, p->pre_color_thres, p->judge_extrema_diff_thres, cap, wk->cand_count, wk->cand_keys,

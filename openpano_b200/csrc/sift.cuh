@@ -14,10 +14,7 @@
 #define SIFT_MAX_PEAKS 18        // a peak needs two lower neighbours: <= 36/2
 
 struct ImgMeta {
-  union {
-    const float* src;           // input, h×w×3 f32 (device)
-    const unsigned char* pix;   // input, 8-bit pixels in format `channels` (device), read as SrcRgb8 / SrcPix8 read them
-  };
+  const void* src;    // input (device): h×w×3 f32, or 8-bit pixels in format `channels`
   int in_w, in_h;
   int w0, h0;         // working size
   float ifx, ify;     // 1/fx (rows), 1/fy (cols) of the working resize

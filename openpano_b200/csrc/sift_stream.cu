@@ -116,21 +116,18 @@ int pano_sift_stream_add(pano_sift_stream* s, int first, int count, const void* 
   if (!srcs) return SIFT_STREAM_MISUSE(s, "sift stream: null source list");
   for (int k = 0; k < count; ++k)
     if (!srcs[k]) return SIFT_STREAM_MISUSE(s, "sift stream: image %d has no source", first + k);
-  const bool u8 = kind == PANO_SRC_RGB8_DEV || kind == PANO_SRC_RGB8_HOST;
-  const bool host = kind == PANO_SRC_F32_HOST || kind == PANO_SRC_RGB8_HOST;
-  if (!u8 && kind != PANO_SRC_F32_DEV && kind != PANO_SRC_F32_HOST) return SIFT_STREAM_MISUSE(s, "sift stream: unknown source kind %d", kind);
-  if (u8 ? !pix8_bytes(channels) : channels != 3)
-    return SIFT_STREAM_MISUSE(s, "sift stream: format %#x for source kind %d", channels, kind);
-  if (kind == PANO_SRC_RGB8_DEV && channels == PANO_PIX_RGBA)
-    for (int k = 0; k < count; ++k)
-      if (int rc = pix8_check(ctx, "sift stream", first + k, channels, srcs[k])) return sift_stream_fail(s, rc);
+  SrcKind sk;
+  if (int rc = src_kind(ctx, "sift stream", kind, &sk)) return sift_stream_fail(s, rc);
+  for (int k = 0; k < count; ++k)
+    if (int rc = src_check(ctx, "sift stream", sk, first + k, channels, srcs[k])) return sift_stream_fail(s, rc);
+  const bool u8 = sk.u8;
 
   std::vector<const void*> d_src(srcs, srcs + count);
   int slot = -1;
-  if (host) {   // queued on the copy stream first, so that it runs while the pending window's SIFT does
+  if (sk.host) {   // queued on the copy stream first, so that it runs while the pending window's SIFT does
     std::vector<size_t> bytes(count);
     for (int k = 0; k < count; ++k)
-      bytes[k] = (size_t)s->w[first + k] * s->h[first + k] * (u8 ? (size_t)pix8_bytes(channels) : 3 * sizeof(float));
+      bytes[k] = src_bytes(s->w[first + k], s->h[first + k], u8, channels);
     if (int rc = s->ring.upload(ctx, count, srcs, bytes.data(), d_src.data(), &slot)) return sift_stream_fail(s, rc);
   }
   if (int rc = sift_stream_resolve(s)) return sift_stream_fail(s, rc);

@@ -114,29 +114,16 @@ __global__ void k_cyl_warp(const float* __restrict__ src, int w, int h, float* _
 }
 
 // The same for a batch of device-resident images: blockIdx.z = image; per-image parameters and the
-// two per-column tables (concatenated) sit in device memory.  Src = SrcF32 reads h×w×3 f32 images,
-// Src = SrcRgb8 (SrcPix8 when a batch holds RGBA or planar images) reads 8-bit pixels and converts every
-// tap as read_img converts it, so the warp of the pixels is the warp of read_img's f32 image, bit for bit.
+// two per-column tables (concatenated) sit in device memory.  Src is the batch's reader (src_reader); an 8-bit
+// reader converts every tap as read_img converts it, so the warp of the pixels is the warp of read_img's f32 image.
 struct CylJobDev {
-  union {
-    const float* src;           // SrcF32
-    const unsigned char* pix;   // SrcRgb8 / SrcPix8
-  };
+  const void* src;              // h×w×3 f32 or 8-bit pixels in format `channels`
   float* dst;
   int w, h, ow, oh;
   int channels;                 // 8-bit sources only: the PANO_PIX_* format
   long long tab_off;            // first entry of this image's col_x[ow] followed by col_cos[ow]
   double r, cy, offy, sizefactor_inv;
 };
-
-template <class Src> __device__ __forceinline__ Src cyl_src(const CylJobDev& jb, const float* lut);
-template <> __device__ __forceinline__ SrcF32 cyl_src<SrcF32>(const CylJobDev& jb, const float*) { return SrcF32{jb.src}; }
-template <> __device__ __forceinline__ SrcRgb8 cyl_src<SrcRgb8>(const CylJobDev& jb, const float* lut) {
-  return SrcRgb8{jb.pix, lut, jb.channels};
-}
-template <> __device__ __forceinline__ SrcPix8 cyl_src<SrcPix8>(const CylJobDev& jb, const float* lut) {
-  return SrcPix8{jb.pix, lut, jb.channels, (size_t)jb.w * jb.h};
-}
 
 template <class Src>
 __global__ void k_cyl_warp_batch(const CylJobDev* __restrict__ jobs, const double* __restrict__ tabs) {
@@ -151,7 +138,7 @@ __global__ void k_cyl_warp_batch(const CylJobDev* __restrict__ jobs, const doubl
   if (j >= jb.ow || i >= jb.oh) return;
   const double* col_x = tabs + jb.tab_off;
   float o0, o1, o2;
-  cyl_warp_px([&] { return cyl_src<Src>(jb, lut); }, jb.w, jb.h, col_x, col_x + jb.ow, jb.r, jb.cy, jb.offy,
+  cyl_warp_px([&] { return Src::at(jb.src, jb.w, jb.h, jb.channels, lut); }, jb.w, jb.h, col_x, col_x + jb.ow, jb.r, jb.cy, jb.offy,
               jb.sizefactor_inv, i, j, &o0, &o1, &o2);
   float* p = jb.dst + ((size_t)i * jb.ow + j) * 3;
   p[0] = o0; p[1] = o1; p[2] = o2;
@@ -186,8 +173,8 @@ static int cyl_warp_batch(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double
                       jb.out_w, jb.out_h, sw, sh);
     CylJobDev& d = dj[k];
     memset(&d, 0, sizeof(d));
-    if (pix) { d.pix = pix[k]; d.channels = channels[k]; }
-    else { d.src = jb.d_rgb_hwc; d.channels = 3; }
+    d.src = pix ? (const void*)pix[k] : jb.d_rgb_hwc;
+    d.channels = pix ? channels[k] : 3;
     d.dst = jb.d_out_hwc;
     d.w = jb.w; d.h = jb.h; d.ow = sw; d.oh = sh;
     d.tab_off = (long long)t0;
@@ -201,11 +188,11 @@ static int cyl_warp_batch(pano_ctx* ctx, int n, const pano_cyl_job* jobs, double
   if ((rc = ctx_put(ctx, d_jobs, dj.data(), dj.size() * sizeof(CylJobDev)))) return rc;
   if ((rc = ctx_put(ctx, d_tabs, tabs.data(), tabs.size() * sizeof(double)))) return rc;
   dim3 b(32, 8), g(ceil_div(max_ow, 32), ceil_div(max_oh, 8), n);   // 256 threads: the 8-bit conversion table
-  if (pix && std::any_of(channels, channels + n, pix8_layout))
-    PANO_LAUNCH(ctx, "k_cyl_warp_pix8", k_cyl_warp_batch<SrcPix8>, g, b, 0, d_jobs, d_tabs);
-  else if (pix) PANO_LAUNCH(ctx, "k_cyl_warp_rgb8", k_cyl_warp_batch<SrcRgb8>, g, b, 0, d_jobs, d_tabs);
-  else PANO_LAUNCH(ctx, "k_cyl_warp", k_cyl_warp_batch<SrcF32>, g, b, 0, d_jobs, d_tabs);
-  return PANO_OK;   // stream-ordered: the blocks are released after the kernel
+  return with_reader(src_reader(pix ? channels : nullptr, n), [&](auto tag) -> int {
+    using Src = typename decltype(tag)::type;
+    PANO_LAUNCH(ctx, src_name<Src>(SRC_NAMES("k_cyl_warp")), k_cyl_warp_batch<Src>, g, b, 0, d_jobs, d_tabs);
+    return PANO_OK;   // stream-ordered: the blocks are released after the kernel
+  });
 }
 
 extern "C" {

@@ -314,6 +314,56 @@ def test_blend_stream_profile_names(engine, bands):
         dev.free()
 
 
+@pytest.mark.parametrize("kernel", ["k_linear_blend", "k_mb_first_level", "k_cyl_warp", "k_pyramid_grey"])
+def test_batch_profile_names(engine, kernel):
+    """The same for the batch entries' source-reading kernels (pano_blend_dev / pano_blend_rgb8_dev with 0 and 3
+    bands, the batched cylinder warp, SIFT): one launch per batch, under _pix8 as soon as one image of the batch is
+    RGBA or planar."""
+    bands = 3 if kernel == "k_mb_first_level" else 0
+    p = default_params(multiband=max(bands, 1))
+    rgb, _, items, geom = _stack(2, ["rgb"] * 2)
+    shapes = [x.shape[:2] for x in rgb]
+    ws, hs = [w for _, w in shapes], [h for h, _ in shapes]
+    tw, th = max(it[2] for it in items), max(it[3] for it in items)
+    outs = [engine.cyl_warp_shape(w, h, 1.0, p)[:2] for w, h in zip(ws, hs)]
+    dev = _Dev(engine)
+    try:
+        d_out = dev.alloc(tw * th * 12)
+        d_warp = [dev.alloc(ow * oh * 12) for ow, oh in outs]
+        for fmts, name in ((None, kernel), (["grey"] * 2, kernel + "_rgb8"), (["rgb"] * 2, kernel + "_rgb8"),
+                           (["rgba"] * 2, kernel + "_pix8"), (["planar"] * 2, kernel + "_pix8"),
+                           (["rgb", "rgba"], kernel + "_pix8")):
+            if fmts is None:
+                d_src, codes = [dev.upload(engine.read_img_rgb8(x)) for x in rgb], None
+            else:
+                d_src, codes = [dev.upload(_lay(x, f)) for x, f in zip(rgb, fmts)], [CODE[f] for f in fmts]
+            engine.profile(True)
+            engine.profile_reset()
+            try:
+                fs = None
+                if kernel == "k_cyl_warp":
+                    if codes is None:
+                        engine.cyl_warp_batch_dev(d_src, shapes, d_warp, None, 1.0, p)
+                    else:
+                        engine.cyl_warp_batch_rgb8_dev(d_src, codes, shapes, d_warp, None, 1.0, p)
+                elif kernel == "k_pyramid_grey":
+                    fs = (engine.sift_detect_batch_ptr(d_src, ws, hs, p, device=True) if codes is None
+                          else engine.sift_detect_batch_rgb8_ptr(d_src, ws, hs, codes, p, device=True))
+                elif codes is None:
+                    engine.blend_dev(d_src, shapes, items, geom, d_out, tw, th, bands, p)
+                else:
+                    engine.blend_rgb8_dev(d_src, codes, shapes, items, geom, d_out, tw, th, bands, p)
+                engine.sync()
+                prof = engine.profile_read()
+            finally:
+                engine.profile(False)
+            if fs is not None:
+                fs.free()
+            assert {k: v[0] for k, v in prof.items() if k.startswith(kernel)} == {name: 1}, (fmts, prof)
+    finally:
+        dev.free()
+
+
 # ----------------------------------------------------------------------------- cylinder warp, conversion
 @pytest.mark.parametrize("hf", [1.0, 1.2])
 def test_cyl_warp_layouts_equal_interleaved(engine, hf):
