@@ -47,6 +47,13 @@ typedef enum pano_status {
 #define PANO_MAX_IMAGES 65535
 #define PANO_MAX_SIFT_BATCH 512
 
+/* Handles.  The blend stream, the blend sweep, the SIFT stream and the crop scan keep state between calls and
+ * share one contract.  Calls on a handle are calls on its ctx (same threading rule), and the ctx must outlive it.
+ * A misuse (each handle lists its own) returns PANO_ERR_INVALID, with the reason in pano_last_error, and launches
+ * nothing.  Every failure, a misuse or a CUDA error, is sticky: each later call on the handle returns the same
+ * code again and does nothing.  Its free is valid in any state, free(NULL) is a no-op, and the ctx stays
+ * usable. */
+
 /* Pixel formats of decoded 8-bit images: the per-image `channels` argument of every 8-bit entry point
  * (pano_sift_detect_batch_rgb8[_dev], pano_sift_stream_add and pano_blend_stream_add with the 8-bit kinds,
  * pano_blend_rgb8_dev, pano_blend_rows_rgb8_dev, pano_cyl_warp_batch_rgb8_dev, pano_planet_pix8[_dev],
@@ -468,12 +475,9 @@ int pano_blend_rows_rgb8_dev(pano_ctx* ctx, int n, const pano_blend_image* imgs,
  * sources go through a two-slot device ring, each slot as large as the largest window uploaded
  * through it; device sources are read in place and take no ring memory.
  *
- * Calls on a stream are calls on its ctx (same threading rule); the ctx must outlive it.  A misuse
- * (null pointers, an unknown kind, a value that is no PANO_PIX_* format for 8-bit or other than 3 for f32
- * sources, a device RGBA source that is not 4-byte aligned, out-of-order,
- * overlapping or excess adds, finish before the last image or twice) returns PANO_ERR_INVALID, and
- * every failure is sticky: later adds and finishes return it again.  pano_blend_stream_free is
- * always valid, and the ctx stays usable. */
+ * A stream is a handle (Handles above).  Its misuses: null pointers, an unknown kind, a value that is no
+ * PANO_PIX_* format for 8-bit or other than 3 for f32 sources, a device RGBA source that is not 4-byte aligned,
+ * out-of-order, overlapping or excess adds, finish before the last image or twice. */
 typedef struct pano_blend_stream pano_blend_stream;
 typedef enum pano_src_kind {
   PANO_SRC_F32_DEV = 0,    /* device, h×w×3 f32 (Mat32f layout) */
@@ -575,11 +579,9 @@ int  pano_blend_sweep_plan(int n, const pano_blend_image* imgs, const pano_blend
  *     the bytes of that strip's sources.
  * Device sources are read in place and take none of the last two.
  *
- * Calls on a sweep are calls on its ctx (same threading rule); the ctx must outlive it.  A misuse (null
- * pointers, bad arguments, a source missing where `want` was set or given where it was not, a source larger
- * than its src_bytes, a strip after the last, finish before the last strip or twice) returns
- * PANO_ERR_INVALID, and every failure is sticky.  pano_blend_sweep_free is always valid, and the ctx stays
- * usable. */
+ * A sweep is a handle (Handles above).  Its misuses: null pointers, bad arguments, a source missing where `want`
+ * was set or given where it was not, a source larger than its src_bytes, a strip after the last, finish before
+ * the last strip or twice. */
 typedef struct pano_blend_sweep pano_blend_sweep;
 /* imgs / g / bands / p / out_w / out_h as for pano_blend; strip_rows / src_bytes / keep_bytes as for
  * pano_blend_sweep_plan (src_bytes NULL: w·h·3 per image).  crop != 0: finish_dev crops as crop() does
@@ -627,12 +629,8 @@ void pano_blend_sweep_free(pano_blend_sweep* s);
  * it; device sources are read in place and take no ring memory.  The work buffers stay with the context for
  * the next window of the same shape, as between batches (PANO_CACHE_MB bounds what it keeps).
  *
- * Calls on a stream are calls on its ctx (same threading rule); the ctx must outlive it.  A misuse (null
- * pointers, an unknown kind, a value that is no PANO_PIX_* format for 8-bit or other than 3 for f32 sources, a
- * device RGBA source that is not 4-byte aligned, out-of-order,
- * overlapping or excess adds, more than PANO_MAX_SIFT_BATCH images in one add, finish before the last image
- * or twice) returns PANO_ERR_INVALID, and every failure is sticky: later adds and finishes return it again.
- * pano_sift_stream_free is always valid, and the ctx stays usable. */
+ * A stream is a handle (Handles above).  Its misuses are the blend stream's, and more than PANO_MAX_SIFT_BATCH
+ * images in one add. */
 typedef struct pano_sift_stream pano_sift_stream;
 /* w[i] × h[i]: image i's shape (at least 2×2); p: the SIFT parameters of every window. */
 int  pano_sift_stream_create(pano_ctx* ctx, int n, const int* w, const int* h, const pano_params* p,
@@ -729,8 +727,8 @@ int pano_crop_rect_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h, int*
  * O(w) ints and the best rectangle so far on the device.  add: d_strip_hwc is the next `rows` lines of the
  * w-wide f32 mosaic, read by work queued on the ctx stream.  rect: valid once all h lines have been added;
  * waits for the scan and writes {x0, y0, width, height} to the host array, pano_crop_rect_dev's rectangle for
- * every strip partition.  A misuse (bad sizes, more than h lines, rect before the last line) returns
- * PANO_ERR_INVALID and is sticky, as on a blend stream; pano_crop_scan_free is always valid. */
+ * every strip partition.  A scan is a handle (Handles above).  Its misuses: bad sizes, more than h lines, a null
+ * rect, rect before the last line. */
 typedef struct pano_crop_scan pano_crop_scan;
 int  pano_crop_scan_create(pano_ctx* ctx, int w, int h, pano_crop_scan** out);
 int  pano_crop_scan_add_dev(pano_crop_scan* c, const float* d_strip_hwc, int rows);

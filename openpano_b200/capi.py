@@ -195,8 +195,29 @@ def _i(a):
     return a.ctypes.data_as(_ip)
 
 
-class FeatureSet:
+class _Handle:
+    """Owns one engine handle (self._h, freed by _FREE): close() frees it once, and so does garbage collection, which
+    swallows errors.  _call raises the context's error for a non-zero return code."""
+    _FREE = None
+
+    def _call(self, rc):
+        self.eng._check(rc)
+
+    def close(self):
+        if self._h:
+            type(self)._FREE(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class FeatureSet(_Handle):
     """Device-resident descriptors + coordinates of a batch of images."""
+    _FREE = LIB.pano_featureset_free
 
     def __init__(self, eng, handle):
         self.eng, self._h = eng, handle
@@ -226,19 +247,12 @@ class FeatureSet:
         """Device-to-device copy of image i's rows (coordinates n×2 f64, descriptors n×128 f32)."""
         self.eng._check(LIB.pano_featureset_export_dev(self._h, i, C.c_void_p(d_coor or 0), C.c_void_p(d_desc or 0)))
 
-    def free(self):
-        if self._h:
-            LIB.pano_featureset_free(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.free()
-        except Exception:
-            pass
+    free = _Handle.close
 
 
-class GpuSiftTrace:
+class GpuSiftTrace(_Handle):
+    _FREE = LIB.pano_sift_trace_free
+
     def __init__(self, eng, handle):
         self.eng, self._h = eng, handle
 
@@ -281,22 +295,12 @@ class GpuSiftTrace:
             LIB.pano_sift_trace_descriptors(self._h, n, _d(coor), _f(desc))
         return coor, desc
 
-    def close(self):
-        if self._h:
-            LIB.pano_sift_trace_free(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class BaSession:
+class BaSession(_Handle):
     """Device-resident state of one bundle adjustment (pano_ba_session): the match coordinates, J and the
     residuals of the last error() call.  error() is calcError + update_stats; normal_equations() is
     get_param_update up to the damping, with b = J^T times the residuals of the LAST error() call."""
+    _FREE = LIB.pano_ba_session_free
 
     def __init__(self, eng, handle, n_cam, n_pair, n_match):
         self.eng, self._h = eng, handle
@@ -328,17 +332,6 @@ class BaSession:
         self.eng._check(LIB.pano_ba_normal_equations(self._h, self.n_pair, _d(m) if m.size else None, _d(jtj), _d(b),
                                                      _d(rows) if want_rows else None))
         return jtj, b, (rows[:self.n_match] if want_rows else None)
-
-    def close(self):
-        if self._h:
-            LIB.pano_ba_session_free(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 # pano_src_kind
@@ -377,13 +370,12 @@ def _fmt_list(fmt, n):
     return list(fmt) if isinstance(fmt, (list, tuple)) else [fmt] * n
 
 
-class _SourceStream:
+class _SourceStream(_Handle):
     """What the windowed streams share: add() takes numpy arrays (host; uint8 H×W / H×W×1 / H×W×3 or float32
     H×W×3, the kind from the dtype) or raw pointers with an explicit kind (SRC_*).  Every failure is sticky, as
     in the C ABI."""
     _NAME = ""
     _ADD = None
-    _FREE = None
     _NULL_OK = False     # None in a numpy window: an image the stream does not read (row-strip blend streams)
 
     def __init__(self, eng, handle, shapes):
@@ -447,17 +439,6 @@ class _SourceStream:
         self._call(type(self)._ADD(self._h, self.added, n, arr, kind, channels))
         self.added += n
 
-    def close(self):
-        if self._h:
-            type(self)._FREE(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 class BlendStream(_SourceStream):
     """A pano_blend_stream: the mosaic of pano_blend, fed window by window (LAZY_READ's memory contract).  A stream
@@ -513,17 +494,14 @@ def blend_sweep_plan(shapes, items, geom, bands, strip_rows, src_bytes, keep_byt
             "retained_high": rh.value}
 
 
-class BlendSweep:
+class BlendSweep(_Handle):
     """A pano_blend_sweep: the canvas's row strips top to bottom, each source handed over once while a later strip
     still reads it (within keep_bytes), then the cropped 8-bit mosaic.  next() gives the next strip and the images
     it wants, strip() takes them."""
+    _FREE = LIB.pano_blend_sweep_free
 
     def __init__(self, eng, handle, n, out_w, out_h):
         self.eng, self._h, self.n, self.out_w, self.out_h = eng, handle, n, out_w, out_h
-
-    def _call(self, rc):
-        if rc != 0:
-            self.eng._raise(rc)
 
     def next(self):
         """(strip index or -1, bool array of the images strip() must be given)."""
@@ -552,17 +530,6 @@ class BlendSweep:
         self._call(LIB.pano_blend_sweep_stats(self._h, C.byref(u), C.byref(b), C.byref(r)))
         return u.value, b.value, r.value
 
-    def close(self):
-        if self._h:
-            LIB.pano_blend_sweep_free(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 class SiftStream(_SourceStream):
     """A pano_sift_stream: the featureset of sift_detect_batch (sift_detect_batch_rgb8 for uint8 sources), fed
@@ -577,32 +544,22 @@ class SiftStream(_SourceStream):
         return FeatureSet(self.eng, out)
 
 
-class CropScan:
+class CropScan(_Handle):
     """A pano_crop_scan: crop()'s rectangle of a mosaic that arrives in row strips (widths up to 80,000)."""
+    _FREE = LIB.pano_crop_scan_free
 
     def __init__(self, eng, handle, w, h):
         self.eng, self._h, self.w, self.h = eng, handle, w, h
 
     def add_dev(self, d_strip, rows):
         """The next `rows` lines of the mosaic: a rows×w×3 f32 device buffer."""
-        self.eng._check(LIB.pano_crop_scan_add_dev(self._h, C.c_void_p(d_strip or 0), rows))
+        self._call(LIB.pano_crop_scan_add_dev(self._h, C.c_void_p(d_strip or 0), rows))
 
     def rect(self):
         """{x0, y0, width, height} once every line has been added."""
         r = np.zeros(4, np.int32)
-        self.eng._check(LIB.pano_crop_scan_rect(self._h, _i(r)))
+        self._call(LIB.pano_crop_scan_rect(self._h, _i(r)))
         return r
-
-    def close(self):
-        if self._h:
-            LIB.pano_crop_scan_free(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def _lazy_windows(imgs, window, fmt):

@@ -741,7 +741,7 @@ static int blend_device(pano_ctx* ctx, int n, const pano_blend_image* imgs, cons
 // A stream of rows [row0, row1) keeps the canvas state of those rows only (blend_plan's strip
 // clipping for multiband) and reads only the sources of the images that reach them.
 struct pano_blend_stream {
-  pano_ctx* ctx = nullptr;
+  Sticky st;                   // every failure is sticky: the canvas state is undefined after it
   int n = 0, bands = 0, lazy = 0, ordered = 0;
   int row0 = 0, row1 = 0;
   BlendJob job;
@@ -753,23 +753,13 @@ struct pano_blend_stream {
   std::vector<CylImg> cyl;     // per entry of job.imgs: the warp's constants and its tables in d_cyl_tab
   DevBuf<CylImg> d_cyl;        // per entry, with its source pointer: written by the add of its window
   DevBuf<double> d_cyl_tab;    // col_x then col_cos of every image, 16 B per warped column
-  int added = 0, err = 0;
-  bool finished = false;
+  int added = 0;
   UploadRing ring;
 };
 
-// every failure is sticky: the canvas state is undefined after it
-static int stream_fail(pano_blend_stream* s, int rc) { s->err = rc; return rc; }
-#define STREAM_MISUSE(s, ...) stream_fail((s), ctx_fail((s)->ctx, PANO_ERR_INVALID, __VA_ARGS__))
-#define STREAM_CUDA(s, call)                                               \
-  do {                                                                     \
-    cudaError_t _e = (call);                                               \
-    if (_e != cudaSuccess) return stream_fail((s), ctx_cuda((s)->ctx, _e, #call)); \
-  } while (0)
-
 template <class Src>
 static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const BlendImg* win, int count) {
-  pano_ctx* ctx = s->ctx;
+  pano_ctx* ctx = s->st.ctx;
   const BlendJob& job = s->job;
   const dim3 b(32, 8);
   if (s->bands == 0) {
@@ -795,7 +785,7 @@ static int stream_launch(pano_blend_stream* s, const BlendImg* d_win, const Blen
 }
 
 static int stream_resolve(pano_blend_stream* s, float* d_out) {
-  pano_ctx* ctx = s->ctx;
+  pano_ctx* ctx = s->st.ctx;
   const size_t npx = (size_t)s->job.tw * (s->row1 - s->row0);
   if (s->bands > 0 && s->job.imgs.empty()) {          // no image reaches the rows
     PANO_LAUNCH(ctx, "k_fill", k_fill, (unsigned)((npx * 3 + 255) / 256), 256, 0, d_out, npx * 3, -1.f);
@@ -804,15 +794,6 @@ static int stream_resolve(pano_blend_stream* s, float* d_out) {
   if (s->bands > 0) return mb_levels(ctx, s->job, &s->dev, s->bands, d_out, s->row0, s->row1);
   PANO_LAUNCH(ctx, "k_linear_resolve", k_linear_resolve, (unsigned)((npx + 255) / 256), 256, 0, s->d_sum, s->d_wsum,
               d_out, npx, s->lazy);
-  return PANO_OK;
-}
-
-static int stream_finish_check(pano_blend_stream* s, const void* out) {
-  if (s->err) return s->err;
-  if (!out) return STREAM_MISUSE(s, "blend stream: null output");
-  if (s->finished) return STREAM_MISUSE(s, "blend stream: already finished");
-  if (s->added != s->n) return STREAM_MISUSE(s, "blend stream: finish after %d of %d images", s->added, s->n);
-  s->finished = true;
   return PANO_OK;
 }
 
@@ -827,7 +808,7 @@ int blend_stream_open(pano_ctx* ctx, int n, const pano_blend_image* imgs, const 
   if (row0 < 0 || row1 > oh || row0 >= row1)
     return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: rows [%d, %d) are no strip of the %d-row canvas", row0, row1, oh);
   std::unique_ptr<pano_blend_stream> s(new pano_blend_stream);
-  s->ctx = ctx; s->n = n; s->bands = bands; s->lazy = p->lazy_read; s->ordered = p->ordered_input;
+  s->st.ctx = ctx; s->n = n; s->bands = bands; s->lazy = p->lazy_read; s->ordered = p->ordered_input;
   s->row0 = row0; s->row1 = row1;
   int rc = blend_plan(ctx, n, imgs, g, bands, p, ow, oh, row0, row1, false, &s->job, nullptr, nullptr, !shared_tab);
   if (!rc && !s->job.imgs.empty()) rc = blend_dev_setup(ctx, &s->job, bands, row0, row1, &s->dev, shared_tab);
@@ -959,28 +940,20 @@ int pano_blend_stream_create_cyl(pano_ctx* ctx, int n, const pano_blend_image* i
 
 int pano_blend_stream_needs(const pano_blend_stream* s, unsigned char* flags) {
   if (!s) return PANO_ERR_INVALID;
-  ctx_enter(s->ctx);
-  if (!flags) return ctx_fail(s->ctx, PANO_ERR_INVALID, "blend stream: null flags");
+  ctx_enter(s->st.ctx);
+  if (!flags) return ctx_fail(s->st.ctx, PANO_ERR_INVALID, "blend stream: null flags");
   for (int k = 0; k < s->n; ++k) flags[k] = s->slot[k] >= 0 ? 1 : 0;
   return PANO_OK;
 }
 
 int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void* const* srcs, int kind, int channels) {
   if (!s) return PANO_ERR_INVALID;
-  pano_ctx* ctx = s->ctx;
+  pano_ctx* ctx = s->st.ctx;
   ctx_enter(ctx);
-  if (s->err) return s->err;
-  if (s->finished) return STREAM_MISUSE(s, "blend stream: add after finish");
-  if (first != s->added || count <= 0 || count > s->n - first)
-    return STREAM_MISUSE(s, "blend stream: images [%d, %d) added, %d of %d so far", first, first + count, s->added, s->n);
-  if (!srcs) return STREAM_MISUSE(s, "blend stream: null source list");
-  for (int k = 0; k < count; ++k)
-    if (!srcs[k] && s->slot[first + k] >= 0) return STREAM_MISUSE(s, "blend stream: image %d has no source", first + k);
   SrcKind sk;
-  if (int rc = src_kind(ctx, "blend stream", kind, &sk)) return stream_fail(s, rc);
-  for (int k = 0; k < count; ++k)   // the alignment of the needed images only
-    if (int rc = src_check(ctx, "blend stream", sk, first + k, channels, s->slot[first + k] >= 0 ? srcs[k] : nullptr))
-      return stream_fail(s, rc);
+  if (int rc = s->st.add_check("blend stream", s->n, s->added, first, count, s->n, srcs, s->slot.data(), kind,
+                               channels, &sk))
+    return rc;
   // The window's needed images.  Their table rows go to d_imgs from the first one's entry on: for multiband
   // they are exactly the consecutive entries mb_levels reads again; linear reads them in this window only.
   // A cylinder stream's entries point at their warp entries in d_cyl, and those at the sources.
@@ -1012,62 +985,61 @@ int pano_blend_stream_add(pano_blend_stream* s, int first, int count, const void
     return PANO_OK;
   }
   int slot = -1, rc = 0;
-  if (sk.host && !s->ring.copy) {      // the copy stream and events of the first host window
-    cudaError_t e = s->ring.init();
-    if (e != cudaSuccess) return stream_fail(s, ctx_cuda(ctx, e, "blend stream: copy stream / events"));
-  }
   std::vector<const void*> d_src(wsrc);   // host sources: their copies in the ring
-  if (sk.host && (rc = s->ring.upload(ctx, nw, wsrc.data(), bytes.data(), d_src.data(), &slot))) return stream_fail(s, rc);
+  if (sk.host && (rc = s->ring.upload(ctx, "blend stream", nw, wsrc.data(), bytes.data(), d_src.data(), &slot)))
+    return s->st.fail(rc);
   for (int k = 0; k < nw; ++k) (cyl ? cwin[k].src : win[k].src) = d_src[k];
   BlendImg* d_win = s->dev.d_imgs + j0;
   if (cyl) {
     void* dsts[2] = {d_win, s->d_cyl + j0};
     const void* hsrcs[2] = {win.data(), cwin.data()};
     size_t sizes[2] = {nw * sizeof(BlendImg), nw * sizeof(CylImg)};
-    if ((rc = ctx_put_many(ctx, 2, dsts, hsrcs, sizes))) return stream_fail(s, rc);
+    if ((rc = ctx_put_many(ctx, 2, dsts, hsrcs, sizes))) return s->st.fail(rc);
   } else {
-    if ((rc = ctx_put(ctx, d_win, win.data(), nw * sizeof(BlendImg)))) return stream_fail(s, rc);
+    if ((rc = ctx_put(ctx, d_win, win.data(), nw * sizeof(BlendImg)))) return s->st.fail(rc);
   }
   rc = with_reader(src_reader(sk.u8 ? &channels : nullptr, 1), [&](auto tag) {
     using Src = typename decltype(tag)::type;
     return cyl ? stream_launch<SrcCyl<Src>>(s, d_win, win.data(), nw) : stream_launch<Src>(s, d_win, win.data(), nw);
   });
-  if (rc) return stream_fail(s, rc);
-  if (slot >= 0) STREAM_CUDA(s, s->ring.release(ctx, slot));
+  if (rc) return s->st.fail(rc);
+  if (slot >= 0 && (rc = s->st.cuda(s->ring.release(ctx, slot), "s->ring.release(ctx, slot)"))) return rc;
   s->added += count;
   return PANO_OK;
 }
 
 int pano_blend_stream_finish_dev(pano_blend_stream* s, float* d_out) {
   if (!s) return PANO_ERR_INVALID;
-  ctx_enter(s->ctx);
-  int rc = stream_finish_check(s, d_out);
-  if (!rc) rc = stream_resolve(s, d_out);
-  return rc ? stream_fail(s, rc) : PANO_OK;
+  ctx_enter(s->st.ctx);
+  if (int rc = s->st.finish_check("blend stream", d_out, s->added, s->n)) return rc;
+  if (int rc = stream_resolve(s, d_out)) return s->st.fail(rc);
+  return PANO_OK;
 }
 
 int pano_blend_stream_finish(pano_blend_stream* s, float* out) {
   if (!s) return PANO_ERR_INVALID;
-  pano_ctx* ctx = s->ctx;
+  pano_ctx* ctx = s->st.ctx;
   ctx_enter(ctx);
-  int rc = stream_finish_check(s, out);
-  if (rc) return stream_fail(s, rc);
+  int rc = s->st.finish_check("blend stream", out, s->added, s->n);
+  if (rc) return rc;
   const size_t nfl = (size_t)s->job.tw * (s->row1 - s->row0) * 3;
   DevBuf<float> d_tmp;
   float* d_out = s->d_sum;     // linear: resolved in place
   if (s->bands > 0) {
-    if ((rc = d_tmp.alloc(ctx, nfl))) return stream_fail(s, rc);
+    if ((rc = d_tmp.alloc(ctx, nfl))) return s->st.fail(rc);
     d_out = d_tmp;
   }
-  if ((rc = stream_resolve(s, d_out))) return stream_fail(s, rc);
-  STREAM_CUDA(s, cudaMemcpyAsync(out, d_out, nfl * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-  STREAM_CUDA(s, cudaStreamSynchronize(ctx->stream));
+  if ((rc = stream_resolve(s, d_out))) return s->st.fail(rc);
+  if ((rc = s->st.cuda(cudaMemcpyAsync(out, d_out, nfl * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream),
+                       "cudaMemcpyAsync(out, d_out, nfl * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream)")) ||
+      (rc = s->st.cuda(cudaStreamSynchronize(ctx->stream), "cudaStreamSynchronize(ctx->stream)")))
+    return rc;
   d_tmp.reset();
   return PANO_OK;
 }
 
 void pano_blend_stream_free(pano_blend_stream* s) {
-  if (s) ctx_enter(s->ctx);
+  if (s) ctx_enter(s->st.ctx);
   delete s;
 }
 

@@ -104,7 +104,7 @@ struct ScanFree { void operator()(pano_crop_scan* c) const { pano_crop_scan_free
 }  // namespace
 
 struct pano_blend_sweep {
-  pano_ctx* ctx = nullptr;
+  Sticky st;
   int n = 0, bands = 0, ow = 0, oh = 0, rows = 0;
   pano_params p;
   pano_blend_geom g;
@@ -117,25 +117,19 @@ struct pano_blend_sweep {
   DevBuf<int> d_rect;
   std::unique_ptr<pano_crop_scan, ScanFree> scan;
   std::vector<Held> held;
-  int done = 0, err = 0;
-  bool finished = false;
+  int done = 0;
   long long uploads = 0;
   unsigned long long upload_bytes = 0, retained_high = 0;
   UploadRing ring;                 // last: its copy stream drains before the blocks above go
 };
 
-static int sweep_fail(pano_blend_sweep* s, int rc) { s->err = rc; return rc; }
-#define SWEEP_MISUSE(s, ...) sweep_fail((s), ctx_fail((s)->ctx, PANO_ERR_INVALID, __VA_ARGS__))
-#define SWEEP_CUDA(s, call)                                                \
-  do {                                                                     \
-    cudaError_t _e = (call);                                               \
-    if (_e != cudaSuccess) return sweep_fail((s), ctx_cuda((s)->ctx, _e, #call)); \
-  } while (0)
-
 // The uploads of the previous strip are over: its pinned buffers are the caller's again.
 static int sweep_wait_previous(pano_blend_sweep* s) {
   if (s->ring.copy)
-    for (int b = 0; b < 2; ++b) SWEEP_CUDA(s, cudaEventSynchronize(s->ring.ev_copied[b].get()));
+    for (int b = 0; b < 2; ++b)
+      if (int rc = s->st.cuda(cudaEventSynchronize(s->ring.ev_copied[b].get()),
+                              "cudaEventSynchronize(s->ring.ev_copied[b].get())"))
+        return rc;
   return PANO_OK;
 }
 
@@ -145,7 +139,7 @@ static int sweep_wait_previous(pano_blend_sweep* s) {
 // A kept one is then copied into a block of its own.  srcs / u8 / host / fmt / sz: the strip call's, checked.
 static int sweep_blend(pano_blend_sweep* s, int st, const void* const* srcs, bool u8, bool host,
                        const std::vector<int>& fmt, const std::vector<size_t>& sz) {
-  pano_ctx* ctx = s->ctx;
+  pano_ctx* ctx = s->st.ctx;
   const int n = s->n;
   const unsigned char* up = &s->plan.uploads[(size_t)st * n];
   const unsigned char* rd = &s->plan.reads[(size_t)st * n];
@@ -180,9 +174,7 @@ static int sweep_blend(pano_blend_sweep* s, int st, const void* const* srcs, boo
     }
     int slot = -1;
     if (upload >= 0) {
-      if (!s->ring.copy)
-        if (cudaError_t e = s->ring.init()) return ctx_cuda(ctx, e, "blend sweep: copy stream / events");
-      if ((rc = s->ring.upload(ctx, 1, &srcs[upload], &sz[upload], &src[upload], &slot))) return rc;
+      if ((rc = s->ring.upload(ctx, "blend sweep", 1, &srcs[upload], &sz[upload], &src[upload], &slot))) return rc;
       if (keep[upload]) {
         Held& h = s->held[upload];
         h = Held();
@@ -231,7 +223,7 @@ int pano_blend_sweep_create(pano_ctx* ctx, int n, const pano_blend_image* imgs, 
   if (n <= 0 || !imgs || !g || !p || bands < 0 || strip_rows < 1) return ctx_fail(ctx, PANO_ERR_INVALID, "blend sweep: bad argument");
   if (n > PANO_MAX_IMAGES) return ctx_fail(ctx, PANO_ERR_INVALID, "blend sweep: %d images (limit %d)", n, PANO_MAX_IMAGES);
   std::unique_ptr<pano_blend_sweep> s(new pano_blend_sweep);
-  s->ctx = ctx; s->n = n; s->bands = bands; s->ow = out_w; s->oh = out_h; s->rows = std::min(strip_rows, out_h);
+  s->st.ctx = ctx; s->n = n; s->bands = bands; s->ow = out_w; s->oh = out_h; s->rows = std::min(strip_rows, out_h);
   s->p = *p; s->g = *g;
   s->imgs.assign(imgs, imgs + n);
   std::vector<double> tab;
@@ -260,8 +252,8 @@ int pano_blend_sweep_create(pano_ctx* ctx, int n, const pano_blend_image* imgs, 
 
 int pano_blend_sweep_next(pano_blend_sweep* s, unsigned char* want) {
   if (!s) return PANO_ERR_INVALID;
-  ctx_enter(s->ctx);
-  if (s->err) return s->err;
+  ctx_enter(s->st.ctx);
+  if (s->st.err) return s->st.err;
   const bool over = s->done >= s->plan.strips;
   if (want)
     for (int k = 0; k < s->n; ++k) want[k] = over ? 0 : s->plan.uploads[(size_t)s->done * s->n + k];
@@ -270,38 +262,39 @@ int pano_blend_sweep_next(pano_blend_sweep* s, unsigned char* want) {
 
 int pano_blend_sweep_strip(pano_blend_sweep* s, const void* const* srcs, const int* formats, int kind) {
   if (!s) return PANO_ERR_INVALID;
-  pano_ctx* ctx = s->ctx;
+  Sticky& ss = s->st;
+  pano_ctx* ctx = ss.ctx;
   ctx_enter(ctx);
-  if (s->err) return s->err;
-  if (s->finished || s->done >= s->plan.strips) return SWEEP_MISUSE(s, "blend sweep: strip after the last");
-  if (!srcs) return SWEEP_MISUSE(s, "blend sweep: null source list");
+  if (ss.err) return ss.err;
+  if (ss.finished || s->done >= s->plan.strips) return ss.misuse("blend sweep: strip after the last");
+  if (!srcs) return ss.misuse("blend sweep: null source list");
   SrcKind sk;
-  if (int rc = src_kind(ctx, "blend sweep", kind, &sk)) return sweep_fail(s, rc);
+  if (int rc = src_kind(ctx, "blend sweep", kind, &sk)) return ss.fail(rc);
   const bool u8 = sk.u8;
-  if (u8 && !formats) return SWEEP_MISUSE(s, "blend sweep: null format list");
+  if (u8 && !formats) return ss.misuse("blend sweep: null format list");
   const int n = s->n, st = s->done;
   const unsigned char* up = &s->plan.uploads[(size_t)st * n];
   std::vector<int> fmt(n, 3);
   std::vector<size_t> sz(n, 0);
   std::vector<int> list;           // the images handed over, in order
   for (int k = 0; k < n; ++k) {
-    if (!srcs[k] && up[k]) return SWEEP_MISUSE(s, "blend sweep: strip %d needs image %d", st, k);
-    if (srcs[k] && !up[k]) return SWEEP_MISUSE(s, "blend sweep: strip %d was not to be given image %d", st, k);
+    if (!srcs[k] && up[k]) return ss.misuse("blend sweep: strip %d needs image %d", st, k);
+    if (srcs[k] && !up[k]) return ss.misuse("blend sweep: strip %d was not to be given image %d", st, k);
     if (!srcs[k]) continue;
     fmt[k] = u8 ? formats[k] : 3;
-    if (int rc = src_check(ctx, "blend sweep", sk, k, fmt[k], srcs[k])) return sweep_fail(s, rc);
+    if (int rc = src_check(ctx, "blend sweep", sk, k, fmt[k], srcs[k])) return ss.fail(rc);
     sz[k] = src_bytes(s->imgs[k].w, s->imgs[k].h, u8, fmt[k]);
     if (sz[k] > s->bytes[k])
-      return SWEEP_MISUSE(s, "blend sweep: image %d takes %zu bytes, planned with %zu", k, sz[k], s->bytes[k]);
+      return ss.misuse("blend sweep: image %d takes %zu bytes, planned with %zu", k, sz[k], s->bytes[k]);
     list.push_back(k);
   }
   if (int rc = sweep_wait_previous(s)) return rc;
-  if (int rc = sweep_blend(s, st, srcs, u8, sk.host, fmt, sz)) return sweep_fail(s, rc);
+  if (int rc = sweep_blend(s, st, srcs, u8, sk.host, fmt, sz)) return ss.fail(rc);
   const int row0 = st * s->rows, row1 = std::min(s->oh, row0 + s->rows);
   if (s->scan)
-    if (int rc = pano_crop_scan_add_dev(s->scan.get(), s->d_strip, row1 - row0)) return sweep_fail(s, rc);
+    if (int rc = pano_crop_scan_add_dev(s->scan.get(), s->d_strip, row1 - row0)) return ss.fail(rc);
   if (int rc = pano_mat32f_to_rgb8_dev(ctx, s->d_strip, s->ow, row1 - row0, nullptr, s->d_rgb + (size_t)row0 * s->ow * 3))
-    return sweep_fail(s, rc);
+    return ss.fail(rc);
   // drop what the plan does not keep past this strip (freed in stream order, after its readers)
   unsigned long long kept_bytes = 0;
   const unsigned char* hold = &s->plan.held[(size_t)st * n];
@@ -318,22 +311,23 @@ int pano_blend_sweep_strip(pano_blend_sweep* s, const void* const* srcs, const i
 
 int pano_blend_sweep_finish_dev(pano_blend_sweep* s, int out_format, unsigned char* d_out, int rect[4]) {
   if (!s) return PANO_ERR_INVALID;
-  pano_ctx* ctx = s->ctx;
+  Sticky& ss = s->st;
+  pano_ctx* ctx = ss.ctx;
   ctx_enter(ctx);
-  if (s->err) return s->err;
-  if (!d_out || !rect) return SWEEP_MISUSE(s, "blend sweep: null output");
-  if (s->finished) return SWEEP_MISUSE(s, "blend sweep: already finished");
-  if (s->done < s->plan.strips) return SWEEP_MISUSE(s, "blend sweep: finish after %d of %d strips", s->done, s->plan.strips);
+  if (ss.err) return ss.err;
+  if (!d_out || !rect) return ss.misuse("blend sweep: null output");
+  if (ss.finished) return ss.misuse("blend sweep: already finished");
+  if (s->done < s->plan.strips) return ss.misuse("blend sweep: finish after %d of %d strips", s->done, s->plan.strips);
   if (out_format != PANO_PIX_RGB && out_format != PANO_PIX_RGBA && out_format != PANO_PIX_RGB_PLANAR)
-    return SWEEP_MISUSE(s, "blend sweep: output format %#x", out_format);
-  s->finished = true;
+    return ss.misuse("blend sweep: output format %#x", out_format);
+  ss.finished = true;
   if (int rc = sweep_wait_previous(s)) return rc;
   int r[4] = {0, 0, s->ow, s->oh};
   if (s->scan)
-    if (int rc = pano_crop_scan_rect(s->scan.get(), r)) return sweep_fail(s, rc);
-  if (int rc = ctx_put(ctx, s->d_rect, r, sizeof(r))) return sweep_fail(s, rc);
+    if (int rc = pano_crop_scan_rect(s->scan.get(), r)) return ss.fail(rc);
+  if (int rc = ctx_put(ctx, s->d_rect, r, sizeof(r))) return ss.fail(rc);
   if (int rc = pano_rgb8_crop_to_pix8_dev(ctx, s->d_rgb, s->ow, s->oh, s->d_rect, out_format, d_out))
-    return sweep_fail(s, rc);
+    return ss.fail(rc);
   for (int q = 0; q < 4; ++q) rect[q] = r[q];
   return PANO_OK;
 }
@@ -348,7 +342,7 @@ int pano_blend_sweep_stats(const pano_blend_sweep* s, long long* uploads, unsign
 }
 
 void pano_blend_sweep_free(pano_blend_sweep* s) {
-  if (s) ctx_enter(s->ctx);
+  if (s) ctx_enter(s->st.ctx);
   delete s;
 }
 

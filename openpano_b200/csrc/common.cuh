@@ -222,17 +222,19 @@ int  ctx_copy_blocks(pano_ctx* ctx, int n, void* const* dst, const void* const* 
 void ctx_prof_begin(pano_ctx* ctx, const char* name);
 void ctx_prof_end(pano_ctx* ctx);
 
-// Two-slot device ring for windows of host sources (pano_blend_stream, pano_sift_stream): window k's upload runs
-// on the ring's own copy stream into slot k & 1 while earlier windows' kernels run on the context's stream;
-// events order each slot's reuse, so at most two windows of sources are resident.  Each slot is as large as the
-// largest window uploaded through it; pageable sources go through a pinned staging buffer per slot.
+// Two-slot device ring for windows of host sources (pano_blend_stream, pano_sift_stream, pano_blend_sweep): window
+// k's upload runs on the ring's own copy stream into slot k & 1 while earlier windows' kernels run on the context's
+// stream; events order each slot's reuse, so at most two windows of sources are resident.  Each slot is as large as
+// the largest window uploaded through it; pageable sources go through a pinned staging buffer per slot.  The copy
+// stream and events are created by the first upload, so a handle given device sources only has none.
 struct UploadRing {
   // the copy stream drains before the staging and slot memory go
   ~UploadRing() { if (copy) cudaStreamSynchronize(copy.get()); }
-  cudaError_t init();
   // Uploads count host sources of bytes[k] each into the next slot and points d_src[k] at their device copies;
-  // the context's stream waits for the upload.  *slot_out: the slot, to hand to release().
-  int upload(pano_ctx* ctx, int count, const void* const* srcs, const size_t* bytes, const void** d_src, int* slot_out);
+  // the context's stream waits for the upload.  *slot_out: the slot, to hand to release().  A failure to create
+  // the copy stream or events is reported as "<what>: copy stream / events".
+  int upload(pano_ctx* ctx, const char* what, int count, const void* const* srcs, const size_t* bytes,
+             const void** d_src, int* slot_out);
   // The slot's last reader has been queued on the context's stream: the upload two windows on may overwrite it.
   cudaError_t release(pano_ctx* ctx, int slot);
 
@@ -310,6 +312,27 @@ static inline size_t src_bytes(int w, int h, bool u8, int fmt) {
 // Checks image i of a source argument: its format (a PANO_PIX_* format for 8-bit sources, 3 for f32 ones) and, for
 // a device source px (null: not checked), pix8_check's alignment; fails the context with `what` in the message.
 int src_check(pano_ctx* ctx, const char* what, const SrcKind& k, int i, int fmt, const void* px);
+
+// The state every stateful handle (blend stream, SIFT stream, blend sweep, crop scan) keeps for the handle contract
+// of pano_b200.h: its context, the failure that every later call returns again, and whether it has finished.
+struct Sticky {
+  pano_ctx* ctx = nullptr;
+  int err = 0;
+  bool finished = false;
+  int fail(int rc) { err = rc; return rc; }
+  // ctx_fail(ctx, PANO_ERR_INVALID, fmt, ...), then fail
+  int misuse(const char* fmt, ...) __attribute__((format(printf, 2, 3)));
+  // PANO_OK for cudaSuccess, else ctx_cuda(ctx, e, what), then fail
+  int cuda(cudaError_t e, const char* what) { return e == cudaSuccess ? PANO_OK : fail(ctx_cuda(ctx, e, what)); }
+  // The checks of an add of images [first, first + count) to a stream of n images that has taken `added`, in this
+  // order: add after finish, the window's range, at most `cap` images in one add, the source list, a null source
+  // and each source's kind and format (src_kind, src_check).  read[i] < 0 marks an image of the stream that is not
+  // read (read null: all are): it needs no source and its alignment is not checked.  Messages start with `what`.
+  int add_check(const char* what, int n, int added, int first, int count, int cap, const void* const* srcs,
+                const int* read, int kind, int fmt, SrcKind* sk);
+  // The checks of a finish after `added` of n images: a null output, a second finish, images missing; then finished.
+  int finish_check(const char* what, const void* out, int added, int n);
+};
 
 // The inverse map of CylinderWarper(h_factor).warp on a w×h image (warp.cu; host arithmetic): the warped shape
 // ow×oh, the constants, and the per-column tables col_x[ow] then col_cos[ow] appended to *tabs when the shape is

@@ -12,14 +12,53 @@
 
 static thread_local std::string g_create_err;
 
-int ctx_fail(pano_ctx* ctx, int code, const char* fmt, ...) {
+static int ctx_vfail(pano_ctx* ctx, int code, const char* fmt, va_list ap) {
   char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
   vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
   if (ctx) ctx->err = buf; else g_create_err = buf;
   return code;
+}
+
+int ctx_fail(pano_ctx* ctx, int code, const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  ctx_vfail(ctx, code, fmt, ap);
+  va_end(ap);
+  return code;
+}
+
+int Sticky::misuse(const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  ctx_vfail(ctx, PANO_ERR_INVALID, fmt, ap);
+  va_end(ap);
+  return fail(PANO_ERR_INVALID);
+}
+
+int Sticky::add_check(const char* what, int n, int added, int first, int count, int cap, const void* const* srcs,
+                      const int* read, int kind, int fmt, SrcKind* sk) {
+  if (err) return err;
+  if (finished) return misuse("%s: add after finish", what);
+  if (first != added || count <= 0 || count > n - first)
+    return misuse("%s: images [%d, %d) added, %d of %d so far", what, first, first + count, added, n);
+  if (count > cap) return misuse("%s: %d images in one add (limit %d)", what, count, cap);
+  if (!srcs) return misuse("%s: null source list", what);
+  for (int k = 0; k < count; ++k)
+    if (!srcs[k] && (!read || read[first + k] >= 0)) return misuse("%s: image %d has no source", what, first + k);
+  if (int rc = src_kind(ctx, what, kind, sk)) return fail(rc);
+  for (int k = 0; k < count; ++k)   // the alignment of the images read only
+    if (int rc = src_check(ctx, what, *sk, first + k, fmt, !read || read[first + k] >= 0 ? srcs[k] : nullptr))
+      return fail(rc);
+  return PANO_OK;
+}
+
+int Sticky::finish_check(const char* what, const void* out, int added, int n) {
+  if (err) return err;
+  if (!out) return misuse("%s: null output", what);
+  if (finished) return misuse("%s: already finished", what);
+  if (added != n) return misuse("%s: finish after %d of %d images", what, added, n);
+  finished = true;
+  return PANO_OK;
 }
 
 int pix8_check(pano_ctx* ctx, const char* what, int i, int fmt, const void* d_pix) {
@@ -401,17 +440,16 @@ int ctx_copy_blocks(pano_ctx* ctx, int n, void* const* dst, const void* const* s
   return PANO_OK;
 }
 
-cudaError_t UploadRing::init() {
-  cudaError_t e = make_stream(&copy);
-  for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
-    e = make_event(&ev_copied[b], cudaEventDisableTiming);
-    if (e == cudaSuccess) e = make_event(&ev_done[b], cudaEventDisableTiming);
+int UploadRing::upload(pano_ctx* ctx, const char* what, int count, const void* const* srcs, const size_t* bytes,
+                       const void** d_src, int* slot_out) {
+  if (!copy) {
+    cudaError_t e = make_stream(&copy);
+    for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
+      e = make_event(&ev_copied[b], cudaEventDisableTiming);
+      if (e == cudaSuccess) e = make_event(&ev_done[b], cudaEventDisableTiming);
+    }
+    if (e != cudaSuccess) return ctx_cuda(ctx, e, (std::string(what) + ": copy stream / events").c_str());
   }
-  return e;
-}
-
-int UploadRing::upload(pano_ctx* ctx, int count, const void* const* srcs, const size_t* bytes, const void** d_src,
-                       int* slot_out) {
   const int b = windows & 1;
   std::vector<size_t> off(count);
   size_t total = 0;

@@ -432,19 +432,18 @@ __global__ void __launch_bounds__(256) k_rgb8_crop(const unsigned char* __restri
 #define CROP_SCAN_MAX_W 80000   // the reference's limit on a mosaic's edge (stitcher_image.cc:105)
 
 struct pano_crop_scan {
-  pano_ctx* ctx = nullptr;
-  int w = 0, h = 0, lines = 0, err = 0;
+  Sticky st;
+  int w = 0, h = 0, lines = 0;
   DevBuf<int> d_last;        // [w] last invalid line of each column so far, -1 if none
   DevBuf<CropBest> d_run;    // the best rectangle so far
   DevBuf<int> d_rect;        // crop()'s rectangle of the lines so far
 };
 
-static int scan_fail(pano_crop_scan* c, int rc) { c->err = rc; return rc; }
-
-// Steps (1) to (3) on the next `rows` lines of the mosaic.
-static int crop_scan_strip(pano_crop_scan* c, const float* d_strip, int rows) {
-  pano_ctx* ctx = c->ctx;
-  const int w = c->w, chunks = ceil_div(rows, CROP_CHUNK), line0 = c->lines;
+// Steps (1) to (3) on lines [line0, line0 + rows) of a w-column mosaic, d_strip holding those lines: d_last and d_run
+// carry the lines before line0 (null for none), and d_rect gets crop()'s rectangle of the lines up to the last.
+static int crop_strip(pano_ctx* ctx, const float* d_strip, int w, int rows, int line0, int* d_last, CropBest* d_run,
+                      int* d_rect) {
+  const int chunks = ceil_div(rows, CROP_CHUNK);
   DevBuf<unsigned> d_masks;
   DevBuf<int> d_carry;
   DevBuf<CropLineBest> d_best;
@@ -452,17 +451,17 @@ static int crop_scan_strip(pano_crop_scan* c, const float* d_strip, int rows) {
   if ((rc = d_masks.alloc(ctx, (size_t)chunks * w)) || (rc = d_carry.alloc(ctx, (size_t)chunks * w)) ||
       (rc = d_best.alloc(ctx, (size_t)rows)))
     return rc;
-  // the line kernel of pano_crop_rect_dev where the line's heights fit in shared memory, else the one that reads
-  // them from the masks and the carry (l1 / l2 of CROP_SCAN_MAX_W columns fit in the run arrays)
+  // the line kernel that keeps the line's heights in shared memory where they fit, else the one that reads them
+  // from the masks and the carry (l1 / l2 of CROP_SCAN_MAX_W columns fit in the run arrays)
   const bool smem_line = CROP_LINE_SMEM(w) <= CROP_LINE_SMEM_MAX;
   const size_t smem = smem_line ? CROP_LINE_SMEM(w) : sizeof(int) * (4 * CROP_RUN_CAP + 1);
   if (smem_line && smem > 48 * 1024)
     PANO_CUDA(ctx, cudaFuncSetAttribute(k_crop_line<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   PANO_LAUNCH(ctx, "k_crop_masks", k_crop_masks, dim3(ceil_div(w, 128), chunks), 128, 0, d_strip, w, rows, d_masks);
-  PANO_LAUNCH(ctx, "k_crop_carry", k_crop_carry, ceil_div(w, 128), 128, 0, d_masks, w, chunks, line0, c->d_last, d_carry);
+  PANO_LAUNCH(ctx, "k_crop_carry", k_crop_carry, ceil_div(w, 128), 128, 0, d_masks, w, chunks, line0, d_last, d_carry);
   if (smem_line) PANO_LAUNCH(ctx, "k_crop_line", k_crop_line<true>, rows, 256, smem, d_masks, d_carry, w, line0, d_best);
   else PANO_LAUNCH(ctx, "k_crop_scan_line", k_crop_line<false>, rows, 256, smem, d_masks, d_carry, w, line0, d_best);
-  PANO_LAUNCH(ctx, "k_crop_final", k_crop_final, 1, 256, 0, d_best, rows, line0, c->d_run, c->d_rect);
+  PANO_LAUNCH(ctx, "k_crop_final", k_crop_final, 1, 256, 0, d_best, rows, line0, d_run, d_rect);
   return PANO_OK;
 }
 
@@ -510,22 +509,10 @@ int pano_crop_rect_dev(pano_ctx* ctx, const float* d_mat_hwc, int w, int h, int*
   ctx_enter(ctx);
   if (!ctx || !d_mat_hwc || !d_rect || w <= 0 || h <= 0)
     return ctx_fail(ctx, PANO_ERR_INVALID, "pano_crop_rect_dev: bad argument");
-  const int chunks = ceil_div(h, CROP_CHUNK);
-  const size_t smem = CROP_LINE_SMEM(w);   // l1/l2 of the fallback fit in the run arrays
-  if (smem > CROP_LINE_SMEM_MAX) return ctx_fail(ctx, PANO_ERR_INVALID, "pano_crop_rect_dev: width %d exceeds the %d-column limit", w, 40000);
-  DevBuf<unsigned> d_masks;
-  DevBuf<int> d_carry;
-  DevBuf<CropLineBest> d_best;
-  if (int rc = d_masks.alloc(ctx, (size_t)chunks * w)) return rc;
-  if (int rc = d_carry.alloc(ctx, (size_t)chunks * w)) return rc;
-  if (int rc = d_best.alloc(ctx, (size_t)h)) return rc;
-  if (smem > 48 * 1024)
-    PANO_CUDA(ctx, cudaFuncSetAttribute(k_crop_line<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  PANO_LAUNCH(ctx, "k_crop_masks", k_crop_masks, dim3(ceil_div(w, 128), chunks), 128, 0, d_mat_hwc, w, h, d_masks);
-  PANO_LAUNCH(ctx, "k_crop_carry", k_crop_carry, ceil_div(w, 128), 128, 0, d_masks, w, chunks, 0, nullptr, d_carry);
-  PANO_LAUNCH(ctx, "k_crop_line", k_crop_line<true>, h, 256, smem, d_masks, d_carry, w, 0, d_best);
-  PANO_LAUNCH(ctx, "k_crop_final", k_crop_final, 1, 256, 0, d_best, h, 0, nullptr, d_rect);
-  return PANO_OK;
+  // the widths whose line heights fit in shared memory: crop_strip's k_crop_line<true>
+  if (CROP_LINE_SMEM(w) > CROP_LINE_SMEM_MAX)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "pano_crop_rect_dev: width %d exceeds the %d-column limit", w, 40000);
+  return crop_strip(ctx, d_mat_hwc, w, h, 0, nullptr, nullptr, d_rect);
 }
 
 int pano_crop_scan_create(pano_ctx* ctx, int w, int h, pano_crop_scan** out) {
@@ -535,7 +522,7 @@ int pano_crop_scan_create(pano_ctx* ctx, int w, int h, pano_crop_scan** out) {
   if (w <= 0 || h <= 0 || w > CROP_SCAN_MAX_W)
     return ctx_fail(ctx, PANO_ERR_INVALID, "crop scan: %dx%d (widths 1 to %d)", w, h, CROP_SCAN_MAX_W);
   std::unique_ptr<pano_crop_scan> c(new pano_crop_scan);
-  c->ctx = ctx; c->w = w; c->h = h;
+  c->st.ctx = ctx; c->w = w; c->h = h;
   int rc = 0;
   if ((rc = c->d_last.alloc(ctx, w)) || (rc = c->d_run.alloc(ctx, 1)) || (rc = c->d_rect.alloc(ctx, 4))) return rc;
   PANO_CUDA(ctx, cudaMemsetAsync(c->d_last, 0xff, sizeof(int) * w, ctx->stream));   // -1
@@ -546,32 +533,30 @@ int pano_crop_scan_create(pano_ctx* ctx, int w, int h, pano_crop_scan** out) {
 
 int pano_crop_scan_add_dev(pano_crop_scan* c, const float* d_strip_hwc, int rows) {
   if (!c) return PANO_ERR_INVALID;
-  pano_ctx* ctx = c->ctx;
-  ctx_enter(ctx);
-  if (c->err) return c->err;
+  ctx_enter(c->st.ctx);
+  if (c->st.err) return c->st.err;
   if (!d_strip_hwc || rows <= 0 || rows > c->h - c->lines)
-    return scan_fail(c, ctx_fail(ctx, PANO_ERR_INVALID, "crop scan: %d lines at line %d of %d", rows, c->lines, c->h));
-  if (int rc = crop_scan_strip(c, d_strip_hwc, rows)) return scan_fail(c, rc);
+    return c->st.misuse("crop scan: %d lines at line %d of %d", rows, c->lines, c->h);
+  if (int rc = crop_strip(c->st.ctx, d_strip_hwc, c->w, rows, c->lines, c->d_last, c->d_run, c->d_rect))
+    return c->st.fail(rc);
   c->lines += rows;
   return PANO_OK;
 }
 
 int pano_crop_scan_rect(pano_crop_scan* c, int rect[4]) {
   if (!c) return PANO_ERR_INVALID;
-  pano_ctx* ctx = c->ctx;
+  pano_ctx* ctx = c->st.ctx;
   ctx_enter(ctx);
-  if (c->err) return c->err;
-  if (!rect) return scan_fail(c, ctx_fail(ctx, PANO_ERR_INVALID, "crop scan: null rect"));
-  if (c->lines != c->h)
-    return scan_fail(c, ctx_fail(ctx, PANO_ERR_INVALID, "crop scan: rect after %d of %d lines", c->lines, c->h));
+  if (c->st.err) return c->st.err;
+  if (!rect) return c->st.misuse("crop scan: null rect");
+  if (c->lines != c->h) return c->st.misuse("crop scan: rect after %d of %d lines", c->lines, c->h);
   cudaError_t e = cudaMemcpyAsync(rect, c->d_rect, 4 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-  if (e != cudaSuccess) return scan_fail(c, ctx_cuda(ctx, e, "crop scan: rect"));
-  return PANO_OK;
+  return c->st.cuda(e, "crop scan: rect");
 }
 
 void pano_crop_scan_free(pano_crop_scan* c) {
-  if (c) ctx_enter(c->ctx);
+  if (c) ctx_enter(c->st.ctx);
   delete c;
 }
 

@@ -33,11 +33,10 @@ struct PackedWindow {
 struct pano_sift_stream {
   ~pano_sift_stream() {
     // the count read-back of a window never resolved still writes into its pinned block
-    if (pending.fs && pending.fs->counts_pending) ctx_wait_signal(ctx, pending.fs->counts_token);
+    if (pending.fs && pending.fs->counts_pending) ctx_wait_signal(st.ctx, pending.fs->counts_token);
   }
-  pano_ctx* ctx = nullptr;
-  int n = 0, added = 0, err = 0;
-  bool finished = false;
+  Sticky st;
+  int n = 0, added = 0;
   std::vector<int> w, h;
   pano_params p;
   std::vector<int> count;                 // descriptors per image of the finished windows
@@ -46,15 +45,11 @@ struct pano_sift_stream {
   PendingWindow pending;
 };
 
-// every failure is sticky: a window may be lost after it
-static int sift_stream_fail(pano_sift_stream* s, int rc) { s->err = rc; return rc; }
-#define SIFT_STREAM_MISUSE(s, ...) sift_stream_fail((s), ctx_fail((s)->ctx, PANO_ERR_INVALID, __VA_ARGS__))
-
 // Reads the pending window's counts (a list overflow re-runs it), frees its ring slot and packs its rows.
 static int sift_stream_resolve(pano_sift_stream* s) {
   PendingWindow& win = s->pending;
   if (!win.fs) return PANO_OK;
-  pano_ctx* ctx = s->ctx;
+  pano_ctx* ctx = s->st.ctx;
   pano_featureset* fs = win.fs.get();
   if (int rc = featureset_sync_counts(fs)) return rc;
   if (win.slot >= 0) PANO_CUDA(ctx, s->ring.release(ctx, win.slot));   // its last reader is queued
@@ -94,32 +89,21 @@ int pano_sift_stream_create(pano_ctx* ctx, int n, const int* w, const int* h, co
   for (int i = 0; i < n; ++i)
     if (w[i] < 2 || h[i] < 2) return ctx_fail(ctx, PANO_ERR_INVALID, "sift stream: image %d is %dx%d (at least 2x2)", i, w[i], h[i]);
   std::unique_ptr<pano_sift_stream> s(new pano_sift_stream);
-  s->ctx = ctx; s->n = n; s->p = *p;
+  s->st.ctx = ctx; s->n = n; s->p = *p;
   s->w.assign(w, w + n); s->h.assign(h, h + n);
   s->count.assign(n, 0);
-  cudaError_t e = s->ring.init();
-  if (e != cudaSuccess) return ctx_cuda(ctx, e, "sift stream: copy stream / events");
   *out = s.release();
   return PANO_OK;
 }
 
 int pano_sift_stream_add(pano_sift_stream* s, int first, int count, const void* const* srcs, int kind, int channels) {
   if (!s) return PANO_ERR_INVALID;
-  pano_ctx* ctx = s->ctx;
+  pano_ctx* ctx = s->st.ctx;
   ctx_enter(ctx);
-  if (s->err) return s->err;
-  if (s->finished) return SIFT_STREAM_MISUSE(s, "sift stream: add after finish");
-  if (first != s->added || count <= 0 || count > s->n - first)
-    return SIFT_STREAM_MISUSE(s, "sift stream: images [%d, %d) added, %d of %d so far", first, first + count, s->added, s->n);
-  if (count > PANO_MAX_SIFT_BATCH)
-    return SIFT_STREAM_MISUSE(s, "sift stream: %d images in one add (limit %d)", count, PANO_MAX_SIFT_BATCH);
-  if (!srcs) return SIFT_STREAM_MISUSE(s, "sift stream: null source list");
-  for (int k = 0; k < count; ++k)
-    if (!srcs[k]) return SIFT_STREAM_MISUSE(s, "sift stream: image %d has no source", first + k);
   SrcKind sk;
-  if (int rc = src_kind(ctx, "sift stream", kind, &sk)) return sift_stream_fail(s, rc);
-  for (int k = 0; k < count; ++k)
-    if (int rc = src_check(ctx, "sift stream", sk, first + k, channels, srcs[k])) return sift_stream_fail(s, rc);
+  if (int rc = s->st.add_check("sift stream", s->n, s->added, first, count, PANO_MAX_SIFT_BATCH, srcs, nullptr, kind,
+                               channels, &sk))
+    return rc;
   const bool u8 = sk.u8;
 
   std::vector<const void*> d_src(srcs, srcs + count);
@@ -128,9 +112,9 @@ int pano_sift_stream_add(pano_sift_stream* s, int first, int count, const void* 
     std::vector<size_t> bytes(count);
     for (int k = 0; k < count; ++k)
       bytes[k] = src_bytes(s->w[first + k], s->h[first + k], u8, channels);
-    if (int rc = s->ring.upload(ctx, count, srcs, bytes.data(), d_src.data(), &slot)) return sift_stream_fail(s, rc);
+    if (int rc = s->ring.upload(ctx, "sift stream", count, srcs, bytes.data(), d_src.data(), &slot)) return s->st.fail(rc);
   }
-  if (int rc = sift_stream_resolve(s)) return sift_stream_fail(s, rc);
+  if (int rc = sift_stream_resolve(s)) return s->st.fail(rc);
 
   std::unique_ptr<pano_featureset> fs(new pano_featureset);
   fs->ctx = ctx;
@@ -141,7 +125,7 @@ int pano_sift_stream_add(pano_sift_stream* s, int first, int count, const void* 
   if (u8) fs->src_channels.assign(count, channels);
   int rc = sift_run_batch(ctx, count, d_src.data(), u8 ? fs->src_channels.data() : nullptr, fs->src_w.data(),
                           fs->src_h.data(), &s->p, fs.get(), nullptr, ctx_sift_cap(ctx));
-  if (rc) return sift_stream_fail(s, rc);
+  if (rc) return s->st.fail(rc);
   s->pending.first = first; s->pending.count = count; s->pending.slot = slot;
   s->pending.fs = std::move(fs);
   s->added += count;
@@ -150,15 +134,11 @@ int pano_sift_stream_add(pano_sift_stream* s, int first, int count, const void* 
 
 int pano_sift_stream_finish(pano_sift_stream* s, pano_featureset** out) {
   if (!s) return PANO_ERR_INVALID;
-  pano_ctx* ctx = s->ctx;
+  pano_ctx* ctx = s->st.ctx;
   ctx_enter(ctx);
   if (out) *out = nullptr;
-  if (s->err) return s->err;
-  if (!out) return SIFT_STREAM_MISUSE(s, "sift stream: null output");
-  if (s->finished) return SIFT_STREAM_MISUSE(s, "sift stream: already finished");
-  if (s->added != s->n) return SIFT_STREAM_MISUSE(s, "sift stream: finish after %d of %d images", s->added, s->n);
-  s->finished = true;
-  if (int rc = sift_stream_resolve(s)) return sift_stream_fail(s, rc);
+  if (int rc = s->st.finish_check("sift stream", out, s->added, s->n)) return rc;
+  if (int rc = sift_stream_resolve(s)) return s->st.fail(rc);
 
   // the packed windows back to back: their concatenation is the featureset's layout
   std::unique_ptr<pano_featureset> fs(new pano_featureset);
@@ -170,7 +150,7 @@ int pano_sift_stream_finish(pano_sift_stream* s, pano_featureset** out) {
   int rc = fs->d_desc.alloc(ctx, rows * 128);
   if (!rc) rc = fs->d_coor.alloc(ctx, rows * 4);
   if (!rc) rc = fs->d_count.alloc(ctx, s->n);
-  if (rc) return sift_stream_fail(s, rc);
+  if (rc) return s->st.fail(rc);
   fs->d_real = fs->d_coor + rows * 2;
   std::vector<void*> dsts; std::vector<const void*> srcs; std::vector<size_t> sizes;
   long long at = 0;
@@ -183,8 +163,8 @@ int pano_sift_stream_finish(pano_sift_stream* s, pano_featureset** out) {
     }
     at += pw.rows;
   }
-  if ((rc = ctx_copy_blocks(ctx, (int)dsts.size(), dsts.data(), srcs.data(), sizes.data()))) return sift_stream_fail(s, rc);
-  if ((rc = ctx_put(ctx, fs->d_count, s->count.data(), s->n * sizeof(int)))) return sift_stream_fail(s, rc);
+  if ((rc = ctx_copy_blocks(ctx, (int)dsts.size(), dsts.data(), srcs.data(), sizes.data()))) return s->st.fail(rc);
+  if ((rc = ctx_put(ctx, fs->d_count, s->count.data(), s->n * sizeof(int)))) return s->st.fail(rc);
   s->packed.clear();   // back to the pool behind the copy
   fs->h_count = s->count;
   fs->counts_on_host = true;
@@ -193,7 +173,7 @@ int pano_sift_stream_finish(pano_sift_stream* s, pano_featureset** out) {
 }
 
 void pano_sift_stream_free(pano_sift_stream* s) {
-  if (s) ctx_enter(s->ctx);
+  if (s) ctx_enter(s->st.ctx);
   delete s;
 }
 

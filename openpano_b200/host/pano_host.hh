@@ -66,6 +66,32 @@ class Context {
   pano_ctx* ctx_ = nullptr;
 };
 
+// Loads refs `window` at a time, hands each window to add(first, count, srcs) and releases it before the next window
+// is loaded, so at most one window of Mat32f is resident on the host.  Mat32f storage is pageable: the streams stage
+// it before add returns.
+template <class Add>
+inline void add_windows(const std::vector<pano::ImageRef*>& refs, int window, Add add) {
+  const int n = (int)refs.size();
+  for (int k0 = 0; k0 < n; k0 += window) {
+    const int k1 = std::min(n, k0 + window);
+    std::vector<const void*> src;
+    for (int k = k0; k < k1; ++k) {
+      refs[k]->load();
+      src.push_back(refs[k]->img->ptr());
+    }
+    add(k0, k1 - k0, src.data());
+    for (int k = k0; k < k1; ++k) refs[k]->release();
+  }
+}
+
+// The blend geometry of a BlenderBase: the projection, its resolution and the range's minimum
+inline pano_blend_geom blend_geom(int projection, Vec2D resolution, Vec2D proj_min) {
+  pano_blend_geom g;
+  g.projection = projection; g.res_x = resolution.x; g.res_y = resolution.y;
+  g.proj_min_x = proj_min.x; g.proj_min_y = proj_min.y;
+  return g;
+}
+
 // ---- features: a FeatureDetector (feature.hh:42-52).  do_detect_feature returns real_coor in
 // [0,1) exactly as SIFTDetector::do_detect_feature does; the non-virtual detect_feature of the
 // base class then applies its own scaling (feature.cc:20-28).
@@ -129,17 +155,11 @@ class B200SIFTDetector : public pano::FeatureDetector {
     pano_params p = snapshot_params();
     pano_sift_stream* s = nullptr;
     c_.check(pano_sift_stream_create(c_.get(), n, w.data(), h.data(), &p, &s));
-    for (int k0 = 0; k0 < n; k0 += window) {
-      const int k1 = std::min(n, k0 + window);
-      std::vector<const void*> src;
-      for (int k = k0; k < k1; ++k) {
-        imgs[k].load();
-        src.push_back(imgs[k].img->ptr());
-      }
-      // Mat32f storage is pageable: the stream stages it before returning
-      c_.check(pano_sift_stream_add(s, k0, k1 - k0, src.data(), PANO_SRC_F32_HOST, 3));
-      for (int k = k0; k < k1; ++k) imgs[k].release();
-    }
+    std::vector<pano::ImageRef*> refs(n);
+    for (int k = 0; k < n; ++k) refs[k] = &imgs[k];
+    add_windows(refs, window, [&](int first, int count, const void* const* src) {
+      c_.check(pano_sift_stream_add(s, first, count, src, PANO_SRC_F32_HOST, 3));
+    });
     pano_featureset* fs = nullptr;
     c_.check(pano_sift_stream_finish(s, &fs));
     pano_sift_stream_free(s);
@@ -224,10 +244,7 @@ class B200PairMatcher {
 class B200Blender : public pano::BlenderBase {
  public:
   B200Blender(const Context& c, int bands, int projection, Vec2D resolution, Vec2D proj_min)
-      : c_(c), bands_(bands) {
-    g_.projection = projection; g_.res_x = resolution.x; g_.res_y = resolution.y;
-    g_.proj_min_x = proj_min.x; g_.proj_min_y = proj_min.y;
-  }
+      : c_(c), bands_(bands), g_(blend_geom(projection, resolution, proj_min)) {}
   void add_image(const Coor& upper_left, const Coor& bottom_right, pano::ImageRef& img, const pano::Homography& homo_inv) {
     img.load();
     pano_blend_image b;
@@ -256,57 +273,64 @@ class B200Blender : public pano::BlenderBase {
 };
 
 // ---- blend with LAZY_READ's memory contract (blender.cc:38-64, multiband.cc:27,49): run() loads the images
-// `window` at a time, hands them to a pano_blend_stream and releases them before the next window, so at most one
-// window of Mat32f is resident on the host and two on the device.  The output is B200Blender's, bit for bit.
-// The stream needs every image's shape up front: each ImageRef must have been loaded once before run() (as
-// calc_feature() does; ImageRef::release keeps the shape).
-class B200LazyBlender : public pano::BlenderBase {
+// `window` at a time (add_windows), hands them to a pano_blend_stream and releases them before the next window, so at
+// most one window of Mat32f is resident on the host and two on the device.  What B200LazyBlender and
+// B200CylinderBlender share; they differ in the stream open() creates.
+class B200StreamBlender : public pano::BlenderBase {
  public:
-  B200LazyBlender(const Context& c, int bands, int projection, Vec2D resolution, Vec2D proj_min, int window = 1)
-      : c_(c), bands_(bands), window_(window < 1 ? 1 : window) {
-    g_.projection = projection; g_.res_x = resolution.x; g_.res_y = resolution.y;
-    g_.proj_min_x = proj_min.x; g_.proj_min_y = proj_min.y;
-  }
-  void add_image(const Coor& upper_left, const Coor& bottom_right, pano::ImageRef& img, const pano::Homography& homo_inv) {
-    pano_blend_image b;
-    b.rgb_hwc = nullptr; b.w = img.width(); b.h = img.height();
-    b.x0 = upper_left.x; b.y0 = upper_left.y; b.x1 = bottom_right.x; b.y1 = bottom_right.y;
-    memcpy(b.homo_inv, homo_inv.data, sizeof(double) * 9);
-    imgs_.push_back(b);
-    refs_.push_back(&img);
-  }
-  void add_image(const Coor&, const Coor&, pano::ImageRef&, std::function<Vec2D(Coor)>) override {
-    error_exit("B200LazyBlender: pass the homography (add_image(ul, br, img, homo_inv)), a closure cannot cross the C ABI");
-  }
   Mat32f run() override {
-    const int n = (int)imgs_.size();
     int ow = 0, oh = 0;
-    c_.check(pano_blend_target_size(n, imgs_.data(), &ow, &oh));
+    c_.check(pano_blend_target_size((int)imgs_.size(), imgs_.data(), &ow, &oh));
     pano_params p = snapshot_params();
-    pano_blend_stream* s = nullptr;
-    c_.check(pano_blend_stream_create(c_.get(), n, imgs_.data(), &g_, bands_, &p, ow, oh, &s));
-    for (int k0 = 0; k0 < n; k0 += window_) {
-      const int k1 = std::min(n, k0 + window_);
-      std::vector<const void*> src;
-      for (int k = k0; k < k1; ++k) {
-        refs_[k]->load();
-        src.push_back(refs_[k]->img->ptr());
-      }
-      // Mat32f storage is pageable: the stream stages it before returning
-      c_.check(pano_blend_stream_add(s, k0, k1 - k0, src.data(), PANO_SRC_F32_HOST, 3));
-      for (int k = k0; k < k1; ++k) refs_[k]->release();
-    }
+    pano_blend_stream* s = open(p, ow, oh);
+    add_windows(refs_, window_, [&](int first, int count, const void* const* src) {
+      c_.check(pano_blend_stream_add(s, first, count, src, PANO_SRC_F32_HOST, 3));
+    });
     Mat32f out(oh, ow, 3);
     c_.check(pano_blend_stream_finish(s, out.ptr()));
     pano_blend_stream_free(s);
     return out;
   }
- private:
+ protected:
+  B200StreamBlender(const Context& c, int bands, int projection, Vec2D resolution, Vec2D proj_min, int window)
+      : c_(c), bands_(bands), window_(window < 1 ? 1 : window), g_(blend_geom(projection, resolution, proj_min)) {}
+  // The image blended as a w×h image over [upper_left, bottom_right] with homo_inv, its source read from img
+  void add(const Coor& upper_left, const Coor& bottom_right, pano::ImageRef& img, const pano::Homography& homo_inv,
+           int w, int h) {
+    pano_blend_image b;
+    b.rgb_hwc = nullptr; b.w = w; b.h = h;
+    b.x0 = upper_left.x; b.y0 = upper_left.y; b.x1 = bottom_right.x; b.y1 = bottom_right.y;
+    memcpy(b.homo_inv, homo_inv.data, sizeof(double) * 9);
+    imgs_.push_back(b);
+    refs_.push_back(&img);
+  }
+  virtual pano_blend_stream* open(const pano_params& p, int ow, int oh) = 0;
+
   const Context& c_;
   int bands_, window_;
   pano_blend_geom g_;
   std::vector<pano_blend_image> imgs_;
   std::vector<pano::ImageRef*> refs_;
+};
+
+// The output is B200Blender's, bit for bit.  The stream needs every image's shape up front: each ImageRef must have
+// been loaded once before run() (as calc_feature() does; ImageRef::release keeps the shape).
+class B200LazyBlender : public B200StreamBlender {
+ public:
+  B200LazyBlender(const Context& c, int bands, int projection, Vec2D resolution, Vec2D proj_min, int window = 1)
+      : B200StreamBlender(c, bands, projection, resolution, proj_min, window) {}
+  void add_image(const Coor& upper_left, const Coor& bottom_right, pano::ImageRef& img, const pano::Homography& homo_inv) {
+    add(upper_left, bottom_right, img, homo_inv, img.width(), img.height());
+  }
+  void add_image(const Coor&, const Coor&, pano::ImageRef&, std::function<Vec2D(Coor)>) override {
+    error_exit("B200LazyBlender: pass the homography (add_image(ul, br, img, homo_inv)), a closure cannot cross the C ABI");
+  }
+ private:
+  pano_blend_stream* open(const pano_params& p, int ow, int oh) override {
+    pano_blend_stream* s = nullptr;
+    c_.check(pano_blend_stream_create(c_.get(), (int)imgs_.size(), imgs_.data(), &g_, bands_, &p, ow, oh, &s));
+    return s;
+  }
 };
 
 // ---- cylinder mode's warp and blend in one (cylstitcher.cc:24-27, 65-67): CylinderWarper(h_factor).warp of every
@@ -315,59 +339,30 @@ class B200LazyBlender : public pano::BlenderBase {
 // the next window; no warped image is made, on the host or the device.  add_image takes the unwarped ImageRef
 // (loaded once before, for its shape) and the range and homo_inv of its warped image; the mosaic is that of
 // LinearBlender / MultiBandBlender over the warped images, bit for bit.
-class B200CylinderBlender : public pano::BlenderBase {
+class B200CylinderBlender : public B200StreamBlender {
  public:
   B200CylinderBlender(const Context& c, int bands, real_t h_factor, Vec2D resolution, Vec2D proj_min, int window = 1)
-      : c_(c), bands_(bands), window_(window < 1 ? 1 : window), h_factor_(h_factor) {
-    g_.projection = PANO_PROJ_FLAT; g_.res_x = resolution.x; g_.res_y = resolution.y;
-    g_.proj_min_x = proj_min.x; g_.proj_min_y = proj_min.y;
-  }
+      : B200StreamBlender(c, bands, PANO_PROJ_FLAT, resolution, proj_min, window), h_factor_(h_factor) {}
   void add_image(const Coor& upper_left, const Coor& bottom_right, pano::ImageRef& img, const pano::Homography& homo_inv) {
     pano_params p = snapshot_params();
-    pano_blend_image b;
+    int w, h;
     double ox, oy;
-    c_.check(pano_cyl_warp_shape(img.width(), img.height(), h_factor_, &p, &b.w, &b.h, &ox, &oy));
-    b.rgb_hwc = nullptr;
-    b.x0 = upper_left.x; b.y0 = upper_left.y; b.x1 = bottom_right.x; b.y1 = bottom_right.y;
-    memcpy(b.homo_inv, homo_inv.data, sizeof(double) * 9);
-    imgs_.push_back(b);
+    c_.check(pano_cyl_warp_shape(img.width(), img.height(), h_factor_, &p, &w, &h, &ox, &oy));
+    add(upper_left, bottom_right, img, homo_inv, w, h);
     src_w_.push_back(img.width()); src_h_.push_back(img.height());
-    refs_.push_back(&img);
   }
   void add_image(const Coor&, const Coor&, pano::ImageRef&, std::function<Vec2D(Coor)>) override {
     error_exit("B200CylinderBlender: pass the homography (add_image(ul, br, img, homo_inv)), a closure cannot cross the C ABI");
   }
-  Mat32f run() override {
-    const int n = (int)imgs_.size();
-    int ow = 0, oh = 0;
-    c_.check(pano_blend_target_size(n, imgs_.data(), &ow, &oh));
-    pano_params p = snapshot_params();
-    pano_blend_stream* s = nullptr;
-    c_.check(pano_blend_stream_create_cyl(c_.get(), n, imgs_.data(), src_w_.data(), src_h_.data(), h_factor_, &g_,
-                                          bands_, &p, ow, oh, &s));
-    for (int k0 = 0; k0 < n; k0 += window_) {
-      const int k1 = std::min(n, k0 + window_);
-      std::vector<const void*> src;
-      for (int k = k0; k < k1; ++k) {
-        refs_[k]->load();
-        src.push_back(refs_[k]->img->ptr());
-      }
-      c_.check(pano_blend_stream_add(s, k0, k1 - k0, src.data(), PANO_SRC_F32_HOST, 3));   // pageable: staged
-      for (int k = k0; k < k1; ++k) refs_[k]->release();
-    }
-    Mat32f out(oh, ow, 3);
-    c_.check(pano_blend_stream_finish(s, out.ptr()));
-    pano_blend_stream_free(s);
-    return out;
-  }
  private:
-  const Context& c_;
-  int bands_, window_;
+  pano_blend_stream* open(const pano_params& p, int ow, int oh) override {
+    pano_blend_stream* s = nullptr;
+    c_.check(pano_blend_stream_create_cyl(c_.get(), (int)imgs_.size(), imgs_.data(), src_w_.data(), src_h_.data(),
+                                          h_factor_, &g_, bands_, &p, ow, oh, &s));
+    return s;
+  }
   real_t h_factor_;
-  pano_blend_geom g_;
-  std::vector<pano_blend_image> imgs_;
   std::vector<int> src_w_, src_h_;
-  std::vector<pano::ImageRef*> refs_;
 };
 
 // ---- cylinder warp: CylinderWarper(h_factor).warp(mat, kpts) (warp.hh:41-66)
