@@ -609,6 +609,49 @@ int  pano_blend_sweep_stats(const pano_blend_sweep* s, long long* uploads, unsig
                             unsigned long long* retained_high);
 void pano_blend_sweep_free(pano_blend_sweep* s);
 
+/* Cylinder mode's output end as a sweep: write_rgb(crop(CylinderStitcher::build())) — the blend of the warped
+ * images (pano_blend_stream_create_cyl, from the UNWARPED sources) followed by perspective_correction
+ * (cylstitcher.cc:139-180) — strip by strip, bit for bit, without the f32 mosaic of the whole canvas.
+ * corr_inv is perspective_correction's `inv` (the caller's getPerspectiveTransform of the four corners, a host
+ * solve like homo_inv): corrected pixel (j, i) is LinearBlender's one-image blend of the mosaic at
+ * inv.trans2d(j, i), with no centre shift and no z test, under LAZY_READ's branch as p selects it.  The corrected
+ * canvas has the mosaic's out_w×out_h.
+ *
+ * Strip s covers corrected rows [s * strip_rows, min(out_h, (s + 1) * strip_rows)) and blends the band of mosaic
+ * rows [b0, b1) its bilinear taps can read: where z keeps one sign at the strip's four corner pixels, the rows
+ * between floor(min y) and floor(max y) + 1 over those corners, widened by one row on each side and clamped to the
+ * mosaic (empty when no tap can land on it); where z changes sign, the whole mosaic.  The band's rows are the
+ * mosaic's rows of a row-strip stream, bit for bit, for multiband too.  The images a strip reads are those such a
+ * stream of its band reads, and the sources are planned over them as for pano_blend_sweep_plan.
+ *
+ * pano_blend_sweep_plan_cyl: pano_blend_sweep_plan's arguments and outputs plus corr_inv (required) and band
+ * (2 ints per strip, {b0, b1}; may be NULL).  No device needed.
+ *
+ * pano_blend_sweep_create_cyl: imgs / g / bands / p / out_w / out_h as for pano_blend over the WARPED images;
+ * src_w / src_h / h_factor as for pano_blend_stream_create_cyl, which validates them the same way; corr_inv,
+ * strip_rows, src_bytes, keep_bytes and crop as above and for pano_blend_sweep_create, with src_bytes NULL meaning
+ * src_w·src_h·3 per source.  It returns an ordinary sweep: next / strip / finish_dev / stats / free as above,
+ * with the UNWARPED sources handed to strip.
+ *
+ * Device memory, besides the per-image table and the projection tables:
+ *   - the tallest band's row-stream state (pano_blend_stream_create_rows of the band's rows), and 12 B per band
+ *     pixel of its f32 rows;
+ *   - 12 B per strip pixel of the corrected rows;
+ *   - 3 B per canvas pixel (the 8-bit canvas) plus the output's bytes per canvas pixel;
+ *   - the two-slot ring and the kept sources, as for pano_blend_sweep_create;
+ *   - 16 B per warped column per image (the warps' column tables, built once). */
+int  pano_blend_sweep_plan_cyl(int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
+                               const pano_params* p, int out_w, int out_h, const double corr_inv[9], int strip_rows,
+                               const size_t* src_bytes, size_t keep_bytes, int* n_strips, int* band,
+                               unsigned char* reads, unsigned char* uploads, unsigned char* kept,
+                               long long* n_uploads, unsigned long long* upload_bytes,
+                               unsigned long long* retained_high);
+int  pano_blend_sweep_create_cyl(pano_ctx* ctx, int n, const pano_blend_image* imgs, const int* src_w,
+                                 const int* src_h, double h_factor, const pano_blend_geom* g, int bands,
+                                 const pano_params* p, int out_w, int out_h, const double corr_inv[9],
+                                 int strip_rows, const size_t* src_bytes, size_t keep_bytes, int crop,
+                                 pano_blend_sweep** out);
+
 /* SIFT whose sources arrive in windows: LAZY_READ's feature stage (config.cfg:10-11, calc_feature in
  * stitcherbase.cc:9-27 loads, detects and releases one image at a time) on the device.  For every
  * partition of the images into windows and every source kind, the featureset from pano_sift_stream_finish

@@ -128,6 +128,14 @@ def _load():
         "pano_blend_sweep_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_longlong), C.POINTER(C.c_ulonglong),
                                              C.POINTER(C.c_ulonglong)]),
         "pano_blend_sweep_free": (None, [C.c_void_p]),
+        "pano_blend_sweep_plan_cyl": (C.c_int, [C.c_int, C.POINTER(PanoBlendImage), C.POINTER(PanoBlendGeom), C.c_int,
+                                                P, C.c_int, C.c_int, _dp, C.c_int, C.POINTER(C.c_size_t), C.c_size_t,
+                                                _ip, _ip, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.POINTER(C.c_longlong), C.POINTER(C.c_ulonglong),
+                                                C.POINTER(C.c_ulonglong)]),
+        "pano_blend_sweep_create_cyl": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(PanoBlendImage), _ip, _ip,
+                                                  C.c_double, C.POINTER(PanoBlendGeom), C.c_int, P, C.c_int, C.c_int,
+                                                  _dp, C.c_int, C.POINTER(C.c_size_t), C.c_size_t, C.c_int, _vpp]),
         "pano_sift_stream_create": (C.c_int, [C.c_void_p, C.c_int, _ip, _ip, P, _vpp]),
         "pano_sift_stream_add": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _vpp, C.c_int, C.c_int]),
         "pano_sift_stream_finish": (C.c_int, [C.c_void_p, _vpp]),
@@ -492,6 +500,31 @@ def blend_sweep_plan(shapes, items, geom, bands, strip_rows, src_bytes, keep_byt
     reads, uploads, kept = (f[:S * n].reshape(S, n).astype(bool) for f in flags)
     return {"reads": reads, "uploads": uploads, "kept": kept, "n_uploads": nu.value, "upload_bytes": ub.value,
             "retained_high": rh.value}
+
+
+def blend_sweep_plan_cyl(shapes, items, geom, bands, corr_inv, strip_rows, src_bytes, keep_bytes, params=None):
+    """pano_blend_sweep_plan_cyl (no device needed): blend_sweep_plan's schedule of a cylinder sweep whose
+    perspective correction is corr_inv (3×3, row-major).  shapes / items / geom are the WARPED images'.  The dict
+    also has "band", a strips × 2 int array of the mosaic rows [b0, b1) each strip blends."""
+    params = params or default_params()
+    n = len(items)
+    arr, g = Engine._blend_args([None] * n, shapes, items, geom)
+    ow, oh = max(it[2] for it in items), max(it[3] for it in items)
+    S = -(-oh // strip_rows) if strip_rows > 0 else 0
+    flags = [np.zeros(max(S * n, 1), np.uint8) for _ in range(3)]
+    band = np.zeros(max(2 * S, 1), np.int32)
+    inv = np.ascontiguousarray(np.asarray(corr_inv, np.float64).reshape(9))
+    nb = (C.c_size_t * n)(*[int(b) for b in src_bytes])
+    ns, nu = C.c_int(), C.c_longlong()
+    ub, rh = C.c_ulonglong(), C.c_ulonglong()
+    rc = LIB.pano_blend_sweep_plan_cyl(n, arr, C.byref(g), bands, C.byref(params), ow, oh, _d(inv), strip_rows, nb,
+                                       min(int(keep_bytes), SIZE_MAX), C.byref(ns), _i(band),
+                                       *(f.ctypes.data for f in flags), C.byref(nu), C.byref(ub), C.byref(rh))
+    if rc != 0:
+        raise PanoError(rc, "cylinder blend sweep plan: bad argument")
+    reads, uploads, kept = (f[:S * n].reshape(S, n).astype(bool) for f in flags)
+    return {"band": band[:2 * S].reshape(S, 2), "reads": reads, "uploads": uploads, "kept": kept,
+            "n_uploads": nu.value, "upload_bytes": ub.value, "retained_high": rh.value}
 
 
 class BlendSweep(_Handle):
@@ -1083,6 +1116,34 @@ class Engine:
         self._check(LIB.pano_blend_sweep_create(self._h, n, arr, C.byref(g), bands, C.byref(params), ow.value, oh.value,
                                                 strip_rows, nb, min(int(keep_bytes), SIZE_MAX), 1 if crop else 0,
                                                 C.byref(h)))
+        return BlendSweep(self, h, n, ow.value, oh.value)
+
+    def blend_sweep_cyl(self, src_shapes, items, geom, h_factor, corr_inv, strip_rows, keep_bytes, bands=0,
+                        params=None, crop=True, src_bytes=None) -> BlendSweep:
+        """A cylinder sweep (pano_blend_sweep_create_cyl): write_rgb(crop(perspective_correction(mosaic))) of the
+        mosaic blend_stream_cyl gives, strip by strip.  src_shapes: the UNWARPED sources' (h, w); items / geom: the
+        warped images'; corr_inv: perspective_correction's inv (3×3, row-major); src_bytes: each source's bytes
+        (None: h·w·3).  strip() takes the unwarped sources."""
+        params = params or default_params()
+        n = len(items)
+        shapes = []
+        for h, w in src_shapes:
+            try:
+                ow, oh, _, _ = self.cyl_warp_shape(w, h, h_factor, params)
+            except PanoError:
+                ow, oh = 0, 0
+            shapes.append((oh, ow))
+        arr, g = self._blend_args([None] * n, shapes, items, geom)
+        ow, oh = C.c_int(), C.c_int()
+        self._check(LIB.pano_blend_target_size(n, arr, C.byref(ow), C.byref(oh)))
+        sw = (C.c_int * max(n, 1))(*[int(s[1]) for s in src_shapes])
+        sh = (C.c_int * max(n, 1))(*[int(s[0]) for s in src_shapes])
+        inv = np.ascontiguousarray(np.asarray(corr_inv, np.float64).reshape(9))
+        nb = (C.c_size_t * n)(*[int(b) for b in src_bytes]) if src_bytes is not None else None
+        h = C.c_void_p()
+        self._check(LIB.pano_blend_sweep_create_cyl(self._h, n, arr, sw, sh, h_factor, C.byref(g), bands,
+                                                    C.byref(params), ow.value, oh.value, _d(inv), strip_rows, nb,
+                                                    min(int(keep_bytes), SIZE_MAX), 1 if crop else 0, C.byref(h)))
         return BlendSweep(self, h, n, ow.value, oh.value)
 
     def blend_lazy(self, imgs, items, geom, bands=0, params=None, window=1, fmt=None):

@@ -186,6 +186,51 @@ __global__ void k_linear_resolve(const float* sum, const float* __restrict__ wsu
   linear_resolve_px(lazy, p[0], p[1], p[2], wsum[t], out + t * 3);
 }
 
+// Cylinder mode's perspective correction (cylstitcher.cc:139-180): a LinearBlender of the one image, the w×h
+// mosaic, over ROI (0, 0)–(w, h) with the map inv.trans2d(c) (homography.hh:60-76) — no centre shift, no z test.
+// One thread per pixel of output rows [row0, row1); `out` starts at row0.  Every output pixel lies in the ROI under
+// both range rules, so the pixel is linear_add_px's one-image case; the taps come from the mosaic rows the band
+// reader holds, judged against the whole mosaic's w×h.
+struct PerspMap { double d[9]; };
+
+template <class Src>
+__global__ void k_persp_correct(BandImg band, PerspMap m, int w, int h, int lazy, int ordered, float* __restrict__ out,
+                                int row0, int row1) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  const int i = row0 + blockIdx.y * blockDim.y + threadIdx.y;
+  if (j >= w || i >= row1) return;
+  const double cx = (double)j, cy = (double)i;
+  const double rx = m.d[0] * cx + m.d[1] * cy + m.d[2] * 1.0;
+  const double ry = m.d[3] * cx + m.d[4] * cy + m.d[5] * 1.0;
+  const double rz = m.d[6] * cx + m.d[7] * cy + m.d[8] * 1.0;
+  const double denom = 1.0 / rz;
+  const double x = rx * denom, y = ry * denom;
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f, wsum = 0.f;
+  if (!(x < 0 || x >= w || y < 0 || y >= h)) {                       // map_coor -> NaN
+    const float r = (float)y, c = (float)x;
+    float c0, c1, c2;
+    if (interpolate_rgb(Src::at(&band, w, h, 3, nullptr), w, h, r, c, &c0, &c1, &c2) && !(c0 < 0)) {
+      float wt = (float)(0.5 - fabs((double)(c / (float)w) - 0.5));
+      if (!ordered) wt = (float)((double)wt * (0.5 - fabs((double)(r / (float)h) - 0.5)));
+      s0 += c0 * wt; s1 += c1 * wt; s2 += c2 * wt;
+      wsum += wt;
+    }
+  }
+  linear_resolve_px(lazy, s0, s1, s2, wsum, out + ((size_t)(i - row0) * w + j) * 3);
+}
+
+int persp_correct_rows(pano_ctx* ctx, const float* d_band, int b0, const double inv[9], int w, int h,
+                       const pano_params* p, float* d_out, int row0, int row1) {
+  if (row0 >= row1) return PANO_OK;
+  PerspMap m;
+  memcpy(m.d, inv, sizeof(m.d));
+  const BandImg band{d_band, b0};
+  const dim3 b(32, 8), g(ceil_div(w, 32), ceil_div(row1 - row0, 8));
+  PANO_LAUNCH(ctx, src_name<SrcBand>(SRC_NAMES("k_persp_correct")), k_persp_correct<SrcBand>, g, b, 0, band, m, w, h,
+              p->lazy_read, p->ordered_input, d_out, row0, row1);
+  return PANO_OK;
+}
+
 // ============================================================ multiband
 // multiband.cc:19-57 create_first_level
 // The first level of an image depends on that image only: a blend stream runs this once per
@@ -836,6 +881,62 @@ int blend_sweep_tables(pano_ctx* ctx, int n, const pano_blend_image* imgs, const
   return PANO_OK;
 }
 
+int cyl_tabs(pano_ctx* ctx, int n, const pano_blend_image* imgs, const int* src_w, const int* src_h, double h_factor,
+             const pano_params* p, CylTabs* ct) {
+  if (n <= 0 || !imgs || !src_w || !src_h || !p)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder blend stream: bad argument");
+  if (n > PANO_MAX_IMAGES)
+    return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: %d images (limit %d)", n, PANO_MAX_IMAGES);
+  // the warp of every source (host arithmetic, as pano_cyl_warp_batch_dev does it) must be the image blended
+  ct->maps.resize(n);
+  ct->off.resize(n);
+  ct->w.assign(src_w, src_w + n);
+  ct->h.assign(src_h, src_h + n);
+  ct->tabs.clear();
+  for (int k = 0; k < n; ++k) {
+    if (src_w[k] < 2 || src_h[k] < 2)
+      return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder blend stream: source %d is %dx%d, under 2x2", k, src_w[k],
+                      src_h[k]);
+    ct->off[k] = ct->tabs.size();
+    if (!cyl_map(src_w[k], src_h[k], h_factor, p, nullptr, 0, &ct->maps[k], &ct->tabs))
+      return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder radius <= 0");
+    if (ct->maps[k].ow != imgs[k].w || ct->maps[k].oh != imgs[k].h)
+      return ctx_fail(ctx, PANO_ERR_INVALID,
+                      "cylinder blend stream: image %d is %dx%d but its %dx%d source warps to %dx%d", k, imgs[k].w,
+                      imgs[k].h, src_w[k], src_h[k], ct->maps[k].ow, ct->maps[k].oh);
+  }
+  return PANO_OK;
+}
+
+int blend_stream_open_cyl(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
+                          const pano_params* p, int ow, int oh, int row0, int row1, const double* shared_tab,
+                          const CylTabs& ct, const double* d_cyl_tab, pano_blend_stream** out) {
+  pano_blend_stream* raw = nullptr;
+  if (int rc = blend_stream_open(ctx, n, imgs, g, bands, p, ow, oh, row0, row1, shared_tab, &raw)) return rc;
+  std::unique_ptr<pano_blend_stream> s(raw);
+  const size_t ne = s->job.imgs.size();
+  int rc = 0;
+  if (!d_cyl_tab) {
+    if ((rc = s->d_cyl_tab.alloc(ctx, std::max<size_t>(ct.tabs.size(), 1)))) return rc;
+    if ((rc = ctx_put(ctx, s->d_cyl_tab, ct.tabs.data(), ct.tabs.size() * sizeof(double)))) return rc;
+    d_cyl_tab = s->d_cyl_tab;
+  }
+  if ((rc = s->d_cyl.alloc(ctx, std::max<size_t>(ne, 1)))) return rc;
+  s->cyl.resize(ne);
+  for (size_t q = 0; q < ne; ++q) {
+    const int k = s->job.src[q];
+    const CylMap& m = ct.maps[k];
+    CylImg& c = s->cyl[q];
+    memset(&c, 0, sizeof(c));
+    c.w = ct.w[k]; c.h = ct.h[k];
+    c.col_x = d_cyl_tab + ct.off[k];
+    c.col_cos = c.col_x + m.ow;
+    c.r = m.r; c.cy = m.cy; c.offy = m.offy; c.sizefactor_inv = m.sizefactor_inv;
+  }
+  *out = s.release();
+  return PANO_OK;
+}
+
 extern "C" {
 
 int pano_blend_target_size(int n, const pano_blend_image* imgs, int* ow, int* oh) {
@@ -895,47 +996,9 @@ int pano_blend_stream_create_cyl(pano_ctx* ctx, int n, const pano_blend_image* i
   ctx_enter(ctx);
   if (!ctx || !out) return PANO_ERR_INVALID;
   *out = nullptr;
-  if (n <= 0 || !imgs || !src_w || !src_h || !p)
-    return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder blend stream: bad argument");
-  if (n > PANO_MAX_IMAGES)
-    return ctx_fail(ctx, PANO_ERR_INVALID, "blend stream: %d images (limit %d)", n, PANO_MAX_IMAGES);
-  // the warp of every source (host arithmetic, as pano_cyl_warp_batch_dev does it) must be the image blended
-  std::vector<CylMap> maps(n);
-  std::vector<size_t> tab_off(n);
-  std::vector<double> tabs;
-  for (int k = 0; k < n; ++k) {
-    if (src_w[k] < 2 || src_h[k] < 2)
-      return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder blend stream: source %d is %dx%d, under 2x2", k, src_w[k],
-                      src_h[k]);
-    tab_off[k] = tabs.size();
-    if (!cyl_map(src_w[k], src_h[k], h_factor, p, nullptr, 0, &maps[k], &tabs))
-      return ctx_fail(ctx, PANO_ERR_INVALID, "cylinder radius <= 0");
-    if (maps[k].ow != imgs[k].w || maps[k].oh != imgs[k].h)
-      return ctx_fail(ctx, PANO_ERR_INVALID,
-                      "cylinder blend stream: image %d is %dx%d but its %dx%d source warps to %dx%d", k, imgs[k].w,
-                      imgs[k].h, src_w[k], src_h[k], maps[k].ow, maps[k].oh);
-  }
-  pano_blend_stream* raw = nullptr;
-  if (int rc = blend_stream_open(ctx, n, imgs, g, bands, p, ow, oh, 0, oh, nullptr, &raw)) return rc;
-  std::unique_ptr<pano_blend_stream> s(raw);
-  const size_t ne = s->job.imgs.size();
-  int rc = 0;
-  if ((rc = s->d_cyl_tab.alloc(ctx, std::max<size_t>(tabs.size(), 1))) ||
-      (rc = s->d_cyl.alloc(ctx, std::max<size_t>(ne, 1))))
-    return rc;
-  if ((rc = ctx_put(ctx, s->d_cyl_tab, tabs.data(), tabs.size() * sizeof(double)))) return rc;
-  s->cyl.resize(ne);
-  for (size_t q = 0; q < ne; ++q) {
-    const int k = s->job.src[q];
-    CylImg& c = s->cyl[q];
-    memset(&c, 0, sizeof(c));
-    c.w = src_w[k]; c.h = src_h[k];
-    c.col_x = s->d_cyl_tab + tab_off[k];
-    c.col_cos = c.col_x + maps[k].ow;
-    c.r = maps[k].r; c.cy = maps[k].cy; c.offy = maps[k].offy; c.sizefactor_inv = maps[k].sizefactor_inv;
-  }
-  *out = s.release();
-  return PANO_OK;
+  CylTabs ct;
+  if (int rc = cyl_tabs(ctx, n, imgs, src_w, src_h, h_factor, p, &ct)) return rc;
+  return blend_stream_open_cyl(ctx, n, imgs, g, bands, p, ow, oh, 0, oh, nullptr, ct, nullptr, out);
 }
 
 int pano_blend_stream_needs(const pano_blend_stream* s, unsigned char* flags) {

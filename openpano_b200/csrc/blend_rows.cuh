@@ -20,3 +20,25 @@ int blend_stream_open(pano_ctx* ctx, int n, const pano_blend_image* imgs, const 
 // tables (empty for the flat projection).
 int blend_sweep_tables(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
                        const pano_params* p, int ow, int oh, std::vector<double>* tab);
+// Cylinder mode's perspective correction of output rows [row0, row1) of a w×h canvas (cylstitcher.cc:139-180, with
+// inv its `inv`) into d_out (from row0 on), the mosaic's rows [b0, b0 + band rows) in d_band.  The band must hold
+// every row persp_band gives for these rows.
+int persp_correct_rows(pano_ctx* ctx, const float* d_band, int b0, const double inv[9], int w, int h,
+                       const pano_params* p, float* d_out, int row0, int row1);
+// The cylinder warps of a cylinder stream's sources (pano_blend_stream_create_cyl): each source's shape, its
+// inverse map and the offset of its column tables in `tabs` (col_x then col_cos, 16 B per warped column).
+struct CylTabs {
+  std::vector<CylMap> maps;
+  std::vector<size_t> off;
+  std::vector<int> w, h;
+  std::vector<double> tabs;
+};
+// Validates the sources as pano_blend_stream_create_cyl does (every warp must have imgs[k]'s shape) and builds
+// their tables.
+int cyl_tabs(pano_ctx* ctx, int n, const pano_blend_image* imgs, const int* src_w, const int* src_h, double h_factor,
+             const pano_params* p, CylTabs* ct);
+// blend_stream_open for rows [row0, row1) of a cylinder stream over ct's sources.  d_cyl_tab: ct.tabs on the
+// device, shared by many streams, or null to upload them for this stream.
+int blend_stream_open_cyl(pano_ctx* ctx, int n, const pano_blend_image* imgs, const pano_blend_geom* g, int bands,
+                          const pano_params* p, int ow, int oh, int row0, int row1, const double* shared_tab,
+                          const CylTabs& ct, const double* d_cyl_tab, pano_blend_stream** out);

@@ -663,10 +663,33 @@ struct SrcCyl {
   }
 };
 
-// The profile name of a kernel templated on its reader: SRC_NAMES(base) lists the six names in kName order, and
+// Rows [b0, b0 + rows) of an h-row f32 image (cylinder mode's mosaic band, blend_sweep.cu): `rows` holds them
+// h×w×3 from row b0 on, and the reader is handed row numbers of the whole image.  The caller reads rows of the band
+// only.
+struct BandImg {
+  const float* rows;
+  int b0;
+};
+struct SrcBand {
+  const float* img;   // row b0 of the whole image
+  int b0;
+  static constexpr bool kMayBeNo = true, kLut = false;
+  static constexpr int kName = 6;
+  // px: the BandImg
+  static __device__ __forceinline__ SrcBand at(const void* px, int, int, int, const float*) {
+    const BandImg* b = static_cast<const BandImg*>(px);
+    return SrcBand{b->rows, b->b0};
+  }
+  __device__ __forceinline__ void fetch(int w, int fr, int fc, float* q) const {
+    SrcF32{img + (size_t)(fr - b0) * w * 3}.fetch(w, 0, fc, q);
+  }
+};
+
+// The profile name of a kernel templated on its reader: SRC_NAMES(base) lists the seven names in kName order, and
 // src_name<Src> picks one.  They are literals because the profiler keeps the pointer until it drains.
-#define SRC_NAMES(base) {base, base "_rgb8", base "_pix8", base "_cyl", base "_cyl_rgb8", base "_cyl_pix8"}
-template <class Src> static inline const char* src_name(const char* const (&names)[6]) { return names[Src::kName]; }
+#define SRC_NAMES(base) \
+  {base, base "_rgb8", base "_pix8", base "_cyl", base "_cyl_rgb8", base "_cyl_pix8", base "_band"}
+template <class Src> static inline const char* src_name(const char* const (&names)[7]) { return names[Src::kName]; }
 
 // The reader of a set of formats: F32 for f32 sources (fmts null), PIX8 when one of the n formats is RGBA or
 // planar, else RGB8.  with_reader(r, f) calls f(ReaderTag<Src>{}) for r's reader type Src.

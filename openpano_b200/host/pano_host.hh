@@ -31,6 +31,8 @@
 #include "stitch/homography.hh"
 #include "stitch/camera.hh"
 #include "stitch/match_info.hh"
+#include "stitch/stitcher_image.hh"
+#include "lib/imgproc.hh"
 
 namespace pano_b200 {
 
@@ -333,6 +335,34 @@ class B200LazyBlender : public B200StreamBlender {
   }
 };
 
+// ---- the two point sets of perspective_correction's getPerspectiveTransform (cylstitcher.cc:139-168): the corners
+// of the bundle's first and last images (their half-extents ±0.5 of the WARPED shape first_w×first_h and
+// last_w×last_h, through the image's homo, normalised by the identity image's warped shape ref_w×ref_h, projected
+// with the bundle's homo2proj, scaled back and moved by -proj_range.min), in the order (-,-) (-,+) of the first and
+// (+,-) (+,+) of the last; and the w×h mosaic's corners (0,0), (0,h), (w,0), (w,h) they are stretched to.  The same
+// double operations in the same order as the reference, so the points, and the homography solved from them, are
+// its bits.
+inline void b200_correction_points(const pano::ConnectedImages& bundle, int ref_w, int ref_h, int first_w, int first_h,
+                                   int last_w, int last_h, int w, int h, std::vector<Vec2D>* corners,
+                                   std::vector<Vec2D>* targets) {
+  const auto homo2proj = bundle.get_homo2proj();
+  const Vec2D proj_min = bundle.proj_range.min;
+  const pano::Homography* homo[2] = {&bundle.component.front().homo, &bundle.component.back().homo};
+  const int sw[2] = {first_w, last_w}, sh[2] = {first_h, last_h};
+  const double fx[4] = {-0.5, -0.5, 0.5, 0.5}, fy[4] = {-0.5, 0.5, -0.5, 0.5};
+  corners->clear();
+  for (int q = 0; q < 4; ++q) {
+    Vec2D v(fx[q], fy[q]);
+    v.x *= sw[q / 2], v.y *= sh[q / 2];
+    Vec p = homo[q / 2]->trans(v);
+    p.x /= ref_w, p.y /= ref_h;
+    Vec2D c = homo2proj(p);
+    c.x *= ref_w, c.y *= ref_h;
+    corners->push_back(c - proj_min);
+  }
+  *targets = {Vec2D(0, 0), Vec2D(0, h), Vec2D(w, 0), Vec2D(w, h)};
+}
+
 // ---- cylinder mode's warp and blend in one (cylstitcher.cc:24-27, 65-67): CylinderWarper(h_factor).warp of every
 // image followed by the flat-projection blend of ConnectedImages::blend, from the UNWARPED images.  run() loads
 // them `window` at a time into a cylinder blend stream (pano_blend_stream_create_cyl) and releases them before
@@ -354,6 +384,32 @@ class B200CylinderBlender : public B200StreamBlender {
   void add_image(const Coor&, const Coor&, pano::ImageRef&, std::function<Vec2D(Coor)>) override {
     error_exit("B200CylinderBlender: pass the homography (add_image(ul, br, img, homo_inv)), a closure cannot cross the C ABI");
   }
+  // main.cc:226-233 on CylinderStitcher::build()'s result — crop() when `crop`, then write_rgb(fname) of
+  // perspective_correction(run()) — without the f32 mosaic: a cylinder sweep (pano_blend_sweep_create_cyl) of `rows`
+  // corrected rows per strip, each blending the band of mosaic rows its correction reads from the unwarped images.
+  // corr_inv is perspective_correction's `inv` (cylstitcher.cc:144-168: the four corners of the bundle's first and
+  // last images in the identity frame, then getPerspectiveTransform to the w×h rectangle, w×h run()'s shape): a host
+  // solve the caller makes, as it makes homo_inv.  An image is loaded (ImageRef::load) for each upload the sweep's
+  // plan asks for and released after that strip; keep_bytes bounds the f32 sources kept on the device between
+  // strips (SIZE_MAX: no limit).  The file is write_rgb's, byte for byte.  Defined in pano_host_io.hh.
+  void write_sweep(const pano::Homography& corr_inv, int rows, size_t keep_bytes, bool crop, const char* fname);
+  // write_sweep with perspective_correction's own inv: the bundle CylinderStitcher::build blends (its components in
+  // add_image's order, identity_idx, proj_range, the flat projection), the corner points b200_correction_points
+  // gives for the warped shapes of add_image's images, and the reference's getPerspectiveTransform
+  // (lib/imgproc.cc:251) of them.  The file is write_rgb(crop(CylinderStitcher::build()))'s, byte for byte.
+  void write_sweep(const pano::ConnectedImages& bundle, int rows, size_t keep_bytes, bool crop, const char* fname) {
+    const int n = (int)imgs_.size();
+    m_assert(n > 0 && (int)bundle.component.size() == n && bundle.identity_idx >= 0 && bundle.identity_idx < n);
+    int ow = 0, oh = 0;
+    c_.check(pano_blend_target_size(n, imgs_.data(), &ow, &oh));
+    const pano_blend_image &ref = imgs_[bundle.identity_idx], &first = imgs_.front(), &last = imgs_.back();
+    std::vector<Vec2D> corners, targets;
+    b200_correction_points(bundle, ref.w, ref.h, first.w, first.h, last.w, last.h, ow, oh, &corners, &targets);
+    write_sweep(pano::Homography(pano::getPerspectiveTransform(corners, targets)), rows, keep_bytes, crop, fname);
+  }
+  // the uploads and loads of the last write_sweep
+  long long last_sweep_uploads() const { return last_sweep_uploads_; }
+  long last_sweep_loads() const { return last_sweep_loads_; }
  private:
   pano_blend_stream* open(const pano_params& p, int ow, int oh) override {
     pano_blend_stream* s = nullptr;
@@ -363,6 +419,8 @@ class B200CylinderBlender : public B200StreamBlender {
   }
   real_t h_factor_;
   std::vector<int> src_w_, src_h_;
+  long long last_sweep_uploads_ = 0;
+  long last_sweep_loads_ = 0;
 };
 
 // ---- cylinder warp: CylinderWarper(h_factor).warp(mat, kpts) (warp.hh:41-66)

@@ -11,6 +11,9 @@
 //   B200PixelBlender::write_sweep
 //                     the same from one blend sweep: each source is decoded and uploaded once while later strips
 //                     read it (within a byte budget), files decoded on demand
+//   B200CylinderBlender::write_sweep
+//                     cylinder mode's crop + write_rgb of main.cc:226-233 on CylinderStitcher::build()'s
+//                     perspective-corrected mosaic, from one cylinder sweep of the unwarped images
 //   b200_planet       planet() of main.cc:294-331 from load_pixels' buffer, left on the device for write_mosaic
 // The buffers go to B200SIFTDetector::detect_batch_rgb8, B200PixelBlender or the streams (pano_b200.h) with
 // their format as the `channels` argument; no Mat32f of a source is built.  Include after the reference's
@@ -271,6 +274,50 @@ class B200PixelBlender {
   long decodes_ = 0;
   long long last_sweep_uploads_ = 0;
 };
+
+inline void B200CylinderBlender::write_sweep(const pano::Homography& corr_inv, int rows, size_t keep_bytes, bool crop,
+                                             const char* fname) {
+  const int n = (int)imgs_.size();
+  int ow = 0, oh = 0;
+  c_.check(pano_blend_target_size(n, imgs_.data(), &ow, &oh));
+  const bool png = endswith(fname, ".png");
+  pano_params p = snapshot_params();
+  std::vector<size_t> bytes(n);
+  for (int k = 0; k < n; ++k) bytes[k] = (size_t)src_w_[k] * src_h_[k] * 3 * sizeof(float);
+  pano_blend_sweep* s = nullptr;
+  c_.check(pano_blend_sweep_create_cyl(c_.get(), n, imgs_.data(), src_w_.data(), src_h_.data(), h_factor_, &g_, bands_,
+                                       &p, ow, oh, corr_inv.data, std::max(rows, 1), bytes.data(), keep_bytes,
+                                       crop ? 1 : 0, &s));
+  std::vector<unsigned char> want(n);
+  std::vector<const void*> src(n);
+  std::vector<int> fmt(n, 3);
+  int st = 0;
+  last_sweep_loads_ = 0;
+  while ((st = pano_blend_sweep_next(s, want.data())) >= 0) {
+    for (int k = 0; k < n; ++k) {
+      src[k] = nullptr;
+      if (!want[k]) continue;
+      refs_[k]->load();
+      ++last_sweep_loads_;
+      m_assert(refs_[k]->width() == src_w_[k] && refs_[k]->height() == src_h_[k]);
+      src[k] = refs_[k]->img->ptr();
+    }
+    c_.check(pano_blend_sweep_strip(s, src.data(), fmt.data(), PANO_SRC_F32_HOST));
+    for (int k = 0; k < n; ++k)   // pageable: staged by the call
+      if (want[k]) refs_[k]->release();
+  }
+  if (st < -1) c_.check(st);
+  void* d_out = nullptr;
+  int rect[4] = {0, 0, ow, oh};
+  c_.check(pano_dev_alloc(c_.get(), (size_t)ow * oh * (png ? 4 : 3), &d_out));
+  c_.check(pano_blend_sweep_finish_dev(s, png ? PANO_PIX_RGBA : PANO_PIX_RGB_PLANAR, (unsigned char*)d_out, rect));
+  std::vector<unsigned char> buf((size_t)rect[2] * rect[3] * (png ? 4 : 3));
+  if (!buf.empty()) c_.check(pano_dev_download(c_.get(), buf.data(), d_out, buf.size()));
+  c_.check(pano_dev_free(c_.get(), d_out));
+  c_.check(pano_blend_sweep_stats(s, &last_sweep_uploads_, nullptr, nullptr));
+  pano_blend_sweep_free(s);
+  encode_mosaic(fname, buf, rect[2], rect[3]);
+}
 
 // main.cc:226-234 on a device mosaic (h×w×3 f32, Color::NO < 0): crop() when `crop`, then write_rgb(fname).
 // The conversion runs on the device into the encoder's layout; the file is what write_rgb writes, byte for byte.

@@ -394,19 +394,11 @@ def mosaic_rgb8_strips(engine: Engine, items, geom, bands, sources, strip_rows, 
 _PIX_BYTES = {1: 1, 3: 3, PIX_RGBA: 4, PIX_RGB_PLANAR: 3}
 
 
-def mosaic_rgb8_sweep(engine: Engine, items, geom, bands, sources, strip_rows, keep_bytes, out_format="rgb", crop=True,
-                      params=None, kind=None, formats=None, shapes=None, fmt=None, stats=None):
-    """mosaic_rgb8_strips' bytes from one blend sweep (Engine.blend_sweep): the strips run top to bottom and each
-    source is handed over once while a later strip still reads it, keeping at most keep_bytes of sources between
-    strips (capi.SIZE_MAX: no limit; 0 hands over every source each strip reads).
-
-    sources: numpy arrays (host, pageable: uint8 read in layout `fmt`, one value or one per image, or float32
-    H×W×3), or pointers of source kind `kind` with PANO_PIX_* codes `formats` (one per image; None: 3) and `shapes`
-    [(h, w)].  Device memory holds one strip's blend state and f32 rows, two sources in the upload ring, the kept
-    sources, and 3 + 3 (4 for "rgba") bytes per canvas pixel.  stats: a dict that receives
-    "uploads", "upload_bytes" and "retained_high" (pano_blend_sweep_stats).  Returns (rect or None, pixels) as
-    mosaic_rgb8_strips does."""
-    n = len(items)
+def _sweep_sources(sources, n, kind, formats, shapes, fmt):
+    """A sweep's sources as (kind, formats, shapes, sources, bytes): numpy arrays (host, pageable: uint8 read in
+    layout `fmt`, one value or one per image, or float32 H×W×3), or pointers of kind `kind` with PANO_PIX_* codes
+    `formats` (None: 3) and `shapes` [(h, w)].  The sources returned are the C-contiguous arrays the sweep reads
+    (copies of the others) or the pointers: the caller holds them until the sweep has run."""
     if kind is None:
         arrs = [np.ascontiguousarray(a) for a in sources]
         u8 = arrs[0].dtype == np.uint8
@@ -416,16 +408,19 @@ def mosaic_rgb8_sweep(engine: Engine, items, geom, bands, sources, strip_rows, k
         else:
             formats, shapes = [3] * n, [a.shape[:2] for a in arrs]
         kind = SRC_RGB8_HOST if u8 else SRC_F32_HOST
-        ptrs, nbytes = [a.ctypes.data for a in arrs], [a.nbytes for a in arrs]
-    else:
-        u8 = kind in (SRC_RGB8_DEV, SRC_RGB8_HOST)
-        formats = list(formats) if formats is not None else [3] * n
-        ptrs = list(sources)
-        nbytes = [h * w * (_PIX_BYTES[f] if u8 else 12) for (h, w), f in zip(shapes, formats)]
-    ow, oh = max(it[2] for it in items), max(it[3] for it in items)
+        return kind, formats, shapes, arrs, [a.nbytes for a in arrs]
+    u8 = kind in (SRC_RGB8_DEV, SRC_RGB8_HOST)
+    formats = list(formats) if formats is not None else [3] * n
+    nbytes = [h * w * (_PIX_BYTES[f] if u8 else 12) for (h, w), f in zip(shapes, formats)]
+    return kind, formats, shapes, list(sources), nbytes
+
+
+def _run_sweep(engine, sweep, srcs, formats, kind, ow, oh, out_format, crop, stats):
+    """Runs every strip of `sweep` on srcs (_sweep_sources' sources, alive for the whole call), then its finish_dev;
+    returns (rect or None, pixels) and frees the sweep."""
+    ptrs = [q.ctypes.data if isinstance(q, np.ndarray) else q for q in srcs]
     code = PIX_FORMATS[out_format]
     bpp = 4 if code == PIX_RGBA else 3
-    sweep = engine.blend_sweep(shapes, items, geom, strip_rows, keep_bytes, bands, params, crop, nbytes)
     d_out = engine.dev_alloc(max(ow * oh * bpp, 256))
     try:
         while True:
@@ -444,6 +439,44 @@ def mosaic_rgb8_sweep(engine: Engine, items, geom, bands, sources, strip_rows, k
         sweep.close()
         engine.dev_free(d_out)
     return (rect if crop else None), (px.reshape(3, ch, cw) if code == PIX_RGB_PLANAR else px.reshape(ch, cw, bpp))
+
+
+def mosaic_rgb8_sweep(engine: Engine, items, geom, bands, sources, strip_rows, keep_bytes, out_format="rgb", crop=True,
+                      params=None, kind=None, formats=None, shapes=None, fmt=None, stats=None):
+    """mosaic_rgb8_strips' bytes from one blend sweep (Engine.blend_sweep): the strips run top to bottom and each
+    source is handed over once while a later strip still reads it, keeping at most keep_bytes of sources between
+    strips (capi.SIZE_MAX: no limit; 0 hands over every source each strip reads).
+
+    sources: numpy arrays (host, pageable: uint8 read in layout `fmt`, one value or one per image, or float32
+    H×W×3), or pointers of source kind `kind` with PANO_PIX_* codes `formats` (one per image; None: 3) and `shapes`
+    [(h, w)].  Device memory holds one strip's blend state and f32 rows, two sources in the upload ring, the kept
+    sources, and 3 + 3 (4 for "rgba") bytes per canvas pixel.  stats: a dict that receives
+    "uploads", "upload_bytes" and "retained_high" (pano_blend_sweep_stats).  Returns (rect or None, pixels) as
+    mosaic_rgb8_strips does."""
+    n = len(items)
+    kind, formats, shapes, srcs, nbytes = _sweep_sources(sources, n, kind, formats, shapes, fmt)
+    ow, oh = max(it[2] for it in items), max(it[3] for it in items)
+    sweep = engine.blend_sweep(shapes, items, geom, strip_rows, keep_bytes, bands, params, crop, nbytes)
+    return _run_sweep(engine, sweep, srcs, formats, kind, ow, oh, out_format, crop, stats)
+
+
+def cylinder_mosaic_rgb8_sweep(engine: Engine, items, geom, h_factor, corr_inv, bands, sources, strip_rows, keep_bytes,
+                               out_format="rgb", crop=True, params=None, kind=None, formats=None, shapes=None, fmt=None,
+                               stats=None):
+    """Cylinder mode's output, write_rgb(crop(CylinderStitcher::build())), from one cylinder sweep
+    (Engine.blend_sweep_cyl): each strip of the corrected canvas blends the band of mosaic rows its perspective
+    correction reads, straight from the UNWARPED sources, and corrects its rows from it; no f32 mosaic of the whole
+    canvas is made.  items / geom: the warped images' (as for Engine.blend_stream_cyl); corr_inv:
+    perspective_correction's inv (3×3).  sources, kind, formats, shapes (the unwarped sources'), fmt, keep_bytes,
+    out_format, crop and stats as for mosaic_rgb8_sweep.  Device memory holds the tallest band's blend state and
+    f32 rows, one strip's f32 rows, two sources in the upload ring, the kept sources, the warps' column tables and
+    3 + 3 (4 for "rgba") bytes per canvas pixel.  Returns (rect or None, pixels) as mosaic_rgb8_sweep does."""
+    n = len(items)
+    kind, formats, shapes, srcs, nbytes = _sweep_sources(sources, n, kind, formats, shapes, fmt)
+    ow, oh = max(it[2] for it in items), max(it[3] for it in items)
+    sweep = engine.blend_sweep_cyl(shapes, items, geom, h_factor, corr_inv, strip_rows, keep_bytes, bands, params,
+                                   crop, nbytes)
+    return _run_sweep(engine, sweep, srcs, formats, kind, ow, oh, out_format, crop, stats)
 
 
 class StitchLanes:
